@@ -21,6 +21,9 @@
  *   ox_s = frac(f32(s) * 0.7548776662f), oy_s = frac(f32(s) * 0.5698402909f)   [ox_0 = oy_0 = 0]
  * colours are summed in sample order in f32, multiplied by 1/spp, then quantised as ray.fut:158-162.
  * At spp = 1 this is bit-identical to the reference's render.
+ *
+ * Ray queries ("ray queries" below): rays the caller made are traced against a prepared scene to their closest hit
+ * (objs_hit) or along their path (ray_colour), bit for bit, by the same warp-queue kernel in ray mode.
  */
 #ifndef RAY_B200_EXT_H
 #define RAY_B200_EXT_H
@@ -118,6 +121,37 @@ int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, flo
 /* Like futhark_entry_render but with explicit spp (library-owned result). */
 int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d **out0, int64_t h, int64_t w,
                               int32_t spp, const struct futhark_opaque_prepared_scene *p);
+
+/* ---- ray queries: caller-supplied rays against a prepared scene ----------------------------------------
+ * The two queries of the reference, for any ray: the closest hit of objs_hit (ray.fut:76-86) and the colour of
+ * ray_colour (ray.fut:126-148), bit for bit, on the warp-queue kernel in ray mode (whatever RAY_KERNEL / the context's
+ * kernel says; a shard setting is ignored: rays are not tiles).  On a RAY_GPUS > 1 context they run on device d, which
+ * holds the scene.  rays_dev: device float[n][6] = origin.xyz, dir.xyz (dir need not be normalised; zero components and
+ * an all-zero direction are fine; rays with non-finite components are outside the contract).  Asynchronous on the
+ * context's stream; ray_b200_context_last_render_ms and ray_b200_context_launch_count count them like renders, and a
+ * prepared scene may be freed or re-uploaded while a query that reads it is in flight.
+ * Errors (nonzero return, futhark_context_get_error; the context stays usable): n < 0 or n > 2^30, a NULL required
+ * pointer with n > 0, an invalid prepared scene, t_min < 0, a non-finite t_min or t_max, max_depth outside [0, 65535].
+ * n == 0 does nothing.  t_max <= t_min is legal: every ray misses. */
+/* Closest hit of ray i = objs_hit objs r t_min t_max (ray.fut:76-86), bit for bit. */
+struct ray_b200_hit {
+  float t;          /* -1 when there is no hit (a hit always has t > t_min >= 0) */
+  int32_t sphere;   /* index into the scene's sphere array as given (scene_from_arrays / scene_get_arrays order), -1 = none */
+  float p[3];       /* point_at_param r t (ray.fut:14-15); 0 when there is no hit */
+  float normal[3];  /* scale (1/radius) (p - centre) (ray.fut:42-43); 0 when there is no hit */
+};                  /* 32 bytes */
+/* Boxes are tested against (t_min, t_max), spheres with epsilon 0.1 whatever t_min is (ray.fut:77-79), the winner is
+ * re-intersected with (t_min, t_best + 1) (ray.fut:85; a failed re-intersection is no hit), and on equal t the lowest
+ * Morton-sorted leaf wins.  hits_dev: device struct ray_b200_hit[n]. */
+int ray_b200_trace_hits(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                        const float *rays_dev, int64_t n, float t_min, float t_max, struct ray_b200_hit *hits_dev);
+/* Colour of ray i = ray_colour objs r max_depth (ray.fut:126-148), bit for bit, before quantisation; every segment
+ * uses (0, 1e9) as ray_colour does.  rgb_dev: device float[n][3]; segments_dev: device int32[n] = objs_hit calls of
+ * the path (or NULL).  Camera rays of a frame through this call, quantised, equal the frame. */
+int ray_b200_trace_paths(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                         const float *rays_dev, int64_t n, int32_t max_depth, float *rgb_dev, int32_t *segments_dev);
+/* sizeof(struct ray_b200_hit) as the library was compiled (32). */
+int64_t ray_b200_hit_size(void);
 
 /* ---- multi-GPU tile sharding (one process per GPU; the gather itself is NCCL, done by the host) -- */
 /* Number of 8x4 tiles rank `rank` of `world` owns for an h x w image, and the padded per-rank count

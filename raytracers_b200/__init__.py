@@ -20,8 +20,8 @@ import os
 
 import numpy as np
 
-__all__ = ["Context", "RayError", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
-           "host_camera", "host_lbvh", "host_sample_offsets"]
+__all__ = ["Context", "RayError", "Hit", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
+           "host_camera", "host_lbvh", "host_sample_offsets", "camera_rays"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 KERNELS = {"auto": 0, "mega": 1, "persistent": 2, "wavefront": 3, "warpqueue": 4, "streamqueue": 5, "lanewalk": 6}
@@ -60,6 +60,11 @@ class RenderJob(C.Structure):
     _fields_ = [("prepared", C.c_void_p), ("h", C.c_int64), ("w", C.c_int64), ("spp", C.c_int32), ("shard_layout", C.c_int32),
                 ("out_dev", C.c_void_p), ("out_rgb_dev", C.c_void_p), ("wait_flag", C.c_void_p), ("wait_value", C.c_uint32),
                 ("reserved0", C.c_uint32), ("done_flag", C.c_void_p)]
+
+
+class Hit(C.Structure):
+    """struct ray_b200_hit (include/ray_b200.h): the closest hit of one ray, 32 bytes."""
+    _fields_ = [("t", C.c_float), ("sphere", C.c_int32), ("p", C.c_float * 3), ("normal", C.c_float * 3)]
 
 
 _libs = {}
@@ -139,6 +144,9 @@ def load_library(variant=""):
         "ray_b200_shard_tiles_padded": (i64, [i64, i64, i32]),
         "ray_b200_render_shard_into": (C.c_int, [vp, vp, i64, i64, i32, vp]),
         "ray_b200_detile": (C.c_int, [vp, vp, vp, i64, i64, i32]),
+        "ray_b200_trace_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
+        "ray_b200_trace_paths": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_hit_size": (i64, []),
         "ray_b200_count_work": (C.c_int, [vp, i64, i64, i32, vp, C.POINTER(WorkCounters)]),
         "ray_b200_ipc_alloc": (C.c_int, [vp, i64, pp, vp]),
         "ray_b200_ipc_free": (C.c_int, [vp, vp]),
@@ -231,6 +239,29 @@ def host_sample_offsets(spp):
     t = np.empty((spp, 2), np.float32)
     load_library().ray_b200_host_sample_offsets(int(spp), _ptr(t))
     return t
+
+
+def camera_rays(camera, h, w, spp=1):
+    """Camera rays of an h x w frame as render traces them: float32[h][w][spp][6] (origin, direction) of sample s of
+    pixel (row j, column i), with the same float32 operations in the same order as the render kernels (ray.fut:109-114,
+    150-154 and the spp extension of ray_b200.h).  camera: the 12 floats of PreparedScene.info()["camera"].  Through
+    Context.trace_paths, quantised, these rays give the frame itself."""
+    c = np.asarray(camera, np.float32).reshape(12)
+    f = np.float32
+    i = np.arange(w, dtype=np.float32)[None, :, None]
+    hj = (f(h) - np.arange(h, dtype=np.float32))[:, None, None]   # f32(H - j): exact for any frame size render accepts
+    if spp == 1:
+        u = np.broadcast_to(i / f(w), (h, w, 1))
+        v = np.broadcast_to(hj / f(h), (h, w, 1))
+    else:
+        off = host_sample_offsets(spp)
+        u = np.broadcast_to((i + off[:, 0][None, None, :]) / f(w), (h, w, spp))
+        v = np.broadcast_to((hj + off[:, 1][None, None, :]) / f(h), (h, w, spp))
+    out = np.empty((h, w, spp, 6), np.float32)
+    out[..., 0:3] = c[0:3]
+    for a in range(3):   # llc + u*horizontal + v*vertical - origin, per component, left to right
+        out[..., 3 + a] = ((c[3 + a] + u * c[6 + a]) + v * c[9 + a]) - c[a]
+    return out
 
 
 class _Handle:
@@ -577,6 +608,51 @@ class Context:
 
     def detile(self, gathered_dev, out_pix_dev, h, w, world):
         self._check(self.lib.ray_b200_detile(self.handle, _ptr(gathered_dev), _ptr(out_pix_dev), int(h), int(w), int(world)))
+
+    # -- ray queries (include/ray_b200.h): caller-supplied rays against a prepared scene --------------------------
+    def trace_hits_into(self, rays_dev, n, prepared, hits_dev, t_min=0.0, t_max=1e9):
+        """Closest hit (objs_hit, ray.fut:76-86) of n rays: rays_dev = device float[n][6] (origin, direction), hits_dev =
+        device Hit[n].  Asynchronous on the context's stream, like render_into."""
+        self._check(self.lib.ray_b200_trace_hits(self.handle, prepared.handle, _ptr(rays_dev), int(n), float(t_min), float(t_max),
+                                                 _ptr(hits_dev)))
+
+    def trace_paths_into(self, rays_dev, n, prepared, rgb_dev, segments_dev=None, max_depth=50):
+        """Colour (ray_colour, ray.fut:126-148) of n rays into device float[n][3], and optionally the objs_hit calls of
+        every path into device int32[n].  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_trace_paths(self.handle, prepared.handle, _ptr(rays_dev), int(n), int(max_depth),
+                                                  _ptr(rgb_dev), _ptr(segments_dev)))
+
+    def _rays_tensor(self, rays):
+        import torch
+        if not isinstance(rays, torch.Tensor) or rays.device.type != "cuda" or rays.device.index != self.device:
+            raise ValueError(f"rays must be a CUDA tensor on cuda:{self.device}")
+        if rays.dtype != torch.float32 or rays.dim() != 2 or rays.shape[1] != 6 or not rays.is_contiguous():
+            raise ValueError(f"rays must be a contiguous float32 tensor of shape [n, 6], got {rays.dtype} {tuple(rays.shape)}")
+        # the rays may still be in flight on torch's stream, which the context's own stream is not ordered after
+        torch.cuda.current_stream(rays.device).synchronize()
+        return torch
+
+    def trace_hits(self, prepared, rays, t_min=0.0, t_max=1e9):
+        """Closest hits of a [n, 6] float32 CUDA tensor of rays.  Returns dict(t [n], sphere [n] int32, p [n, 3],
+        normal [n, 3]): views of one [n, 8] buffer of Hit records.  t = -1 and sphere = -1 where a ray hits nothing.
+        Waits for torch's current stream before, and synchronises the context after the query."""
+        torch = self._rays_tensor(rays)
+        n = rays.shape[0]
+        buf = torch.empty((n, 8), dtype=torch.float32, device=rays.device)
+        self.trace_hits_into(rays.data_ptr(), n, prepared, buf.data_ptr(), t_min=t_min, t_max=t_max)
+        self.sync()
+        return {"t": buf[:, 0], "sphere": buf[:, 1].view(torch.int32), "p": buf[:, 2:5], "normal": buf[:, 5:8]}
+
+    def trace_paths(self, prepared, rays, max_depth=50):
+        """Colours of a [n, 6] float32 CUDA tensor of rays: (rgb [n, 3] float32, segments [n] int32 = objs_hit calls of
+        every path).  Waits for torch's current stream before, and synchronises the context after the query."""
+        torch = self._rays_tensor(rays)
+        n = rays.shape[0]
+        rgb = torch.empty((n, 3), dtype=torch.float32, device=rays.device)
+        seg = torch.empty((n,), dtype=torch.int32, device=rays.device)
+        self.trace_paths_into(rays.data_ptr(), n, prepared, rgb.data_ptr(), seg.data_ptr(), max_depth=max_depth)
+        self.sync()
+        return rgb, seg
 
     def count_work(self, h, w, prepared, spp=1):
         wc = WorkCounters()

@@ -90,7 +90,7 @@ struct futhark_context {
     TileOrderBuffers tile_order_plan{};
   } lanes[2];
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool plan_auto_k2 = false, suppress_auto_k2 = false;   // fill_params: the K = 2 plan was chosen automatically / must not be
+  bool plan_auto_k2 = false;            // fill_params: the K = 2 plan was chosen automatically
   bool pipeline = false;                // ray_b200_context_set_pipeline: batches do not join lane 1 back
   uint32_t lane_seq = 0;                // pipelined submission: frames alternate lanes across calls
   cudaStream_t reclaim = nullptr;       // scene memory is freed here, ordered after its last use on either lane
@@ -170,6 +170,17 @@ inline int64_t tiles_of_rank(int64_t h, int64_t w, int32_t rank, int32_t world) 
 int resolve_kernel(const futhark_context *ctx);
 int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
                 int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P);
+// The warp-queue kernel's plan for one launch (pixel frames and ray queries): rays in flight per warp (32 k), warps per
+// CTA, node-queue cap, packet threshold and how much of the scene is staged in shared memory.
+struct WqPlan {
+  int32_t k = 1, warps = 1, packet = 0, ncap = 512;
+  bool auto_k2 = false;
+  int32_t smem_nodes = 0, smem_spheres = 0;
+};
+int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool will_spread, bool coherent, bool rays,
+                   const char *what, WqPlan &wp);
+int64_t cap_staging(const futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t budget);
+void split_staging(const futhark_opaque_prepared_scene *p, int64_t budget, int32_t &smem_nodes, int32_t &smem_spheres);
 void free_wavefront(futhark_context *ctx);
 // Peer-frame protocol of one frame (include/ray_b200.h): wait for *wait_flag >= wait_value before the kernel, bump
 // *done_flag when this rank's pixels have landed.

@@ -110,62 +110,23 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
     ctx->plan_wq_warps = (int32_t)wq_w;
   }
   if (kern == RAY_B200_KERNEL_WARPQUEUE) {
-    // one CTA per SM: as many warps as asked for (<= 32) while their queues leave >= 8 KB for staging;
-    // deep trees need bigger node stacks, so they get fewer warps
-    // Rays in flight per warp (32 K) and node-queue cap.  wq_k = 0 (default): K = 2 with a kAutoK2Ncap-entry node queue and
-    // as many warps (>= kAutoK2MinWarps) as still leave the WHOLE scene (tree + spheres) staged - a round of 64 rays has
-    // relatively fewer partial batches at its end than a round of 32 (spread samples keep 4 instead of 16 bytes of
-    // per-slot sample state, so 28 warps fit on rgbbox) - and K = 1 with 32 warps otherwise (a scene that is only partly
-    // staged loses more from the staging space the bigger slots take than it gains from fuller batches).
-    int k = ctx->cfg.wq_k == 2 ? 2 : 1;
-    int ncap_cfg = ctx->cfg.wq_ncap, warps_cfg = ctx->cfg.wq_warps;
-    bool auto_k2 = false;
     // samples will be spread if the finished-sample buffer fits the budget (do_render allocates it; a failed allocation
     // there falls back to pixel-bound samples, whose bigger slots are checked again at launch)
     const bool will_spread = spp > 1 && spp <= 65535 && ctx->cfg.wq_spread &&
                              (size_t)ctx->sm_count * kWqMaxWarps * kWqRing * (size_t)spp * sizeof(float4) <= kSpreadBudget;
-    if (ctx->cfg.wq_k == 0 && !ctx->suppress_auto_k2) {
-      const int64_t scene_bytes = 128 + (int64_t)(p->n - 1) * 64 + (int64_t)p->n * 16;
-      const int64_t pw2 = (int64_t)wq_warp_bytes(2, wq_node_capacity(2, p->max_depth, kAutoK2Ncap), false, will_spread);
-      int64_t w2 = ((int64_t)ctx->max_smem_optin - scene_bytes - 512 - 128) / pw2;   // as many warps as still leave the scene whole
-      if (w2 > kWqMaxWarps) w2 = kWqMaxWarps;
-      w2 &= ~(int64_t)3;             // the same number of warps on each of the SM's four schedulers
-      if (w2 >= kAutoK2MinWarps) {   // 28 warps with spread samples (80-byte slots), 24 with pixel-bound ones, on rgbbox
-        k = 2;
-        auto_k2 = true;
-        if (warps_cfg < 1) warps_cfg = (int)w2;
-        if (ctx->cfg.wq_ncap == 512) ncap_cfg = kAutoK2Ncap;   // (512 = the configured default: not set by the caller)
-      }
-    }
-    // Packet steps pay off when item-mode node fetches are expensive (part of the tree not staged in shared memory)
-    // AND the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame.
-    // The plan is made twice: first assuming packets, to see whether the tree would be fully staged anyway.
-    // (the K = 2 plan is only made for scenes that are staged whole, where packets never pay: without this the first
-    // attempt below would reserve the packet stacks, find the scene no longer fits next to them and switch packets ON)
-    int want_packet = (auto_k2 && ctx->cfg.wq_packet < 0) ? 0 : ctx->cfg.wq_packet;
+    // the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame
     const bool coherent = spp > 1 || h * w >= ((int64_t)1 << 22);
-    int64_t per_warp = 0, wq_w = 0;
-    for (int attempt = 0; attempt < 2; attempt++) {
-      const bool pk = want_packet != 0;
-      per_warp = (int64_t)wq_warp_bytes(k, wq_node_capacity(k, p->max_depth, ncap_cfg), pk, will_spread);
-      // 32 warps hide latency best, also for the 1 M-sphere tree (64 MB of nodes) once its staging area is capped so
-      // that the SM keeps 32 KB of L1 (below)
-      const int auto_warps = 32;
-      wq_w = warps_cfg < 1 ? auto_warps : (warps_cfg > kWqMaxWarps ? kWqMaxWarps : warps_cfg);
-      while (wq_w > 1 && wq_w * per_warp + 8192 > (int64_t)ctx->max_smem_optin) wq_w--;
-      if (want_packet >= 0) break;
-      const int64_t b = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512 - 128;
-      const bool fully_staged = b / 64 >= (int64_t)(p->n - 1);
-      want_packet = (!fully_staged && coherent) ? 24 : 0;
-      if (want_packet != 0) break;  // the first plan (with packets) stands
-    }
-    budget = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512;
-    if (budget < 256) { set_error(ctx, "render: warp-queue kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
-    ctx->plan_wq_packet = want_packet > 32 ? 32 : want_packet;
-    ctx->plan_wq_warps = (int32_t)wq_w;
-    ctx->plan_wq_k = k;
-    ctx->plan_wq_ncap = ncap_cfg;
-    ctx->plan_auto_k2 = auto_k2;
+    WqPlan wp;
+    if (plan_warpqueue(ctx, p, will_spread, coherent, false, "render", wp)) return 1;
+    ctx->plan_wq_packet = wp.packet;
+    ctx->plan_wq_warps = wp.warps;
+    ctx->plan_wq_k = wp.k;
+    ctx->plan_wq_ncap = wp.ncap;
+    ctx->plan_auto_k2 = wp.auto_k2;
+    ctx->plan_kernel = kern;
+    P.smem_nodes = wp.smem_nodes;
+    P.smem_spheres = wp.smem_spheres;
+    return 0;
   }
   if (kern == RAY_B200_KERNEL_LANEWALK) {
     // one CTA per SM: lw_warps warps (32 unless told otherwise) x lw_slots path slots each (48 unless told otherwise,
@@ -184,31 +145,94 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
     ctx->plan_wq_warps = (int32_t)w;
     ctx->plan_lw_slots = (int32_t)r;
     ctx->plan_wq_packet = 0;
+    budget = cap_staging(ctx, p, budget);
   }
   ctx->plan_kernel = kern;
-  if (kern == RAY_B200_KERNEL_WARPQUEUE || kern == RAY_B200_KERNEL_LANEWALK) {
-    // Shared memory not used by the kernel stays L1: a tree far larger than the caches gains more from 60-100 KB of L1
-    // for its hot middle levels than from a few hundred more staged top nodes
-    const bool huge = (int64_t)(p->n - 1) * 64 > ((int64_t)8 << 20);
-    // the carve-out granule below the maximum is 196 KB (sm_90: 228 KB of shared memory + L1 per SM): staying under it
-    // leaves the SM 32 KB of L1 instead of ~0
-    const int64_t queues = (int64_t)ctx->max_smem_optin - 512 - budget;
-    // (the driver reserves 1 KB of shared memory per CTA on top of what the kernel asks for, hence the 2 KB margin)
-    const int64_t under_196k = std::max<int64_t>(1024, (int64_t)196 * 1024 - 2048 - queues);
-    const int64_t cap = ctx->cfg.stage_cap >= 0 ? ctx->cfg.stage_cap : (huge ? under_196k : budget);
-    budget = std::min<int64_t>(budget, std::max<int64_t>(cap, 256));
-  }
-  int64_t nodes_fit = std::max<int64_t>(0, budget / 64);
-  P.smem_nodes = (int32_t)std::min<int64_t>(P.n_inner, nodes_fit);
-  const int64_t left = budget - (int64_t)P.smem_nodes * 64;
-  P.smem_spheres = (P.smem_nodes == P.n_inner && left >= (int64_t)P.n_leaves * 16) ? P.n_leaves : 0;
-  if (kern == RAY_B200_KERNEL_WARPQUEUE && ctx->plan_auto_k2 && !(P.smem_nodes == P.n_inner && P.smem_spheres == P.n_leaves)) {
+  split_staging(p, budget, P.smem_nodes, P.smem_spheres);
+  return 0;
+}
+
+// Shared memory not used by the warp-queue / lane-walk kernels stays L1: a tree far larger than the caches gains more from
+// 60-100 KB of L1 for its hot middle levels than from a few hundred more staged top nodes.  Returns the staging budget.
+int64_t cap_staging(const futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t budget) {
+  const bool huge = (int64_t)(p->n - 1) * 64 > ((int64_t)8 << 20);
+  // the carve-out granule below the maximum is 196 KB (sm_90: 228 KB of shared memory + L1 per SM): staying under it
+  // leaves the SM 32 KB of L1 instead of ~0
+  const int64_t queues = (int64_t)ctx->max_smem_optin - 512 - budget;
+  // (the driver reserves 1 KB of shared memory per CTA on top of what the kernel asks for, hence the 2 KB margin)
+  const int64_t under_196k = std::max<int64_t>(1024, (int64_t)196 * 1024 - 2048 - queues);
+  const int64_t cap = ctx->cfg.stage_cap >= 0 ? ctx->cfg.stage_cap : (huge ? under_196k : budget);
+  return std::min<int64_t>(budget, std::max<int64_t>(cap, 256));
+}
+
+// Staging area of `budget` bytes: BFS prefix of the node array, then the sphere records if they all fit.
+void split_staging(const futhark_opaque_prepared_scene *p, int64_t budget, int32_t &smem_nodes, int32_t &smem_spheres) {
+  const int32_t n_inner = (int32_t)(p->n - 1), n_leaves = (int32_t)p->n;
+  const int64_t nodes_fit = std::max<int64_t>(0, budget / 64);
+  smem_nodes = (int32_t)std::min<int64_t>(n_inner, nodes_fit);
+  const int64_t left = budget - (int64_t)smem_nodes * 64;
+  smem_spheres = (smem_nodes == n_inner && left >= (int64_t)n_leaves * 16) ? n_leaves : 0;
+}
+
+// The warp-queue kernel's plan for a prepared scene (pixel frames and ray queries): one CTA per SM, as many warps as asked
+// for (<= 32) while their queues leave >= 8 KB for staging; deep trees need bigger node stacks, so they get fewer warps.
+// `coherent`: the rays a warp holds are coherent enough for the packet walk; `rays`: no packet walk at all.
+int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool will_spread, bool coherent, bool rays,
+                   const char *what, WqPlan &wp) {
+  for (int pass = 0; pass < 2; pass++) {
+    // Rays in flight per warp (32 K) and node-queue cap.  wq_k = 0 (default): K = 2 with a kAutoK2Ncap-entry node queue and
+    // as many warps (>= kAutoK2MinWarps) as still leave the WHOLE scene (tree + spheres) staged - a round of 64 rays has
+    // relatively fewer partial batches at its end than a round of 32 (spread samples keep 4 instead of 16 bytes of
+    // per-slot sample state, so 28 warps fit on rgbbox) - and K = 1 with 32 warps otherwise (a scene that is only partly
+    // staged loses more from the staging space the bigger slots take than it gains from fuller batches).
+    int k = ctx->cfg.wq_k == 2 ? 2 : 1;
+    int ncap_cfg = ctx->cfg.wq_ncap, warps_cfg = ctx->cfg.wq_warps;
+    bool auto_k2 = false;
+    if (ctx->cfg.wq_k == 0 && pass == 0) {
+      const int64_t scene_bytes = 128 + (int64_t)(p->n - 1) * 64 + (int64_t)p->n * 16;
+      const int64_t pw2 = (int64_t)wq_warp_bytes(2, wq_node_capacity(2, p->max_depth, kAutoK2Ncap), false, will_spread);
+      int64_t w2 = ((int64_t)ctx->max_smem_optin - scene_bytes - 512 - 128) / pw2;   // as many warps as still leave the scene whole
+      if (w2 > kWqMaxWarps) w2 = kWqMaxWarps;
+      w2 &= ~(int64_t)3;             // the same number of warps on each of the SM's four schedulers
+      if (w2 >= kAutoK2MinWarps) {   // 28 warps with spread samples (80-byte slots), 24 with pixel-bound ones, on rgbbox
+        k = 2;
+        auto_k2 = true;
+        if (warps_cfg < 1) warps_cfg = (int)w2;
+        if (ctx->cfg.wq_ncap == 512) ncap_cfg = kAutoK2Ncap;   // (512 = the configured default: not set by the caller)
+      }
+    }
+    // Packet steps pay off when item-mode node fetches are expensive (part of the tree not staged in shared memory)
+    // AND the rays a warp holds are coherent.  The plan is made twice: first assuming packets, to see whether the tree
+    // would be fully staged anyway.
+    // (the K = 2 plan is only made for scenes that are staged whole, where packets never pay: without this the first
+    // attempt below would reserve the packet stacks, find the scene no longer fits next to them and switch packets ON)
+    int want_packet = rays ? 0 : ((auto_k2 && ctx->cfg.wq_packet < 0) ? 0 : ctx->cfg.wq_packet);
+    int64_t per_warp = 0, wq_w = 0;
+    for (int attempt = 0; attempt < 2; attempt++) {
+      const bool pk = want_packet != 0;
+      per_warp = (int64_t)wq_warp_bytes(k, wq_node_capacity(k, p->max_depth, ncap_cfg), pk, will_spread);
+      // 32 warps hide latency best, also for the 1 M-sphere tree (64 MB of nodes) once its staging area is capped so
+      // that the SM keeps 32 KB of L1 (cap_staging)
+      const int auto_warps = 32;
+      wq_w = warps_cfg < 1 ? auto_warps : (warps_cfg > kWqMaxWarps ? kWqMaxWarps : warps_cfg);
+      while (wq_w > 1 && wq_w * per_warp + 8192 > (int64_t)ctx->max_smem_optin) wq_w--;
+      if (want_packet >= 0) break;
+      const int64_t b = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512 - 128;
+      const bool fully_staged = b / 64 >= (int64_t)(p->n - 1);
+      want_packet = (!fully_staged && coherent) ? 24 : 0;
+      if (want_packet != 0) break;  // the first plan (with packets) stands
+    }
+    int64_t budget = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512;
+    if (budget < 256) { set_error(ctx, "%s: warp-queue kernel does not fit shared memory (tree depth %d)", what, p->max_depth); return 1; }
+    wp.packet = want_packet > 32 ? 32 : want_packet;
+    wp.warps = (int32_t)wq_w;
+    wp.k = k;
+    wp.ncap = ncap_cfg;
+    wp.auto_k2 = auto_k2;
+    split_staging(p, cap_staging(ctx, p, budget), wp.smem_nodes, wp.smem_spheres);
     // belt and braces: the K = 2 plan is only worth anything when the scene is staged whole (a scene that just misses
     // fetches its lower nodes from L2 with half the warps); if anything above left it short, plan again with K = 1
-    ctx->suppress_auto_k2 = true;
-    const int rc = fill_params(ctx, p, h, w, spp, rank, world, out_pix, out_rgb, tile_major, P);
-    ctx->suppress_auto_k2 = false;
-    return rc;
+    if (!auto_k2 || (wp.smem_nodes == (int32_t)(p->n - 1) && wp.smem_spheres == (int32_t)p->n)) break;
   }
   return 0;
 }

@@ -37,18 +37,20 @@ __device__ __forceinline__ RayInv ray_invariants(const Ray &r) {
   return q;
 }
 
-// aabb_hit box r 0.0 1e9 (ray.fut:53-70, called at ray.fut:77 with the ORIGINAL t range).
+// aabb_hit box r t0 t1 (ray.fut:53-70, called at ray.fut:77 with the ORIGINAL t range: (0, 1e9) from
+// ray_colour, or the interval of a ray query).
 // The reference early-outs after each axis; tmin is non-decreasing, tmax non-increasing and neither
-// can be NaN (fmaxf/fminf drop a NaN operand and the seeds 0 / 1e9 are finite), so the final test
+// can be NaN (fmaxf/fminf drop a NaN operand and the seeds t0 / t1 are finite), so the final test
 // alone gives the same boolean.
 __device__ __forceinline__ bool box_hit(float bminx, float bminy, float bminz, float bmaxx, float bmaxy,
-                                        float bmaxz, const Ray &r, const RayInv &q) {
+                                        float bmaxz, const Ray &r, const RayInv &q, const float t0 = 0.0f,
+                                        const float t1 = 1000000000.0f) {
   const float x0 = (bminx - r.o.x) * q.ix, x1 = (bmaxx - r.o.x) * q.ix;
   const float y0 = (bminy - r.o.y) * q.iy, y1 = (bmaxy - r.o.y) * q.iy;
   const float z0 = (bminz - r.o.z) * q.iz, z1 = (bmaxz - r.o.z) * q.iz;
   const bool sx = q.ix < 0.0f, sy = q.iy < 0.0f, sz = q.iz < 0.0f;
-  float tmin = fmaxf(sx ? x1 : x0, 0.0f);
-  float tmax = fminf(sx ? x0 : x1, 1000000000.0f);
+  float tmin = fmaxf(sx ? x1 : x0, t0);
+  float tmax = fminf(sx ? x0 : x1, t1);
   tmin = fmaxf(sy ? y1 : y0, tmin);
   tmax = fminf(sy ? y0 : y1, tmax);
   tmin = fmaxf(sz ? z1 : z0, tmin);

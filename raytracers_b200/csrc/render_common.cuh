@@ -125,10 +125,12 @@ __device__ __forceinline__ void find_closest(const Scene &sc, const float *root_
 // ------------------------------------------------------------------ one ray_colour iteration (ray.fut:130-148)
 // The part of a ray_colour iteration after the closest-hit search: given the fold result (j, tb),
 // re-intersect, scatter or shade the sky.  `a` = dot r.d r.d.  Returns true if the path continues
-// (r/light/depth updated), false if it ended with `colour` set.
+// (r/light/depth updated), false if it ended with `colour` set.  `max_depth`: ray_colour's depth limit (ray.fut:154
+// passes 50; a path query passes its own).
 template <class Scene>
 __device__ __forceinline__ bool shade_segment(const Scene &sc, const RenderParams &P, Ray &r, const float a, const int j,
-                                              const float tb, V3 &light, int &depth, V3 &colour) {
+                                              const float tb, V3 &light, int &depth, V3 &colour,
+                                              const int max_depth = kMaxDepth) {
   if (j >= 0) {
     // objs_hit, second half (ray.fut:83-85): re-intersect the winner with t_min = 0, t_max = t_best + 1
     const float4 g = sc.sphere(j);
@@ -146,7 +148,7 @@ __device__ __forceinline__ bool shade_segment(const Scene &sc, const RenderParam
         r.d = refl;
         light = vmul(light, v3(col.x, col.y, col.z));               // ray.fut:135
         depth = depth + 1;
-        if (depth < kMaxDepth) return true;
+        if (depth < max_depth) return true;
         colour = v3(0.0f, 0.0f, 0.0f);                              // loop exit with colour = light*0 (ray.fut:136)
         return false;
       }

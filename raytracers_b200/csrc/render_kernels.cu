@@ -122,10 +122,18 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // grain is one sample instead of one pixel x spp (no long tails, scales to many GPUs), and every
 // finished sample's colour is parked in an L2-resident buffer so that the pixel is summed in SAMPLE
 // ORDER when its last sample lands, which keeps the result bit-identical to the sequential definition.
+//
+// Ray mode (kRays, include/ray_b200.h "ray queries"): the work items are the caller's rays instead of pixels.  A claim c
+// is ray c (no tile order), a slot is filled from Q.rays, boxes and spheres are tested against the query's (t_min, t_max)
+// instead of the literal (0, 1e9), the depth limit is Q.max_depth, and a finished path writes Q.rgb / Q.segments.  A hit
+// query (Q.hits != NULL, warp-uniform) is a path query of one segment whose owner lane writes the hit record instead of
+// shading.  Rays of a batch are not coherent: ray mode has no packet walk and no spread samples.  Q is unused otherwise.
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres>
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, bool kRays = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
-                                                                   const int packet_min, const int refill_min, const int nlow) {
+                                                                   const int packet_min, const int refill_min, const int nlow,
+                                                                   const __grid_constant__ RayQuery Q) {
+  static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without the packet walk");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -172,8 +180,10 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   uint32_t *lstk = reinterpret_cast<uint32_t *>(kPacket ? pk_mask + kWqPacketStack : reinterpret_cast<unsigned *>(pk_node));
   uint32_t *nstk = lstk + kWqLeafStack;
 
-  const int total = (int)(P.local_tiles * kTilePixels);
-  const int total_claims = P.n_chunks << 11;
+  const int total = kRays ? Q.n : (int)(P.local_tiles * kTilePixels);
+  const int total_claims = kRays ? Q.n : P.n_chunks << 11;
+  // the query's interval (ray mode) or the literal one of ray_colour (ray.fut:130)
+  const float t_lo = kRays ? Q.t_min : 0.0f, t_hi = kRays ? Q.t_max : 1000000000.0f;
   const int spp = P.spp;
 #pragma unroll
   for (int k = 0; k < K; k++) p_item[lane + 32 * k] = -1;
@@ -187,6 +197,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
 
   // A path in `slot` has ended with `colour`.
   auto finish_path = [&](const int slot, const V3 colour, const int segs) {
+    if constexpr (kRays) {
+      // a path ended by the depth limit has segs = max_depth + 1 here, but made max_depth objs_hit calls (ray.fut:129)
+      const int item = p_item[slot];
+      float *c = Q.rgb + 3 * (size_t)item;
+      c[0] = colour.x; c[1] = colour.y; c[2] = colour.z;
+      if (Q.segments) Q.segments[item] = segs < Q.max_depth ? segs : Q.max_depth;
+      p_item[slot] = -1;
+      return;
+    }
     // learned claim order (recording frame only): the longest path of the tile, sample 0 of its 32 pixels is evidence enough
     if (P.tile_cost && ((kSpread ? p_ms[slot] : __float_as_int(p_sum[slot].w)) & 0xffff) == 0)
       atomicMax(P.tile_cost + (p_item[slot] >> 5), (unsigned)segs);
@@ -214,6 +233,14 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         p_item[slot] = -1;
       }
     }
+  };
+  // hit query: struct ray_b200_hit of the slot's ray (t = -1, sphere = -1, p = normal = 0 when there is no hit)
+  [[maybe_unused]] auto finish_hit = [&](const int slot, const float t, const int sphere, const V3 p, const V3 n) {
+    float *h = Q.hits + 8 * (size_t)p_item[slot];
+    h[0] = t; h[1] = __int_as_float(sphere);
+    h[2] = p.x; h[3] = p.y; h[4] = p.z;
+    h[5] = n.x; h[6] = n.y; h[7] = n.z;
+    p_item[slot] = -1;
   };
   // spread: pixels whose last sample has landed are summed IN SAMPLE ORDER and written; frees the ring entry
   auto finalize_pixels = [&]() {
@@ -272,9 +299,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             const int slot = lane + 32 * k;
             if (p_item[slot] < 0) {
               const int c = base + rank++;
-              const int item = c < total_claims ? claim_to_item(P, c) : total;
+              const int item = c < total_claims ? (kRays ? c : claim_to_item(P, c)) : total;
               int pi, pj;
-              if (item < total) {
+              if (kRays && item < total) {
+                const float *rp = Q.rays + 6 * (size_t)item;
+                p_item[slot] = item;
+                ray_o[slot] = make_float4(rp[0], rp[1], rp[2], 0.0f);
+                ray_d[slot] = make_float4(rp[3], rp[4], rp[5], 0.0f);
+                p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
+              } else if (item < total) {
                 if (item_pixel(P, item, pi, pj)) {
                   const Ray r = primary_ray(P, pi, pj, 0);
                   p_item[slot] = item;
@@ -350,12 +383,16 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             r.o = v3(ro.x, ro.y, ro.z);
             r.d = v3(rd.x, rd.y, rd.z);
             const RayInv q = ray_invariants(r);
-            if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q)) {
+            if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, t_lo, t_hi)) {
               ray_o[slot] = make_float4(ro.x, ro.y, ro.z, q.a);
               ray_i[slot] = make_float4(q.ix, q.iy, q.iz, 0.0f);
               best_t[slot] = kItemNoHit;
               go = true;
               break;
+            }
+            if (kRays && Q.hits) {
+              finish_hit(slot, -1.0f, -1, v3(0.0f, 0.0f, 0.0f), v3(0.0f, 0.0f, 0.0f));
+              continue;
             }
             const float4 pl = p_light[slot];  // miss (ray.fut:141-148)
             V3 light = v3(pl.x, pl.y, pl.z), colour;
@@ -408,7 +445,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         Ray r;
         r.o = v3(ro.x, ro.y, ro.z);
         r.d = v3(rd.x, rd.y, rd.z);
-        const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, 0.1f, 1000000000.0f);
+        const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, 0.1f, t_hi);  // epsilon 0.1 whatever t_min is (ray.fut:79)
         hit = t >= 0.0f;
         tb = __float_as_uint(t);
       }
@@ -437,8 +474,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         q.ix = ri.x; q.iy = ri.y; q.iz = ri.z; q.a = ro.w;
         lptr = __float_as_int(q0.w);
         rptr = __float_as_int(q1.w);
-        const bool hl = box_hit(q0.x, q0.y, q0.z, q1.x, q1.y, q1.z, r, q);
-        const bool hr = box_hit(q2.x, q2.y, q2.z, q3.x, q3.y, q3.z, r, q);
+        const bool hl = box_hit(q0.x, q0.y, q0.z, q1.x, q1.y, q1.z, r, q, t_lo, t_hi);
+        const bool hr = box_hit(q2.x, q2.y, q2.z, q3.x, q3.y, q3.z, r, q, t_lo, t_hi);
         pl_leaf = lptr < 0;          // a leaf child has no box in the reference: always visited
         pr_leaf = rptr < 0;
         pl_node = hl && !pl_leaf;
@@ -593,7 +630,23 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       int depth = __float_as_int(pl.w);
       const int j = bt == kItemNoHit ? -1 : (int)best_l[slot];
       const float tb = __uint_as_float(bt);
-      if (shade_segment(sc, P, r, ro.w, j, tb, light, depth, colour)) {
+      if (kRays && Q.hits) {
+        // objs_hit, second half (ray.fut:83-85) with the query's t_min; a failed re-intersection is no hit
+        float t = -1.0f;
+        V3 p = v3(0.0f, 0.0f, 0.0f), n = p;
+        if (j >= 0) {
+          const float4 g = sc.sphere(j);
+          t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, Q.t_min, tb + 1.0f);
+          if (t >= 0.0f) {
+            p = vadd(r.o, vscale(t, r.d));                            // point_at_param, ray.fut:14-15
+            n = vscale(1.0f / g.w, vsub(p, v3(g.x, g.y, g.z)));       // ray.fut:42-43
+          }
+        }
+        if (t >= 0.0f) finish_hit(slot, t, __ldg(Q.perm + j), p, n);
+        else finish_hit(slot, -1.0f, -1, p, n);
+        continue;
+      }
+      if (shade_segment(sc, P, r, ro.w, j, tb, light, depth, colour, kRays ? Q.max_depth : kMaxDepth)) {
         ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
         ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
         p_light[slot] = make_float4(light.x, light.y, light.z, __int_as_float(depth));
@@ -677,11 +730,12 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   const long long useful = (rays + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
   if (ctas > useful) ctas = useful;
   cudaError_t e = cudaSuccess;
+  const RayQuery no_rays{};
 #define RAYB200_WQ(KK, SP, PK, A, S)                                                                                        \
   do {                                                                                                                      \
     e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, SP, PK, A, S>>(lc.max_dynamic_smem);                                \
     if (e == cudaSuccess)                                                                                                   \
-      render_warpqueue_kernel<KK, SP, PK, A, S><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, lc.wq_packet, lc.wq_refill, nlow); \
+      render_warpqueue_kernel<KK, SP, PK, A, S><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, lc.wq_packet, lc.wq_refill, nlow, no_rays); \
   } while (0)
 #define RAYB200_WQ2(KK, SP, PK)                                                           \
   do {                                                                                    \
@@ -699,6 +753,41 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
 #undef RAYB200_WQ3
 #undef RAYB200_WQ2
 #undef RAYB200_WQ
+  if (e == cudaSuccess) (*launches)++;
+  return e;
+}
+
+// Ray queries: the same kernel in ray mode, one CTA per SM (fewer for small batches), planned like a pixel frame
+// without spread samples or packets.  The four variants per K are loaded on first use.
+cudaError_t launch_rays(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches) {
+  if (q.n <= 0) return cudaSuccess;
+  const bool all_nodes = p.smem_nodes == p.n_inner, sph = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
+  const int k = lc.wq_k == 1 ? 1 : 2;
+  const int wthreads = 32 * lc.wq_warps;
+  const int ncap = wq_node_capacity(k, p.max_depth, lc.wq_ncap);
+  const int nring = 1 << (31 - __builtin_clz((unsigned)ncap));
+  const int nlow = lc.wq_low < 0 ? 0 : (lc.wq_low == 0 ? nring / 2 : (lc.wq_low > nring - 96 ? nring - 96 : lc.wq_low));
+  const size_t wsmem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * wq_warp_bytes(k, ncap, false, false);
+  long long ctas = lc.sm_count;
+  const long long useful = ((long long)q.n + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
+  if (ctas > useful) ctas = useful;
+  cudaError_t e = cudaSuccess;
+#define RAYB200_WQR(KK, A, S)                                                                                              \
+  do {                                                                                                                     \
+    e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, false, false, A, S, true>>(lc.max_dynamic_smem);                   \
+    if (e == cudaSuccess)                                                                                                  \
+      render_warpqueue_kernel<KK, false, false, A, S, true><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, 0, 1, nlow, q); \
+  } while (0)
+#define RAYB200_WQR2(KK)                                                                                                   \
+  do {                                                                                                                     \
+    if (all_nodes && sph) RAYB200_WQR(KK, true, true);                                                                     \
+    else if (all_nodes) RAYB200_WQR(KK, true, false);                                                                      \
+    else if (sph) RAYB200_WQR(KK, false, true);                                                                            \
+    else RAYB200_WQR(KK, false, false);                                                                                    \
+  } while (0)
+  if (k == 1) RAYB200_WQR2(1); else RAYB200_WQR2(2);
+#undef RAYB200_WQR2
+#undef RAYB200_WQR
   if (e == cudaSuccess) (*launches)++;
   return e;
 }

@@ -58,6 +58,20 @@ struct RenderParams {
   unsigned long long *warp_trace;
 };
 
+// Ray queries (include/ray_b200.h "ray queries"): the warp-queue kernel's ray-mode instantiations trace caller-supplied
+// rays instead of camera rays.  A block of its own, passed after the kernel's scalar parameters: new fields at the end of
+// RenderParams would move those parameters, and with them the constant-bank offsets in every pixel instantiation's code.
+struct RayQuery {
+  const float *rays;        // [n][6]: origin.xyz, dir.xyz
+  float *rgb;               // path query: [n][3] colour of ray_colour (ray.fut:126-148)
+  int32_t *segments;        // path query, optional: [n] objs_hit calls of the path
+  float *hits;              // hit query (non-NULL = hit mode): [n][8] struct ray_b200_hit
+  const int32_t *perm;      // Morton-sorted leaf -> index into the caller's sphere array
+  int32_t n;
+  float t_min, t_max;       // hit query: the call's interval; path query: (0, 1e9) as ray_colour passes it
+  int32_t max_depth;        // path query: the depth limit of ray_colour (1 for a hit query)
+};
+
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
 struct WavefrontBuffers {
   float4 *ray_o[2];   // {origin.xyz, bits(path id = local item index)}
@@ -99,6 +113,8 @@ struct LaunchConfig {
 
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches);
+// Ray queries: the warp-queue kernel in ray mode (render_kernels.cu), whatever lc.kernel says
+cudaError_t launch_rays(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
 // build without RAYB200_ALL_KERNELS returns cudaErrorNotSupported)
 cudaError_t launch_lanewalk(const RenderParams &p, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches);

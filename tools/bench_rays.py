@@ -1,0 +1,109 @@
+#!/usr/bin/env python
+"""Ray queries on one GPU (include/ray_b200.h "ray queries"); prints one JSON line.
+
+    python tools/bench_rays.py [--rays N] [--seed S]
+
+- rays_irreg_paths_4M: N random rays (default 2^22) through trace_paths on irreg;
+- rays_irreg_hits_4M: the same rays through trace_hits;
+- rays_random1M_hits_4M: N random rays through trace_hits on the 1 M-sphere scene;
+- camera_rays_irreg_1000: irreg's 1000x1000 camera rays through trace_paths, next to the render call of the same frame
+  (the generic path against the fused one) and whether the quantised colours equal its pixels.
+Random rays come from a fixed seed: origins uniform in the scene's bounding box expanded by 10 % per side, directions
+uniform on the sphere, so every run sees the same inputs.  `ms` = the median of 3 queries (CUDA events of the context,
+after one warm-up query that loads the kernel); Mrays/s = objs_hit calls / kernel time (one per ray for a hit query, the
+segments trace_paths reports for a path query); `parity` = differing values against the CPU oracle
+(tests/ray_query_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+
+def random_rays(np, spheres, count, seed):
+    lo = (spheres[:, :3] - spheres[:, 6:7]).min(0)
+    hi = (spheres[:, :3] + spheres[:, 6:7]).max(0)
+    rng = np.random.default_rng(seed)
+    o = rng.uniform(lo - 0.1 * (hi - lo), hi + 0.1 * (hi - lo), (count, 3)).astype(np.float32)
+    d = rng.standard_normal((count, 3)).astype(np.float32)
+    return np.ascontiguousarray(np.concatenate([o, d / np.linalg.norm(d, axis=1, keepdims=True)], 1), np.float32)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rays", type=int, default=1 << 22)
+    ap.add_argument("--seed", type=int, default=2024)
+    args = ap.parse_args()
+    import numpy as np
+    import torch
+
+    import ray_query_oracle as Q
+    import raytracers_b200 as R
+
+    def bits(a):
+        return np.ascontiguousarray(a, np.float32).view(np.uint32)
+
+    gpu = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                         capture_output=True, text=True).stdout.strip().split(", ")
+    ctx = R.Context(device=0)
+
+    def timed(fn):
+        fn()   # the first query loads the ray-mode kernel
+        torch.cuda.synchronize()
+        ms = []
+        for _ in range(3):
+            fn()
+            torch.cuda.synchronize()
+            ms.append(ctx.last_render_ms())
+        return sorted(ms)[1]
+
+    out = {}
+    for tag, name, n_spheres, hh, ww, mode in (("rays_irreg_paths_4M", "irreg", None, 1000, 1000, "paths"),
+                                               ("rays_irreg_hits_4M", "irreg", None, 1000, 1000, "hits"),
+                                               ("rays_random1M_hits_4M", "random", 1000000, 2000, 2000, "hits"),
+                                               ("camera_rays_irreg_1000", "irreg", None, 1000, 1000, "camera")):
+        sc = ctx.scene(name, n=n_spheres)
+        pr = ctx.prepare_scene(hh, ww, sc)
+        rays = (R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6) if mode == "camera"
+                else random_rays(np, sc.arrays()[0], args.rays, args.seed))
+        cnt = rays.shape[0]
+        d_rays = torch.from_numpy(rays).cuda()
+        rgb = torch.empty((cnt, 3), dtype=torch.float32, device="cuda")
+        seg = torch.empty((cnt,), dtype=torch.int32, device="cuda")
+        hits = torch.empty((cnt, 8), dtype=torch.float32, device="cuda")
+        torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
+        if mode == "hits":
+            ms = timed(lambda: ctx.trace_hits_into(d_rays.data_ptr(), cnt, pr, hits.data_ptr()))
+            segments = cnt
+        else:
+            ms = timed(lambda: ctx.trace_paths_into(d_rays.data_ptr(), cnt, pr, rgb.data_ptr(), seg.data_ptr()))
+            segments = int(seg.sum(dtype=torch.int64))
+        rec = {"rays": cnt, "ms": round(ms, 3), "segments": segments, "Mrays_s": round(segments / ms / 1e3, 1)}
+        if mode == "camera":   # the fused path: the render call on the same frame
+            fr = torch.empty((hh, ww), dtype=torch.int32, device="cuda")
+            rec["render_ms"] = round(timed(lambda: ctx.render_into(fr.data_ptr(), hh, ww, pr, spp=1)), 3)
+            q = (np.float32(255.99) * rgb.cpu().numpy()).astype(np.int32)
+            rec["quantised_equals_render_pixels"] = bool(((q[:, 0] << 16 | q[:, 1] << 8 | q[:, 2]).reshape(hh, ww) == fr.cpu().numpy()).all())
+        sub = np.linspace(0, cnt - 1, 4096).astype(np.int64)
+        o = Q.prepare(name, hh, ww, n=n_spheres)
+        if mode == "hits":
+            rec["parity"] = int((bits(hits.cpu().numpy()[sub]) != bits(o.trace_hits(rays[sub]))).sum())
+        else:
+            want_rgb, want_seg = o.trace_paths(rays[sub])
+            rec["parity"] = int((bits(rgb.cpu().numpy()[sub]) != bits(want_rgb)).sum()) + int((seg.cpu().numpy()[sub] != want_seg).sum())
+        out[tag] = rec
+        del d_rays, rgb, seg, hits
+        pr.free(); sc.free()
+    ctx.close()
+    print(json.dumps({"gpu": gpu[0] if gpu else None, "power_limit_w": float(gpu[1]) if len(gpu) > 1 else None,
+                      "sm_max_mhz": int(gpu[2]) if len(gpu) > 2 else None, "rays": args.rays, "seed": args.seed, **out}), flush=True)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
