@@ -23,7 +23,8 @@
  * At spp = 1 this is bit-identical to the reference's render.
  *
  * Ray queries ("ray queries" below): rays the caller made are traced against a prepared scene to their closest hit
- * (objs_hit) or along their path (ray_colour), bit for bit, by the same warp-queue kernel in ray mode.
+ * (objs_hit), along their path (ray_colour), bit for bit, or to their first accepted sphere (occlusion), by the same
+ * warp-queue kernel in ray mode.
  */
 #ifndef RAY_B200_EXT_H
 #define RAY_B200_EXT_H
@@ -150,6 +151,16 @@ int ray_b200_trace_hits(struct futhark_context *ctx, const struct futhark_opaque
  * the path (or NULL).  Camera rays of a frame through this call, quantised, equal the frame. */
 int ray_b200_trace_paths(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
                          const float *rays_dev, int64_t n, int32_t max_depth, float *rgb_dev, int32_t *segments_dev);
+/* Occlusion (shadow / visibility rays): occluded_dev[i] = 1 if the reference's bvh_fold (bvh.fut:61-84) reaches some leaf
+ * whose sphere_hit L[i] r t_min t_max (ray.fut:32-51) is a hit, boxes tested against (t_min, t_max) as objs_hit tests
+ * them, else 0.  Unlike ray_b200_trace_hits there is no epsilon 0.1 (t_min bounds the sphere tests too) and no
+ * re-intersection, and the occluding sphere is not reported.  The answer is an OR over the reached leaves, so it does
+ * not depend on traversal order, and a ray's traversal stops at its first accepted sphere.  At t_min = 0.1 it equals
+ * "ray_b200_trace_hits(t_min = 0.1, t_max) reports a hit" for every ray whose closest hit has t < 2^24.
+ * occluded_dev: device uint8_t[n] (a torch.bool buffer).  Point-to-point visibility: origin = the point, direction =
+ * target - origin (not normalised), and an interval such as (1e-4, 1 - 1e-4), which excludes both end points. */
+int ray_b200_trace_occluded(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                            const float *rays_dev, int64_t n, float t_min, float t_max, uint8_t *occluded_dev);
 /* sizeof(struct ray_b200_hit) as the library was compiled (32). */
 int64_t ray_b200_hit_size(void);
 

@@ -146,6 +146,7 @@ def load_library(variant=""):
         "ray_b200_detile": (C.c_int, [vp, vp, vp, i64, i64, i32]),
         "ray_b200_trace_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
         "ray_b200_trace_paths": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_trace_occluded": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
         "ray_b200_hit_size": (i64, []),
         "ray_b200_count_work": (C.c_int, [vp, i64, i64, i32, vp, C.POINTER(WorkCounters)]),
         "ray_b200_ipc_alloc": (C.c_int, [vp, i64, pp, vp]),
@@ -622,6 +623,13 @@ class Context:
         self._check(self.lib.ray_b200_trace_paths(self.handle, prepared.handle, _ptr(rays_dev), int(n), int(max_depth),
                                                   _ptr(rgb_dev), _ptr(segments_dev)))
 
+    def trace_occluded_into(self, rays_dev, n, prepared, out_dev, t_min=0.0, t_max=1e9):
+        """Occlusion of n rays: out_dev = device uint8[n] (a torch.bool buffer), 1 where some sphere the BVH walk reaches
+        is hit in (t_min, t_max), else 0.  For point-to-point visibility pass direction = target - origin and an interval
+        such as (1e-4, 1 - 1e-4).  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_trace_occluded(self.handle, prepared.handle, _ptr(rays_dev), int(n), float(t_min),
+                                                     float(t_max), _ptr(out_dev)))
+
     def _rays_tensor(self, rays):
         import torch
         if not isinstance(rays, torch.Tensor) or rays.device.type != "cuda" or rays.device.index != self.device:
@@ -653,6 +661,16 @@ class Context:
         self.trace_paths_into(rays.data_ptr(), n, prepared, rgb.data_ptr(), seg.data_ptr(), max_depth=max_depth)
         self.sync()
         return rgb, seg
+
+    def trace_occluded(self, prepared, rays, t_min=0.0, t_max=1e9):
+        """Occlusion of a [n, 6] float32 CUDA tensor of rays: torch.bool [n].  Waits for torch's current stream before,
+        and synchronises the context after the query."""
+        torch = self._rays_tensor(rays)
+        n = rays.shape[0]
+        out = torch.empty((n,), dtype=torch.bool, device=rays.device)
+        self.trace_occluded_into(rays.data_ptr(), n, prepared, out.data_ptr(), t_min=t_min, t_max=t_max)
+        self.sync()
+        return out
 
     def count_work(self, h, w, prepared, spp=1):
         wc = WorkCounters()

@@ -1,6 +1,6 @@
 // C ABI, part 5: ray queries (include/ray_b200.h "ray queries") - caller-supplied rays traced against a prepared scene
-// by the warp-queue kernel in ray mode (render_kernels.cu), either to their closest hit (objs_hit) or along their whole
-// path (ray_colour).
+// by the warp-queue kernel in ray mode (render_kernels.cu), either to their closest hit (objs_hit), along their whole
+// path (ray_colour), or to their first accepted sphere (occlusion, the any-hit instantiations).
 #include "api_internal.h"
 
 #include <cmath>
@@ -11,9 +11,10 @@ static_assert(sizeof(struct ray_b200_hit) == 32, "struct ray_b200_hit is 32 byte
 
 namespace {
 
-// Validates, plans and enqueues one query on the context's stream (lane 0).  hits != NULL: hit query, else path query.
+// Validates, plans and enqueues one query on the context's stream (lane 0).  hits != NULL: hit query, occluded != NULL:
+// occlusion query, else path query.
 int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const float *rays, int64_t n, float t_min, float t_max,
-          int32_t max_depth, ray_b200_hit *hits, float *rgb, int32_t *segments, const char *what) {
+          int32_t max_depth, ray_b200_hit *hits, float *rgb, int32_t *segments, uint8_t *occluded, const char *what) {
   if (bad_ctx(ctx)) return 1;
   std::lock_guard<std::mutex> g(ctx->mu);
   if (n < 0 || n > ((int64_t)1 << 30)) { set_error(ctx, "%s: n = %lld is outside [0, 2^30]", what, (long long)n); return 1; }
@@ -23,14 +24,14 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const fl
   }
   if (max_depth < 0 || max_depth > 65535) { set_error(ctx, "%s: max_depth %d is outside [0, 65535]", what, max_depth); return 1; }
   if (n == 0) return 0;
-  if (!rays || (!hits && !rgb)) { set_error(ctx, "%s: NULL device buffer", what); return 1; }
+  if (!rays || (!hits && !rgb && !occluded)) { set_error(ctx, "%s: NULL device buffer", what); return 1; }
   if (!p || !p->dev.nodes || !p->dev.perm) { set_error(ctx, "%s: invalid prepared scene", what); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "%s: BVH depth %d exceeds the traversal stack", what, p->max_depth); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
   futhark_context::Lane &L = ctx->lanes[0];
   L.stream = ctx->stream;
   CUDA_TRY(ctx, cudaEventRecord(ctx->ev_start, L.stream));
-  if (!hits && max_depth == 0) {  // ray_colour's loop does not run: colour 0, no objs_hit call
+  if (!hits && !occluded && max_depth == 0) {  // ray_colour's loop does not run: colour 0, no objs_hit call
     CUDA_TRY(ctx, cudaMemsetAsync(rgb, 0, (size_t)n * 3 * sizeof(float), L.stream));
     if (segments) CUDA_TRY(ctx, cudaMemsetAsync(segments, 0, (size_t)n * sizeof(int32_t), L.stream));
   } else {
@@ -52,9 +53,11 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const fl
     Q.hits = reinterpret_cast<float *>(hits);
     Q.perm = p->dev.perm;
     Q.n = (int32_t)n;
-    Q.t_min = hits ? t_min : 0.0f;            // ray_colour calls objs_hit with (0, 1e9) (ray.fut:130)
-    Q.t_max = hits ? t_max : 1000000000.0f;
-    Q.max_depth = hits ? 1 : max_depth;
+    const bool one_segment = hits || occluded;
+    Q.t_min = one_segment ? t_min : 0.0f;            // ray_colour calls objs_hit with (0, 1e9) (ray.fut:130)
+    Q.t_max = one_segment ? t_max : 1000000000.0f;
+    Q.max_depth = one_segment ? 1 : max_depth;
+    Q.occluded = occluded;
     LaunchConfig lc;
     memset(&lc, 0, sizeof lc);
     lc.kernel = RAY_B200_KERNEL_WARPQUEUE;
@@ -83,12 +86,17 @@ extern "C" {
 
 int ray_b200_trace_hits(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev, int64_t n,
                         float t_min, float t_max, struct ray_b200_hit *hits_dev) {
-  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, hits_dev, nullptr, nullptr, "trace_hits");
+  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, hits_dev, nullptr, nullptr, nullptr, "trace_hits");
 }
 
 int ray_b200_trace_paths(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev, int64_t n,
                          int32_t max_depth, float *rgb_dev, int32_t *segments_dev) {
-  return trace(ctx, p, rays_dev, n, 0.0f, 1000000000.0f, max_depth, nullptr, rgb_dev, segments_dev, "trace_paths");
+  return trace(ctx, p, rays_dev, n, 0.0f, 1000000000.0f, max_depth, nullptr, rgb_dev, segments_dev, nullptr, "trace_paths");
+}
+
+int ray_b200_trace_occluded(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev,
+                            int64_t n, float t_min, float t_max, uint8_t *occluded_dev) {
+  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, nullptr, nullptr, nullptr, occluded_dev, "trace_occluded");
 }
 
 int64_t ray_b200_hit_size(void) { return (int64_t)sizeof(struct ray_b200_hit); }

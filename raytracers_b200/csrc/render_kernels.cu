@@ -128,12 +128,32 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // instead of the literal (0, 1e9), the depth limit is Q.max_depth, and a finished path writes Q.rgb / Q.segments.  A hit
 // query (Q.hits != NULL, warp-uniform) is a path query of one segment whose owner lane writes the hit record instead of
 // shading.  Rays of a batch are not coherent: ray mode has no packet walk and no spread samples.  Q is unused otherwise.
+//
+// Any-hit ray mode (kAnyHit, an occlusion query): one segment whose answer is "does some leaf the boxes admit accept its
+// sphere in (t_min, t_max)".  That is an OR over the set of reached leaves, so it is order-free like the closest-hit fold,
+// and it may stop early.  best_t[slot] is a "found" flag (kItemNoHit = nothing yet) set by a plain shared store: every
+// writer stores the same value.  Once a slot is marked, its leaf items skip the sphere test and its node items push no
+// children, which prunes the rest of that ray's tree; items already queued cost one pop each.  The drain still runs the
+// queues dry before a slot is refilled, so no stale item reaches a reused slot, and skipping only removes pushes, so the
+// queue bounds and the overflow guard hold as they are.  The owner lane writes Q.occluded and frees the slot.
+// Queue discipline of these instantiations: node batches as in the other instantiations, leaf batches from
+// kAnyHitLeafMin items on.
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, bool kRays = false>
+// any-hit instantiations: a leaf batch runs as soon as this many leaf items are queued (the other instantiations wait
+// for 32, a full batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured
+// against 1, 8 and 32, and newest-first node batches (wq_low = -1) against the default, in DESIGN.md §5.
+#ifndef RAYB200_ANYHIT_LEAF_MIN
+#define RAYB200_ANYHIT_LEAF_MIN 16
+#endif
+constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
+static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
+
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, bool kRays = false, bool kAnyHit = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without the packet walk");
+  static_assert(!kAnyHit || kRays, "the any-hit variant is a ray-mode query");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -390,6 +410,11 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               go = true;
               break;
             }
+            if constexpr (kAnyHit) {  // the root box already misses: not occluded
+              Q.occluded[p_item[slot]] = 0;
+              p_item[slot] = -1;
+              continue;
+            }
             if (kRays && Q.hits) {
               finish_hit(slot, -1.0f, -1, v3(0.0f, 0.0f, 0.0f), v3(0.0f, 0.0f, 0.0f));
               continue;
@@ -436,6 +461,25 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       bool hit = false;
       uint32_t tb = 0;
       int slot = 0, li = 0;
+      if constexpr (kAnyHit) {
+        // sphere_hit L[i] r t_min t_max with the query's own t_min (no epsilon); items of a marked ray are skipped
+        if (kFull || lane < n) {
+          const uint32_t it = lstk[ltop - 1 - lane];
+          slot = (int)(it >> kSlotShift);
+          li = (int)(it & kIndexMask);
+          if (best_t[slot] == kItemNoHit) {
+            const float4 ro = ray_o[slot], rd = ray_d[slot];
+            const float4 g = sc.sphere(li);
+            Ray r;
+            r.o = v3(ro.x, ro.y, ro.z);
+            r.d = v3(rd.x, rd.y, rd.z);
+            hit = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, t_lo, t_hi) >= 0.0f;
+          }
+        }
+        ltop -= n;
+        if (hit) best_t[slot] = 0u;  // any value but kItemNoHit: occluded
+        return;
+      }
       if (kFull || lane < n) {
         const uint32_t it = lstk[ltop - 1 - lane];
         slot = (int)(it >> kSlotShift);
@@ -464,22 +508,24 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const uint32_t it = nstk[ring(kDeque && bottom ? nhead + lane : ntop + ~lane)];
         tag = it & ~kIndexMask;
         const int slot = (int)(it >> kSlotShift), cur = (int)(it & kIndexMask);
-        const float4 ro = ray_o[slot], ri = ray_i[slot];
-        float4 q0, q1, q2, q3;
-        sc.node(cur, q0, q1, q2, q3);
-        Ray r;
-        r.o = v3(ro.x, ro.y, ro.z);
-        r.d = v3(0.0f, 0.0f, 0.0f);
-        RayInv q;
-        q.ix = ri.x; q.iy = ri.y; q.iz = ri.z; q.a = ro.w;
-        lptr = __float_as_int(q0.w);
-        rptr = __float_as_int(q1.w);
-        const bool hl = box_hit(q0.x, q0.y, q0.z, q1.x, q1.y, q1.z, r, q, t_lo, t_hi);
-        const bool hr = box_hit(q2.x, q2.y, q2.z, q3.x, q3.y, q3.z, r, q, t_lo, t_hi);
-        pl_leaf = lptr < 0;          // a leaf child has no box in the reference: always visited
-        pr_leaf = rptr < 0;
-        pl_node = hl && !pl_leaf;
-        pr_node = hr && !pr_leaf;
+        if (!kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: a marked ray pushes nothing, its subtree is pruned
+          const float4 ro = ray_o[slot], ri = ray_i[slot];
+          float4 q0, q1, q2, q3;
+          sc.node(cur, q0, q1, q2, q3);
+          Ray r;
+          r.o = v3(ro.x, ro.y, ro.z);
+          r.d = v3(0.0f, 0.0f, 0.0f);
+          RayInv q;
+          q.ix = ri.x; q.iy = ri.y; q.iz = ri.z; q.a = ro.w;
+          lptr = __float_as_int(q0.w);
+          rptr = __float_as_int(q1.w);
+          const bool hl = box_hit(q0.x, q0.y, q0.z, q1.x, q1.y, q1.z, r, q, t_lo, t_hi);
+          const bool hr = box_hit(q2.x, q2.y, q2.z, q3.x, q3.y, q3.z, r, q, t_lo, t_hi);
+          pl_leaf = lptr < 0;          // a leaf child has no box in the reference: always visited
+          pr_leaf = rptr < 0;
+          pl_node = hl && !pl_leaf;
+          pr_node = hr && !pr_leaf;
+        }
       }
       __syncwarp();  // top pops: all of them have been read before anything is pushed over them
       if (kDeque && bottom) nhead += n; else ntop -= n;
@@ -512,15 +558,17 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     auto drain = [&]() {
       __syncwarp();
       const int nroom = ncap - 96;
+      constexpr int kLeafMin = kAnyHit ? kAnyHitLeafMin : 32;  // leaf items that make a leaf batch due
       for (;;) {
         // the common case first and alone in its loop: full node batches while nothing else is due (the general
         // dispatch below costs ~12 instructions per batch).  One copy of the batch body for both pop directions.
-        while ((unsigned)(ntop - nhead - 32) <= (unsigned)(nroom - 32) && ltop < 32) {
+        while ((unsigned)(ntop - nhead - 32) <= (unsigned)(nroom - 32) && ltop < kLeafMin) {
           node_batch(full_t{}, kDeque && ntop - nhead <= nlow, 32);
           __syncwarp();
         }
         const int cnt = ntop - nhead;
         if (ltop >= 32) leaf_batch(full_t{}, 32);
+        else if (kLeafMin < 32 && ltop >= kLeafMin) leaf_batch(part_t{}, ltop);
         else if (cnt > 0) node_batch(part_t{}, false, cnt > nroom ? 1 : (cnt < 32 ? cnt : 32));
         else if (ltop > 0) leaf_batch(part_t{}, ltop);
         else break;
@@ -621,6 +669,11 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     for (int k = 0; k < K; k++) {
       if (!((trav >> k) & 1u)) continue;
       const int slot = lane + 32 * k;
+      if constexpr (kAnyHit) {
+        Q.occluded[p_item[slot]] = best_t[slot] != kItemNoHit ? 1 : 0;
+        p_item[slot] = -1;
+        continue;
+      }
       const float4 ro = ray_o[slot], rd = ray_d[slot], pl = p_light[slot];
       const uint32_t bt = best_t[slot];
       Ray r;
@@ -758,10 +811,12 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
 }
 
 // Ray queries: the same kernel in ray mode, one CTA per SM (fewer for small batches), planned like a pixel frame
-// without spread samples or packets.  The four variants per K are loaded on first use.
+// without spread samples or packets.  The four variants per K and query kind (closest hit / path, or any hit) are loaded
+// on first use.
 cudaError_t launch_rays(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches) {
   if (q.n <= 0) return cudaSuccess;
   const bool all_nodes = p.smem_nodes == p.n_inner, sph = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
+  const bool any_hit = q.occluded != nullptr;
   const int k = lc.wq_k == 1 ? 1 : 2;
   const int wthreads = 32 * lc.wq_warps;
   const int ncap = wq_node_capacity(k, p.max_depth, lc.wq_ncap);
@@ -772,20 +827,21 @@ cudaError_t launch_rays(const RenderParams &p, const RayQuery &q, const LaunchCo
   const long long useful = ((long long)q.n + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
   if (ctas > useful) ctas = useful;
   cudaError_t e = cudaSuccess;
-#define RAYB200_WQR(KK, A, S)                                                                                              \
+#define RAYB200_WQR(KK, A, S, AH)                                                                                          \
   do {                                                                                                                     \
-    e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, false, false, A, S, true>>(lc.max_dynamic_smem);                   \
+    e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, false, false, A, S, true, AH>>(lc.max_dynamic_smem);               \
     if (e == cudaSuccess)                                                                                                  \
-      render_warpqueue_kernel<KK, false, false, A, S, true><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, 0, 1, nlow, q); \
+      render_warpqueue_kernel<KK, false, false, A, S, true, AH><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, 0, 1, nlow, q); \
   } while (0)
-#define RAYB200_WQR2(KK)                                                                                                   \
+#define RAYB200_WQR2(KK, AH)                                                                                               \
   do {                                                                                                                     \
-    if (all_nodes && sph) RAYB200_WQR(KK, true, true);                                                                     \
-    else if (all_nodes) RAYB200_WQR(KK, true, false);                                                                      \
-    else if (sph) RAYB200_WQR(KK, false, true);                                                                            \
-    else RAYB200_WQR(KK, false, false);                                                                                    \
+    if (all_nodes && sph) RAYB200_WQR(KK, true, true, AH);                                                                 \
+    else if (all_nodes) RAYB200_WQR(KK, true, false, AH);                                                                  \
+    else if (sph) RAYB200_WQR(KK, false, true, AH);                                                                        \
+    else RAYB200_WQR(KK, false, false, AH);                                                                                \
   } while (0)
-  if (k == 1) RAYB200_WQR2(1); else RAYB200_WQR2(2);
+  if (any_hit) { if (k == 1) RAYB200_WQR2(1, true); else RAYB200_WQR2(2, true); }
+  else { if (k == 1) RAYB200_WQR2(1, false); else RAYB200_WQR2(2, false); }
 #undef RAYB200_WQR2
 #undef RAYB200_WQR
   if (e == cudaSuccess) (*launches)++;

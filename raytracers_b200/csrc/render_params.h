@@ -68,8 +68,9 @@ struct RayQuery {
   float *hits;              // hit query (non-NULL = hit mode): [n][8] struct ray_b200_hit
   const int32_t *perm;      // Morton-sorted leaf -> index into the caller's sphere array
   int32_t n;
-  float t_min, t_max;       // hit query: the call's interval; path query: (0, 1e9) as ray_colour passes it
-  int32_t max_depth;        // path query: the depth limit of ray_colour (1 for a hit query)
+  float t_min, t_max;       // hit / occlusion query: the call's interval; path query: (0, 1e9) as ray_colour passes it
+  int32_t max_depth;        // path query: the depth limit of ray_colour (1 for a hit or occlusion query)
+  uint8_t *occluded;        // occlusion query (non-NULL = the any-hit instantiations): [n] 0 / 1
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.

@@ -1,18 +1,24 @@
 #!/usr/bin/env python
 """Ray queries on one GPU (include/ray_b200.h "ray queries"); prints one JSON line.
 
-    python tools/bench_rays.py [--rays N] [--seed S]
+    python tools/bench_rays.py [--rays N] [--seed S] [--only WORKLOAD,...]
 
 - rays_irreg_paths_4M: N random rays (default 2^22) through trace_paths on irreg;
 - rays_irreg_hits_4M: the same rays through trace_hits;
 - rays_random1M_hits_4M: N random rays through trace_hits on the 1 M-sphere scene;
 - camera_rays_irreg_1000: irreg's 1000x1000 camera rays through trace_paths, next to the render call of the same frame
-  (the generic path against the fused one) and whether the quantised colours equal its pixels.
+  (the generic path against the fused one) and whether the quantised colours equal its pixels;
+- rays_irreg_occluded_4M, rays_random1M_occluded_4M: the random rays of the hit workloads through trace_occluded with the
+  interval (0.1, 1e9);
+- shadow_irreg_1000: irreg's 1000x1000 camera rays through trace_hits, then a segment from every hit point to a point
+  light above the scene (direction = light - point, interval (1e-4, 1 - 1e-4)) through trace_occluded.
+An occlusion record has trace_hits' time on the same rays and interval beside its own (`hits_ms`) and the fraction of
+rays occluded; its Mrays/s counts one ray per query.
 Random rays come from a fixed seed: origins uniform in the scene's bounding box expanded by 10 % per side, directions
 uniform on the sphere, so every run sees the same inputs.  `ms` = the median of 3 queries (CUDA events of the context,
 after one warm-up query that loads the kernel); Mrays/s = objs_hit calls / kernel time (one per ray for a hit query, the
 segments trace_paths reports for a path query); `parity` = differing values against the CPU oracle
-(tests/ray_query_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
+(tests/ray_query_oracle.py, tests/occlusion_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
 """
 import argparse
 import json
@@ -38,10 +44,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rays", type=int, default=1 << 22)
     ap.add_argument("--seed", type=int, default=2024)
+    ap.add_argument("--only", default="", help="comma-separated workload names (default: all)")
     args = ap.parse_args()
     import numpy as np
     import torch
 
+    import occlusion_oracle as OQ
     import ray_query_oracle as Q
     import raytracers_b200 as R
 
@@ -66,38 +74,64 @@ def main():
     for tag, name, n_spheres, hh, ww, mode in (("rays_irreg_paths_4M", "irreg", None, 1000, 1000, "paths"),
                                                ("rays_irreg_hits_4M", "irreg", None, 1000, 1000, "hits"),
                                                ("rays_random1M_hits_4M", "random", 1000000, 2000, 2000, "hits"),
-                                               ("camera_rays_irreg_1000", "irreg", None, 1000, 1000, "camera")):
+                                               ("camera_rays_irreg_1000", "irreg", None, 1000, 1000, "camera"),
+                                               ("rays_irreg_occluded_4M", "irreg", None, 1000, 1000, "occluded"),
+                                               ("rays_random1M_occluded_4M", "random", 1000000, 2000, 2000, "occluded"),
+                                               ("shadow_irreg_1000", "irreg", None, 1000, 1000, "shadow")):
+        if args.only and tag not in args.only.split(","):
+            continue
         sc = ctx.scene(name, n=n_spheres)
         pr = ctx.prepare_scene(hh, ww, sc)
-        rays = (R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6) if mode == "camera"
-                else random_rays(np, sc.arrays()[0], args.rays, args.seed))
+        t_min, t_max = (1e-4, 1 - 1e-4) if mode == "shadow" else (0.1, 1e9)
+        if mode in ("camera", "shadow"):
+            rays = R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6)
+        else:
+            rays = random_rays(np, sc.arrays()[0], args.rays, args.seed)
+        if mode == "shadow":   # the same construction as tests/test_occlusion.py
+            hit = ctx.trace_hits(pr, torch.from_numpy(rays).cuda())
+            p = hit["p"].cpu().numpy()[hit["t"].cpu().numpy() >= 0]
+            s = sc.arrays()[0]
+            lo, hi = (s[:, :3] - s[:, 6:7]).min(0), (s[:, :3] + s[:, 6:7]).max(0)
+            light = np.float32([(lo[0] + hi[0]) / 2, hi[1] + (hi[1] - lo[1]), (lo[2] + hi[2]) / 2])
+            rays = np.ascontiguousarray(np.concatenate([p, light[None] - p], 1), np.float32)
         cnt = rays.shape[0]
         d_rays = torch.from_numpy(rays).cuda()
         rgb = torch.empty((cnt, 3), dtype=torch.float32, device="cuda")
         seg = torch.empty((cnt,), dtype=torch.int32, device="cuda")
         hits = torch.empty((cnt, 8), dtype=torch.float32, device="cuda")
+        occ = torch.empty((cnt,), dtype=torch.bool, device="cuda")
         torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
-        if mode == "hits":
+        if mode in ("occluded", "shadow"):
+            ms = timed(lambda: ctx.trace_occluded_into(d_rays.data_ptr(), cnt, pr, occ.data_ptr(), t_min=t_min, t_max=t_max))
+            segments = cnt
+        elif mode == "hits":
             ms = timed(lambda: ctx.trace_hits_into(d_rays.data_ptr(), cnt, pr, hits.data_ptr()))
             segments = cnt
         else:
             ms = timed(lambda: ctx.trace_paths_into(d_rays.data_ptr(), cnt, pr, rgb.data_ptr(), seg.data_ptr()))
             segments = int(seg.sum(dtype=torch.int64))
         rec = {"rays": cnt, "ms": round(ms, 3), "segments": segments, "Mrays_s": round(segments / ms / 1e3, 1)}
+        if mode in ("occluded", "shadow"):   # the closest-hit query on the same rays and interval, timed the same way
+            rec["t_min"], rec["t_max"] = t_min, t_max
+            rec["hits_ms"] = round(timed(lambda: ctx.trace_hits_into(d_rays.data_ptr(), cnt, pr, hits.data_ptr(), t_min=t_min, t_max=t_max)), 3)
+            rec["hits_over_occluded"] = round(rec["hits_ms"] / rec["ms"], 3)
+            rec["occluded_fraction"] = round(float(occ.float().mean()), 4)
         if mode == "camera":   # the fused path: the render call on the same frame
             fr = torch.empty((hh, ww), dtype=torch.int32, device="cuda")
             rec["render_ms"] = round(timed(lambda: ctx.render_into(fr.data_ptr(), hh, ww, pr, spp=1)), 3)
             q = (np.float32(255.99) * rgb.cpu().numpy()).astype(np.int32)
             rec["quantised_equals_render_pixels"] = bool(((q[:, 0] << 16 | q[:, 1] << 8 | q[:, 2]).reshape(hh, ww) == fr.cpu().numpy()).all())
         sub = np.linspace(0, cnt - 1, 4096).astype(np.int64)
-        o = Q.prepare(name, hh, ww, n=n_spheres)
-        if mode == "hits":
+        o = (OQ if mode in ("occluded", "shadow") else Q).prepare(name, hh, ww, n=n_spheres)
+        if mode in ("occluded", "shadow"):
+            rec["parity"] = int((occ.cpu().numpy()[sub] != o.trace_occluded(rays[sub], t_min, t_max)).sum())
+        elif mode == "hits":
             rec["parity"] = int((bits(hits.cpu().numpy()[sub]) != bits(o.trace_hits(rays[sub]))).sum())
         else:
             want_rgb, want_seg = o.trace_paths(rays[sub])
             rec["parity"] = int((bits(rgb.cpu().numpy()[sub]) != bits(want_rgb)).sum()) + int((seg.cpu().numpy()[sub] != want_seg).sum())
         out[tag] = rec
-        del d_rays, rgb, seg, hits
+        del d_rays, rgb, seg, hits, occ
         pr.free(); sc.free()
     ctx.close()
     print(json.dumps({"gpu": gpu[0] if gpu else None, "power_limit_w": float(gpu[1]) if len(gpu) > 1 else None,

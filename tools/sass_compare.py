@@ -4,9 +4,10 @@
     python tools/sass_compare.py OLD.so NEW.so
 
 cuobjdump -sass of both files, split into functions, names demangled.  A function of OLD must exist in NEW with the
-same instructions and encodings.  The ray-mode template parameter of the warp-queue kernel (kRays, default false) and
-its RayQuery parameter only change the symbol names of the pixel instantiations; they are mapped back before the
-comparison.  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
+same instructions and encodings.  The any-hit template parameter of the warp-queue kernel (kAnyHit, default false)
+only changes the symbol names of the pixel and the closest-hit / path instantiations; it is mapped back before the
+comparison, so OLD is a build that has ray mode (kRays) but no any-hit variants.  Functions that exist in NEW only are
+listed.  Exit code 0 = every function of OLD is identical.
 """
 import collections
 import re
@@ -41,9 +42,9 @@ def functions(path):
 
 
 def normalise(name):
-    # render_warpqueue_kernel<K, kSpread, kPacket, kAllNodes, kSpheres, false>(RenderParams, int x 4, RayQuery)
-    # -> the name the same instantiation had before ray mode existed
-    return re.sub(r"render_warpqueue_kernel<([^>]*), false>\((.*), rayb200::RayQuery\)", r"render_warpqueue_kernel<\1>(\2)", name)
+    # render_warpqueue_kernel<K, kSpread, kPacket, kAllNodes, kSpheres, kRays, false>(...)
+    # -> the name the same instantiation had before the any-hit parameter existed
+    return re.sub(r"render_warpqueue_kernel<((?:[^,<>]+, ){5}[^,<>]+), false>\(", r"render_warpqueue_kernel<\1>(", name)
 
 
 def main():
