@@ -67,7 +67,6 @@ struct futhark_context {
   struct PinnedBlock { unsigned char *ptr; size_t bytes; cudaEvent_t last_use; };
   std::vector<PinnedBlock> pinned_cache;    // page-locked upload buffers of freed prepared scenes, reused by the next prepare_scene
   BvhBuildResult *d_build_result = nullptr, *h_build_result = nullptr;  // device scratch / page-locked host mirror
-  int32_t plan_wq_warps = 0, plan_wq_packet = 0, plan_wq_k = 1, plan_wq_ncap = 512, plan_lw_slots = 0, plan_kernel = 0;  // fill_params' plan for the frame being set up
   // single-process multi-GPU (cfg.gpus > 1): one helper context per extra device; this context is rank 0 and owns them
   std::vector<futhark_context *> peers;
   bool is_peer = false;
@@ -90,7 +89,6 @@ struct futhark_context {
     TileOrderBuffers tile_order_plan{};
   } lanes[2];
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool plan_auto_k2 = false;            // fill_params: the K = 2 plan was chosen automatically
   bool pipeline = false;                // ray_b200_context_set_pipeline: batches do not join lane 1 back
   uint32_t lane_seq = 0;                // pipelined submission: frames alternate lanes across calls
   cudaStream_t reclaim = nullptr;       // scene memory is freed here, ordered after its last use on either lane
@@ -168,17 +166,15 @@ inline int64_t tiles_of_rank(int64_t h, int64_t w, int32_t rank, int32_t world) 
 
 // api_render.cu
 int resolve_kernel(const futhark_context *ctx);
+// The parameter block of one frame and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
+// slots, ...), which the caller hands to do_render.
 int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
-                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P);
+                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc);
+void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P);  // zeroes P, then its scene half
 // The warp-queue kernel's plan for one launch (pixel frames and ray queries): rays in flight per warp (32 k), warps per
-// CTA, node-queue cap, packet threshold and how much of the scene is staged in shared memory.
-struct WqPlan {
-  int32_t k = 1, warps = 1, packet = 0, ncap = 512;
-  bool auto_k2 = false;
-  int32_t smem_nodes = 0, smem_spheres = 0;
-};
+// CTA, node-queue cap and packet threshold in lc, how much of the scene is staged in shared memory in P.
 int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool will_spread, bool coherent, bool rays,
-                   const char *what, WqPlan &wp);
+                   const char *what, RenderParams &P, LaunchConfig &lc);
 int64_t cap_staging(const futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t budget);
 void split_staging(const futhark_opaque_prepared_scene *p, int64_t budget, int32_t &smem_nodes, int32_t &smem_spheres);
 void free_wavefront(futhark_context *ctx);
@@ -189,8 +185,8 @@ struct FrameFlags {
   uint32_t wait_value = 0;
   uint32_t *done_flag = nullptr;
 };
-int do_render(futhark_context *ctx, RenderParams &P, int lane_id = 0, bool timed = true, const FrameFlags *ff = nullptr,
-              const futhark_opaque_prepared_scene *scene = nullptr);
+int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id = 0, bool timed = true,
+              const FrameFlags *ff = nullptr, const futhark_opaque_prepared_scene *scene = nullptr);
 // api_multigpu.cu: the single-process multi-GPU mode (RAY_GPUS > 1) of futhark_entry_render
 int create_helper_contexts(futhark_context *ctx, const futhark_context_config *cfg, int ndev);
 int render_multi_device(futhark_context *ctx, futhark_i32_2d *img, int64_t h, int64_t w, int32_t spp, const futhark_opaque_prepared_scene *p);

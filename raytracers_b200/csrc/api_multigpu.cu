@@ -90,10 +90,11 @@ int render_multi_device(futhark_context *ctx, futhark_i32_2d *img, int64_t h, in
   cudaSetDevice(ctx->cfg.device);
   // rank 0's own shard straight into slot 0 of the gather buffer
   RenderParams P;
-  if (fill_params(ctx, p, h, w, spp, 0, world, ctx->gathered, nullptr, true, P)) return 1;
+  LaunchConfig lc;
+  if (fill_params(ctx, p, h, w, spp, 0, world, ctx->gathered, nullptr, true, P, lc)) return 1;
   if (P.local_tiles < padded)
     cudaMemsetAsync(ctx->gathered + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4, ctx->stream);
-  if (do_render(ctx, P, 0, true, nullptr, p)) return 1;
+  if (do_render(ctx, P, lc, 0, true, nullptr, p)) return 1;
   for (int r = 1; r < world; r++) {
     futhark_context *peer = ctx->peers[(size_t)r - 1];
     cudaStreamWaitEvent(ctx->stream, peer->peer_done, 0);

@@ -35,16 +35,10 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const fl
     CUDA_TRY(ctx, cudaMemsetAsync(rgb, 0, (size_t)n * 3 * sizeof(float), L.stream));
     if (segments) CUDA_TRY(ctx, cudaMemsetAsync(segments, 0, (size_t)n * sizeof(int32_t), L.stream));
   } else {
-    WqPlan wp;
-    if (plan_warpqueue(ctx, p, false, false, true, what, wp)) return 1;
     RenderParams P;
-    memset(&P, 0, sizeof P);
-    P.nodes = p->dev.nodes; P.nodes_soa = p->dev.nodes_soa; P.geom = p->dev.geom; P.colour = p->dev.colour;
-    P.n_inner = (int32_t)(p->n - 1); P.n_leaves = (int32_t)p->n;
-    P.max_depth = p->max_depth;
-    memcpy(P.root_box, p->root_box, sizeof P.root_box);
-    P.smem_nodes = wp.smem_nodes;
-    P.smem_spheres = wp.smem_spheres;
+    LaunchConfig lc;
+    fill_scene_params(p, P);
+    if (plan_warpqueue(ctx, p, false, false, true, what, P, lc)) return 1;
     P.work_cursor = L.work_cursor;
     RayQuery Q;
     Q.rays = rays;
@@ -58,17 +52,8 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const fl
     Q.t_max = one_segment ? t_max : 1000000000.0f;
     Q.max_depth = one_segment ? 1 : max_depth;
     Q.occluded = occluded;
-    LaunchConfig lc;
-    memset(&lc, 0, sizeof lc);
-    lc.kernel = RAY_B200_KERNEL_WARPQUEUE;
-    lc.sm_count = ctx->sm_count;
-    lc.wq_warps = wp.warps;
-    lc.wq_k = wp.k;
-    lc.wq_ncap = wp.ncap;
-    lc.wq_low = ctx->cfg.wq_low;
-    lc.max_dynamic_smem = ctx->max_smem_optin;
     CUDA_TRY(ctx, cudaMemsetAsync(L.work_cursor, 0, 2 * sizeof(int32_t), L.stream));
-    CUDA_TRY(ctx, launch_rays(P, Q, lc, L.stream, &ctx->launches));
+    CUDA_TRY(ctx, launch_warpqueue(P, Q, lc, L.stream, &ctx->launches));
     CUDA_TRY(ctx, cudaGetLastError());
   }
   // this query reads the scene's device memory until here on lane 0 (release_scene_block waits for it)

@@ -1,5 +1,5 @@
-// C ABI, part 3: the render path - per-frame parameter block and shared-memory plan (fill_params), launch of one frame
-// on a lane (do_render), the entries render / render_spp and the render extensions (render_into, render_host, shards,
+// C ABI, part 3: the render path - per-frame parameter block and launch plan (fill_params), launch of one frame on a
+// lane (do_render), the entries render / render_spp and the render extensions (render_into, render_host, shards,
 // batches with two frames in flight, de-tiling, peer-memory frames, work counters).
 #include "api_internal.h"
 
@@ -40,9 +40,38 @@ int ensure_offsets(futhark_context *ctx, int32_t spp) {
 
 int resolve_kernel(const futhark_context *ctx);
 
-// Fills the kernel parameter block for one frame.
+// Zeroes the kernel parameter block and fills its scene half from a prepared scene.
+void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P) {
+  memset(&P, 0, sizeof P);
+  P.nodes = p->dev.nodes; P.nodes_soa = p->dev.nodes_soa; P.geom = p->dev.geom; P.colour = p->dev.colour;
+  P.n_inner = (int32_t)(p->n - 1); P.n_leaves = (int32_t)p->n;
+  P.max_depth = p->max_depth;
+  memcpy(P.root_box, p->root_box, sizeof P.root_box);
+}
+
+// The launch plan every kernel's own planning starts from: the context's tuning, one warp, K = 1, no packet walk.
+static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
+  LaunchConfig lc;
+  lc.kernel = kernel;
+  lc.blocks_per_sm = ctx->cfg.blocks_per_sm;
+  lc.sm_count = ctx->sm_count;
+  lc.refill_min = ctx->cfg.refill_min;
+  lc.wq_warps = 1;
+  lc.wq_k = 1;
+  lc.wq_refill = ctx->cfg.wq_refill < 1 ? 1 : (ctx->cfg.wq_refill > 32 ? 32 : ctx->cfg.wq_refill);
+  lc.wq_low = ctx->cfg.wq_low;
+  lc.wq_packet = 0;
+  lc.wq_ncap = ctx->cfg.wq_ncap;
+  lc.lw_slots = 0;
+  lc.lw_idle_min = ctx->cfg.lw_idle_min;
+  lc.lw_passes = ctx->cfg.lw_passes;
+  lc.max_dynamic_smem = ctx->max_smem_optin;
+  return lc;
+}
+
+// Fills the kernel parameter block for one frame, and the frame's launch plan.
 int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
-                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P) {
+                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc) {
   if (!p || !p->dev.nodes) { set_error(ctx, "render: invalid prepared scene"); return 1; }
   if (h <= 0 || w <= 0 || h > 65536 || w > 65536 || ((h + 3) / 4) * ((w + 7) / 8) > ((int64_t)1 << 25)) {
     // work items are 32-bit: at most 2^30 (padded) pixels per frame
@@ -53,11 +82,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   if (world < 1 || rank < 0 || rank >= world) { set_error(ctx, "render: bad shard %d/%d", rank, world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
   if (ensure_offsets(ctx, spp)) return 1;
-  memset(&P, 0, sizeof P);
-  P.nodes = p->dev.nodes; P.nodes_soa = p->dev.nodes_soa; P.geom = p->dev.geom; P.colour = p->dev.colour;
-  P.n_inner = (int32_t)(p->n - 1); P.n_leaves = (int32_t)p->n;
-  P.max_depth = p->max_depth;
-  memcpy(P.root_box, p->root_box, sizeof P.root_box);
+  fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
   // h, w only set the pixel grid (ray.fut:246-247) — exactly as in the reference.
   memcpy(P.cam, &p->cam, sizeof P.cam);
@@ -99,6 +124,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
     const size_t need = (size_t)ctx->sm_count * kWqMaxWarps * kWqRing * (size_t)spp * sizeof(float4);
     if (!ctx->cfg.wq_spread || spp > 65535 || need > kSpreadBudget) kern = RAY_B200_KERNEL_WARPQUEUE;
   }
+  lc = launch_config(ctx, kern);
   if (kern == RAY_B200_KERNEL_STREAMQUEUE) {
     const int k = 1;
     const int64_t per_warp = (int64_t)sq_warp_bytes(k, wq_node_capacity(k, p->max_depth));
@@ -106,8 +132,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
     while (wq_w > 1 && wq_w * per_warp + 8192 > (int64_t)ctx->max_smem_optin) wq_w--;
     budget = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512;
     if (budget < 256) { set_error(ctx, "render: stream-queue kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
-    ctx->plan_wq_packet = 0;
-    ctx->plan_wq_warps = (int32_t)wq_w;
+    lc.wq_warps = (int32_t)wq_w;
   }
   if (kern == RAY_B200_KERNEL_WARPQUEUE) {
     // samples will be spread if the finished-sample buffer fits the budget (do_render allocates it; a failed allocation
@@ -116,17 +141,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
                              (size_t)ctx->sm_count * kWqMaxWarps * kWqRing * (size_t)spp * sizeof(float4) <= kSpreadBudget;
     // the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame
     const bool coherent = spp > 1 || h * w >= ((int64_t)1 << 22);
-    WqPlan wp;
-    if (plan_warpqueue(ctx, p, will_spread, coherent, false, "render", wp)) return 1;
-    ctx->plan_wq_packet = wp.packet;
-    ctx->plan_wq_warps = wp.warps;
-    ctx->plan_wq_k = wp.k;
-    ctx->plan_wq_ncap = wp.ncap;
-    ctx->plan_auto_k2 = wp.auto_k2;
-    ctx->plan_kernel = kern;
-    P.smem_nodes = wp.smem_nodes;
-    P.smem_spheres = wp.smem_spheres;
-    return 0;
+    return plan_warpqueue(ctx, p, will_spread, coherent, false, "render", P, lc);
   }
   if (kern == RAY_B200_KERNEL_LANEWALK) {
     // one CTA per SM: lw_warps warps (32 unless told otherwise) x lw_slots path slots each (48 unless told otherwise,
@@ -142,12 +157,10 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
       else { set_error(ctx, "render: lane-walk kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
     }
     budget = (int64_t)ctx->max_smem_optin - w * (int64_t)lw_warp_bytes((int)r, scap) - 512;
-    ctx->plan_wq_warps = (int32_t)w;
-    ctx->plan_lw_slots = (int32_t)r;
-    ctx->plan_wq_packet = 0;
+    lc.wq_warps = (int32_t)w;
+    lc.lw_slots = (int32_t)r;
     budget = cap_staging(ctx, p, budget);
   }
-  ctx->plan_kernel = kern;
   split_staging(p, budget, P.smem_nodes, P.smem_spheres);
   return 0;
 }
@@ -176,9 +189,11 @@ void split_staging(const futhark_opaque_prepared_scene *p, int64_t budget, int32
 
 // The warp-queue kernel's plan for a prepared scene (pixel frames and ray queries): one CTA per SM, as many warps as asked
 // for (<= 32) while their queues leave >= 8 KB for staging; deep trees need bigger node stacks, so they get fewer warps.
-// `coherent`: the rays a warp holds are coherent enough for the packet walk; `rays`: no packet walk at all.
+// `coherent`: the rays a warp holds are coherent enough for the packet walk; `rays`: no packet walk at all.  The staging
+// split goes to P.smem_nodes / P.smem_spheres, the rest of the plan to lc.
 int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool will_spread, bool coherent, bool rays,
-                   const char *what, WqPlan &wp) {
+                   const char *what, RenderParams &P, LaunchConfig &lc) {
+  lc = launch_config(ctx, RAY_B200_KERNEL_WARPQUEUE);
   for (int pass = 0; pass < 2; pass++) {
     // Rays in flight per warp (32 K) and node-queue cap.  wq_k = 0 (default): K = 2 with a kAutoK2Ncap-entry node queue and
     // as many warps (>= kAutoK2MinWarps) as still leave the WHOLE scene (tree + spheres) staged - a round of 64 rays has
@@ -224,15 +239,14 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
     }
     int64_t budget = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512;
     if (budget < 256) { set_error(ctx, "%s: warp-queue kernel does not fit shared memory (tree depth %d)", what, p->max_depth); return 1; }
-    wp.packet = want_packet > 32 ? 32 : want_packet;
-    wp.warps = (int32_t)wq_w;
-    wp.k = k;
-    wp.ncap = ncap_cfg;
-    wp.auto_k2 = auto_k2;
-    split_staging(p, cap_staging(ctx, p, budget), wp.smem_nodes, wp.smem_spheres);
+    lc.wq_packet = want_packet > 32 ? 32 : want_packet;
+    lc.wq_warps = (int32_t)wq_w;
+    lc.wq_k = k;
+    lc.wq_ncap = ncap_cfg;
+    split_staging(p, cap_staging(ctx, p, budget), P.smem_nodes, P.smem_spheres);
     // belt and braces: the K = 2 plan is only worth anything when the scene is staged whole (a scene that just misses
     // fetches its lower nodes from L2 with half the warps); if anything above left it short, plan again with K = 1
-    if (!auto_k2 || (wp.smem_nodes == (int32_t)(p->n - 1) && wp.smem_spheres == (int32_t)p->n)) break;
+    if (!auto_k2 || (P.smem_nodes == (int32_t)(p->n - 1) && P.smem_spheres == (int32_t)p->n)) break;
   }
   return 0;
 }
@@ -291,30 +305,35 @@ int ensure_wavefront(futhark_context *ctx, int64_t items) {
   return 0;
 }
 
-// Enqueues one frame on lane `lane_id` (0 = the context's stream).  `timed`: bracket it with the context's timing events.
-// `ff`: peer-frame protocol of the frame (api_internal.h).
-int do_render(futhark_context *ctx, RenderParams &P, int lane_id, bool timed, const FrameFlags *ff,
+// The lane's scratch for sorting `tiles` tile keys into a claim order (keys, sorted keys, ids, order, cub temp: one
+// allocation, grown on demand), laid out in L.tile_order_plan.
+static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64_t tiles) {
+  const size_t n = (size_t)tiles, tmp = tile_order_sort_bytes(tiles);
+  auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t need = 4 * up(4 * n) + up(tmp);
+  if (need > L.tile_order_bytes) {
+    CUDA_TRY(ctx, cudaStreamSynchronize(L.stream));
+    if (L.tile_order_block) CUDA_TRY(ctx, cudaFree(L.tile_order_block));
+    L.tile_order_block = nullptr; L.tile_order_bytes = 0;
+    CUDA_TRY(ctx, cudaMalloc(&L.tile_order_block, need));
+    L.tile_order_bytes = need;
+  }
+  TileOrderBuffers &tb = L.tile_order_plan;
+  unsigned char *q = L.tile_order_block;
+  tb.keys = reinterpret_cast<uint32_t *>(q); q += up(4 * n);
+  tb.keys_sorted = reinterpret_cast<uint32_t *>(q); q += up(4 * n);
+  tb.ids = reinterpret_cast<int32_t *>(q); q += up(4 * n);
+  tb.order = reinterpret_cast<int32_t *>(q); q += up(4 * n);
+  tb.sort_tmp = q; tb.sort_tmp_bytes = tmp;
+  return 0;
+}
+
+// Enqueues one frame with launch plan `lc` (fill_params) on lane `lane_id` (0 = the context's stream).  `timed`: bracket
+// it with the context's timing events.  `ff`: peer-frame protocol of the frame (api_internal.h).
+int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff,
               const futhark_opaque_prepared_scene *scene) {
   futhark_context::Lane &L = ctx->lanes[lane_id];
   if (lane_id == 0) L.stream = ctx->stream;
-  LaunchConfig lc;
-  lc.kernel = ctx->plan_kernel;
-  lc.blocks_per_sm = ctx->cfg.blocks_per_sm;
-  lc.sm_count = ctx->sm_count;
-  lc.smem_budget = ctx->cfg.smem_budget;
-  lc.refill_min = ctx->cfg.refill_min;
-  lc.tail_from = ctx->cfg.tail_from;
-  lc.wq_warps = ctx->plan_wq_warps > 0 ? ctx->plan_wq_warps : 1;
-  lc.wq_k = ctx->plan_wq_k == 2 ? 2 : 1;
-  lc.wq_low = ctx->cfg.wq_low;
-  lc.wq_refill = ctx->cfg.wq_refill < 1 ? 1 : (ctx->cfg.wq_refill > 32 ? 32 : ctx->cfg.wq_refill);
-  lc.wq_packet = ctx->plan_wq_packet;
-  lc.wq_ncap = lc.kernel == RAY_B200_KERNEL_WARPQUEUE ? ctx->plan_wq_ncap : ctx->cfg.wq_ncap;
-  lc.lw_slots = ctx->plan_lw_slots;
-  lc.lw_idle_min = ctx->cfg.lw_idle_min;
-  lc.lw_passes = ctx->cfg.lw_passes;
-  lc.max_dynamic_smem = ctx->max_smem_optin;
-
   if (lc.kernel == RAY_B200_KERNEL_WAVEFRONT && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
   P.sample_buf = nullptr;
   if ((lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_STREAMQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK) && P.spp > 1 && P.spp <= 65535 && ctx->cfg.wq_spread) {
@@ -341,25 +360,8 @@ int do_render(futhark_context *ctx, RenderParams &P, int lane_id, bool timed, co
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
     P.probe_segments = std::min(std::max(ctx->cfg.probe_segments, 1), kMaxDepth);
-    const size_t n = (size_t)P.local_tiles, tmp = tile_order_sort_bytes(P.local_tiles);
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t need = 4 * up(4 * n) + up(tmp);
-    if (need > L.tile_order_bytes) {
-      CUDA_TRY(ctx, cudaStreamSynchronize(L.stream));
-      if (L.tile_order_block) CUDA_TRY(ctx, cudaFree(L.tile_order_block));
-      L.tile_order_block = nullptr; L.tile_order_bytes = 0;
-      CUDA_TRY(ctx, cudaMalloc(&L.tile_order_block, need));
-      L.tile_order_bytes = need;
-    }
-    TileOrderBuffers tb;
-    unsigned char *q = L.tile_order_block;
-    tb.keys = reinterpret_cast<uint32_t *>(q); q += up(4 * n);
-    tb.keys_sorted = reinterpret_cast<uint32_t *>(q); q += up(4 * n);
-    tb.ids = reinterpret_cast<int32_t *>(q); q += up(4 * n);
-    tb.order = reinterpret_cast<int32_t *>(q); q += up(4 * n);
-    tb.sort_tmp = q; tb.sort_tmp_bytes = tmp;
-    P.tile_order = tb.order;
-    L.tile_order_plan = tb;
+    if (plan_tile_order(ctx, L, P.local_tiles)) return 1;
+    P.tile_order = L.tile_order_plan.order;
   }
   // Learned claim order (every frame of a prepared scene, single calls - the protocol of main.c, which renders the same
   // frame `runs` times - and batch frames on either lane alike).  First frame of a geometry: record the longest path per
@@ -392,26 +394,9 @@ int do_render(futhark_context *ctx, RenderParams &P, int lane_id, bool timed, co
       CUDA_TRY(ctx, cudaMemsetAsync(oc.cost, 0, (size_t)P.local_tiles * sizeof(uint32_t), L.stream));
       P.tile_cost = oc.cost;
       record_order = true;
-      // scratch of the sort that follows the frame (same layout as the heavy-first probe's)
-      const size_t n = (size_t)P.local_tiles, tmp = tile_order_sort_bytes(P.local_tiles);
-      auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-      const size_t need = 4 * up(4 * n) + up(tmp);
-      if (need > L.tile_order_bytes) {
-        CUDA_TRY(ctx, cudaStreamSynchronize(L.stream));
-        if (L.tile_order_block) CUDA_TRY(ctx, cudaFree(L.tile_order_block));
-        L.tile_order_block = nullptr; L.tile_order_bytes = 0;
-        CUDA_TRY(ctx, cudaMalloc(&L.tile_order_block, need));
-        L.tile_order_bytes = need;
-      }
-      TileOrderBuffers tb;
-      unsigned char *q = L.tile_order_block;
-      tb.keys = reinterpret_cast<uint32_t *>(q); q += up(4 * n);
-      tb.keys_sorted = reinterpret_cast<uint32_t *>(q); q += up(4 * n);
-      tb.ids = reinterpret_cast<int32_t *>(q); q += up(4 * n);
-      tb.order = oc.order;
-      q += up(4 * n);
-      tb.sort_tmp = q; tb.sort_tmp_bytes = tmp;
-      L.tile_order_plan = tb;
+      // scratch of the sort that follows the frame; the sorted order goes to the scene's table
+      if (plan_tile_order(ctx, L, P.local_tiles)) return 1;
+      L.tile_order_plan.order = oc.order;
     }
   }
   P.work_cursor = L.work_cursor;
@@ -476,6 +461,7 @@ int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d
   cudaError_t e = cudaMallocAsync(&img->dev, bytes ? bytes : 4, ctx->stream);
   if (e != cudaSuccess) { set_error(ctx, "render: cudaMallocAsync: %s", cudaGetErrorString(e)); delete img; return 1; }
   RenderParams P;
+  LaunchConfig lc;
   if (!ctx->peers.empty()) {  // single-process multi-GPU (RAY_GPUS > 1): api_multigpu.cu
     if (render_multi_device(ctx, img, h, w, spp, p)) { cudaFreeAsync(img->dev, ctx->stream); delete img; return 1; }
     *out0 = img;
@@ -483,7 +469,7 @@ int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d
   }
   // With a shard configured, the row-major frame only receives this rank's tiles; clear the rest.
   if (ctx->cfg.world > 1) cudaMemsetAsync(img->dev, 0, bytes, ctx->stream);
-  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, img->dev, nullptr, false, P) || do_render(ctx, P, 0, true, nullptr, p)) {
+  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, img->dev, nullptr, false, P, lc) || do_render(ctx, P, lc, 0, true, nullptr, p)) {
     cudaFreeAsync(img->dev, ctx->stream);
     delete img;
     return 1;
@@ -506,8 +492,9 @@ int ray_b200_render_into(struct futhark_context *ctx, int32_t *out_pix_dev, floa
   if (!ctx->peers.empty()) { set_error(ctx, "render_into: not available on a single-process multi-GPU context (RAY_GPUS > 1): only futhark_entry_render / ray_b200_entry_render_spp gather the helper devices' tiles"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
   RenderParams P;
-  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P)) return 1;
-  return do_render(ctx, P, 0, true, nullptr, p);
+  LaunchConfig lc;
+  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc)) return 1;
+  return do_render(ctx, P, lc, 0, true, nullptr, p);
 }
 
 int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, float *out_rgb_host, int64_t h, int64_t w, int32_t spp,
@@ -522,7 +509,8 @@ int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, flo
   CUDA_TRY(ctx, cudaMallocAsync(&d_pix, px * 4, ctx->stream));
   if (out_rgb_host) CUDA_TRY(ctx, cudaMallocAsync(&d_rgb, px * 12, ctx->stream));
   RenderParams P;
-  int rc = fill_params(ctx, p, h, w, spp, 0, 1, d_pix, d_rgb, false, P) || do_render(ctx, P, 0, true, nullptr, p);
+  LaunchConfig lc;
+  int rc = fill_params(ctx, p, h, w, spp, 0, 1, d_pix, d_rgb, false, P, lc) || do_render(ctx, P, lc, 0, true, nullptr, p);
   if (!rc) {
     if (cudaMemcpyAsync(out_pix_host, d_pix, px * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) rc = 1;
     if (!rc && d_rgb && cudaMemcpyAsync(out_rgb_host, d_rgb, px * 12, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) rc = 1;
@@ -550,12 +538,13 @@ int ray_b200_render_shard_into(struct futhark_context *ctx, int32_t *out_tiles_d
   if (!ctx->peers.empty()) { set_error(ctx, "render_shard_into: not available on a single-process multi-GPU context (RAY_GPUS > 1)"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
   RenderParams P;
-  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_tiles_dev, nullptr, true, P)) return 1;
+  LaunchConfig lc;
+  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_tiles_dev, nullptr, true, P, lc)) return 1;
   // ranks that own one tile fewer than the padded count leave a zeroed tail
   const int64_t padded = ray_b200_shard_tiles_padded(h, w, ctx->cfg.world);
   if (P.local_tiles < padded)
     CUDA_TRY(ctx, cudaMemsetAsync(out_tiles_dev + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4, ctx->stream));
-  return do_render(ctx, P, 0, true, nullptr, p);
+  return do_render(ctx, P, lc, 0, true, nullptr, p);
 }
 // Several frames in one call, up to two of them in flight: job i runs on lane i % 2, lane 1 forks from the context's
 // stream at the start of the call and joins it at the end, so for the caller the batch behaves like one stream-ordered
@@ -594,8 +583,9 @@ int ray_b200_render_batch(struct futhark_context *ctx, const struct ray_b200_ren
     const int lane = pipe ? (int)(ctx->lane_seq++ & 1u) : (two_lanes ? (i & 1) : 0);
     const int32_t spp = j.spp > 0 ? j.spp : ctx->cfg.spp;
     RenderParams P;
+    LaunchConfig lc;
     if (j.shard_layout) {
-      rc = fill_params(ctx, j.prepared, j.h, j.w, spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, nullptr, true, P);
+      rc = fill_params(ctx, j.prepared, j.h, j.w, spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, nullptr, true, P, lc);
       const int64_t padded = rc ? 0 : ray_b200_shard_tiles_padded(j.h, j.w, ctx->cfg.world);
       if (!rc && P.local_tiles < padded &&
           cudaMemsetAsync(j.out_dev + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4,
@@ -604,11 +594,11 @@ int ray_b200_render_batch(struct futhark_context *ctx, const struct ray_b200_ren
         rc = 1;
       }
     } else {
-      rc = fill_params(ctx, j.prepared, j.h, j.w, spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, j.out_rgb_dev, false, P);
+      rc = fill_params(ctx, j.prepared, j.h, j.w, spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, j.out_rgb_dev, false, P, lc);
     }
     FrameFlags ff;
     ff.wait_flag = j.wait_flag; ff.wait_value = j.wait_value; ff.done_flag = j.done_flag;
-    if (!rc) rc = do_render(ctx, P, lane, false, (ff.wait_flag || ff.done_flag) ? &ff : nullptr, j.prepared);
+    if (!rc) rc = do_render(ctx, P, lc, lane, false, (ff.wait_flag || ff.done_flag) ? &ff : nullptr, j.prepared);
   }
   // join even after a failure: whatever was enqueued on lane 1 must be ordered before later work on the context's stream
   // (pipelined submission: no join - the caller orders its reads, see ray_b200_context_set_pipeline)
@@ -749,7 +739,8 @@ int ray_b200_count_work(struct futhark_context *ctx, int64_t h, int64_t w, int32
   int32_t *scratch = nullptr;
   CUDA_TRY(ctx, cudaMallocAsync(&scratch, (size_t)h * w * 4, ctx->stream));
   RenderParams P;
-  int rc = fill_params(ctx, p, h, w, spp, 0, 1, scratch, nullptr, false, P);
+  LaunchConfig lc;
+  int rc = fill_params(ctx, p, h, w, spp, 0, 1, scratch, nullptr, false, P, lc);
   if (!rc) {
     cudaMemsetAsync(ctx->counters, 0, 4 * sizeof(unsigned long long), ctx->stream);
     launch_count_work(P, ctx->stream, &ctx->launches);

@@ -548,8 +548,6 @@ __global__ void wavefront_sort_keys_kernel(const __grid_constant__ RenderParams 
 
 }  // namespace
 
-bool alt_kernels_built() { return true; }
-
 size_t wavefront_sort_bytes(int64_t items) {
   size_t bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const int32_t *)nullptr,
@@ -569,11 +567,6 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
     const long long max_useful = (items + 31) / 32;
     if (want > max_useful) want = max_useful;
     const int tail = wf->tail_from < 0 ? 0 : (wf->tail_from > kMaxDepth - 1 ? kMaxDepth - 1 : wf->tail_from);
-#define RAYB200_WF(A, S)                                                                          \
-  do {                                                                                            \
-    e = opt_in_dynamic_smem<wavefront_bounce_kernel<A, S>>(lc.max_dynamic_smem);                  \
-    if (e == cudaSuccess) wavefront_bounce_kernel<A, S><<<(unsigned)want, threads, smem, stream>>>(p, *wf, b, s, rte, use_order); \
-  } while (0)
     for (int s = 0; s < p.spp && e == cudaSuccess; s++) {
       cudaMemsetAsync(wf->qlen, 0, 2 * (kMaxDepth + 2) * sizeof(int32_t), stream);  // qlen and cursor are contiguous
       for (int b = 0; b <= tail && e == cudaSuccess; b++) {
@@ -586,18 +579,17 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
                                           (int)wf->capacity, 0, 32, stream);
           (*launches) += 2;
         }
-        if (all_nodes && sph) RAYB200_WF(true, true);
-        else if (all_nodes) RAYB200_WF(true, false);
-        else if (sph) RAYB200_WF(false, true);
-        else RAYB200_WF(false, false);
+        e = with_flags([&](auto a, auto spheres) {  // (s is the sample pass)
+          return launch_opted_in<wavefront_bounce_kernel<a, spheres>>(lc.max_dynamic_smem, (unsigned)want, threads, smem,
+                                                                      stream, p, *wf, b, s, rte, use_order);
+        }, all_nodes, sph);
         (*launches)++;
       }
     }
-#undef RAYB200_WF
     return e;
   }
   if (lc.kernel == 5) {  // RAY_B200_KERNEL_STREAMQUEUE: one CTA per SM, rays refilled continuously (no rounds); 32 rays per warp
-    const int k = 1;
+    constexpr int k = 1;
     const int wthreads = 32 * lc.wq_warps;
     const int ncap = wq_node_capacity(k, p.max_depth);
     const size_t wsmem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * sq_warp_bytes(k, ncap);
@@ -606,21 +598,10 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
     const long long rays = items * (spread ? (long long)p.spp : 1ll);
     const long long useful = (rays + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
     if (ctas > useful) ctas = useful;
-#define RAYB200_SQ(KK, SP, A, S)                                                                                   \
-  do {                                                                                                             \
-    e = opt_in_dynamic_smem<render_streamqueue_kernel<KK, SP, A, S>>(lc.max_dynamic_smem);                         \
-    if (e == cudaSuccess) render_streamqueue_kernel<KK, SP, A, S><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, lc.wq_refill); \
-  } while (0)
-#define RAYB200_SQ2(KK, SP)                                                               \
-  do {                                                                                    \
-    if (all_nodes && sph) RAYB200_SQ(KK, SP, true, true);                                 \
-    else if (all_nodes) RAYB200_SQ(KK, SP, true, false);                                  \
-    else if (sph) RAYB200_SQ(KK, SP, false, true);                                        \
-    else RAYB200_SQ(KK, SP, false, false);                                                \
-  } while (0)
-    if (spread) RAYB200_SQ2(1, true); else RAYB200_SQ2(1, false);
-#undef RAYB200_SQ2
-#undef RAYB200_SQ
+    e = with_flags([&](auto sp, auto a, auto s) {
+      return launch_opted_in<render_streamqueue_kernel<k, sp, a, s>>(lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem,
+                                                                     stream, p, ncap, lc.wq_refill);
+    }, spread, all_nodes, sph);
     if (e == cudaSuccess) (*launches)++;
     return e;
   }
@@ -629,22 +610,14 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
   const long long max_useful = (items + threads - 1) / threads;
   if (want > max_useful) want = max_useful;
   const int refill = lc.refill_min < 1 ? 1 : (lc.refill_min > 32 ? 32 : lc.refill_min);
-#define RAYB200_PS(A, S)                                                                          \
-  do {                                                                                            \
-    e = opt_in_dynamic_smem<render_persistent_kernel<A, S>>(lc.max_dynamic_smem);                 \
-    if (e == cudaSuccess) render_persistent_kernel<A, S><<<(unsigned)want, threads, smem, stream>>>(p, refill); \
-  } while (0)
-  if (all_nodes && sph) RAYB200_PS(true, true);
-  else if (all_nodes) RAYB200_PS(true, false);
-  else if (sph) RAYB200_PS(false, true);
-  else RAYB200_PS(false, false);
-#undef RAYB200_PS
+  e = with_flags([&](auto a, auto s) {
+    return launch_opted_in<render_persistent_kernel<a, s>>(lc.max_dynamic_smem, (unsigned)want, threads, smem, stream, p, refill);
+  }, all_nodes, sph);
   if (e == cudaSuccess) (*launches)++;
   return e;
 }
 #else   // product build: the alternatives are not compiled in
 
-bool alt_kernels_built() { return false; }
 size_t wavefront_sort_bytes(int64_t) { return 0; }
 
 cudaError_t launch_alt_kernel(const RenderParams &, const LaunchConfig &, const WavefrontBuffers *, cudaStream_t, int64_t *) {

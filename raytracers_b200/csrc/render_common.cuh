@@ -370,6 +370,25 @@ cudaError_t opt_in_dynamic_smem(int max_dynamic_smem) {
   return e;
 }
 
+// Variant dispatch of the host launchers: with_flags(f, b0, b1, ...) calls f(std::bool_constant<b0>{}, ...), so run-time
+// flags pick compile-time template arguments.  f is instantiated for every combination of the flags passed, so a
+// launcher passes only axes whose combinations all exist (K3's ray-mode axes are dispatched apart from its pixel axes).
+template <class F>
+cudaError_t with_flags(F &&f) { return f(); }
+template <class F, class... B>
+cudaError_t with_flags(F &&f, bool b, B... rest) {
+  if (b) return with_flags([&](auto... c) { return f(std::true_type{}, c...); }, rest...);
+  return with_flags([&](auto... c) { return f(std::false_type{}, c...); }, rest...);
+}
+
+// Opts Kern in to the device's dynamic shared memory on first use, then launches it.
+template <auto Kern, class... Args>
+cudaError_t launch_opted_in(int max_dynamic_smem, unsigned grid, int block, size_t smem, cudaStream_t stream, const Args &...args) {
+  const cudaError_t e = opt_in_dynamic_smem<Kern>(max_dynamic_smem);
+  if (e == cudaSuccess) Kern<<<grid, block, smem, stream>>>(args...);
+  return e;
+}
+
 }  // namespace
 
 }  // namespace rayb200

@@ -750,8 +750,10 @@ __global__ void detile_kernel(const int32_t *__restrict__ gathered, int32_t *__r
 }  // namespace
 
 // ---------------------------------------------------------------------------------------- host launchers
-// Kernels opt in to > 48 KB of dynamic shared memory on first use (opt_in_dynamic_smem), not at context creation:
-// futhark_context_new no longer touches ~50 template instantiations it will never launch.
+// Each launcher takes the plan of its frame or query (LaunchConfig: fill_params or the ray-query entry points make it),
+// derives the launch geometry once and picks the template instantiation with with_flags (render_common.cuh).  Kernels
+// opt in to > 48 KB of dynamic shared memory on first use (launch_opted_in), not at context creation:
+// futhark_context_new does not touch the ~50 template instantiations it will never launch.
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches) {
   const long long items = p.local_tiles * kTilePixels;
@@ -765,102 +767,59 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   }
   if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
   if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  // RAY_B200_KERNEL_WARPQUEUE: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp
+  return launch_warpqueue(p, RayQuery{}, lc, stream, launches);                   // RAY_B200_KERNEL_WARPQUEUE
+}
+
+// K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query when q.rays is set:
+// the same kernel in ray mode, without spread samples or packets, closest hit / path or (q.occluded set) any hit.
+cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
+                             int64_t *launches) {
+  const bool rays = q.rays != nullptr;
+  const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
+  // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
+  // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
+  const long long work = rays ? (long long)q.n : p.local_tiles * kTilePixels * (spread ? (long long)p.spp : 1ll);
+  if (work <= 0) return cudaSuccess;
   const bool all_nodes = p.smem_nodes == p.n_inner, sph = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
   const int k = lc.wq_k == 1 ? 1 : 2;
   const int wthreads = 32 * lc.wq_warps;
   const int ncap = wq_node_capacity(k, p.max_depth, lc.wq_ncap);
-  const bool packet = lc.wq_packet > 0;
   // breadth-first below this many queued node items (0 = half the ring, < 0 = never: plain LIFO)
   const int nring = 1 << (31 - __builtin_clz((unsigned)ncap));
   const int nlow = lc.wq_low < 0 ? 0 : (lc.wq_low == 0 ? nring / 2 : (lc.wq_low > nring - 96 ? nring - 96 : lc.wq_low));
-  const size_t wsmem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * wq_warp_bytes(k, ncap, packet, p.sample_buf != nullptr);
+  const size_t wsmem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * wq_warp_bytes(k, ncap, packet, spread);
   long long ctas = lc.sm_count;
-  const bool spread = p.sample_buf != nullptr;
-  // no more CTAs than there are rays to start at once: a slot takes one SAMPLE when samples are spread, one pixel
-  // otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
-  const long long rays = items * (spread ? (long long)p.spp : 1ll);
-  const long long useful = (rays + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
+  const long long useful = (work + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
   if (ctas > useful) ctas = useful;
-  cudaError_t e = cudaSuccess;
-  const RayQuery no_rays{};
-#define RAYB200_WQ(KK, SP, PK, A, S)                                                                                        \
-  do {                                                                                                                      \
-    e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, SP, PK, A, S>>(lc.max_dynamic_smem);                                \
-    if (e == cudaSuccess)                                                                                                   \
-      render_warpqueue_kernel<KK, SP, PK, A, S><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, lc.wq_packet, lc.wq_refill, nlow, no_rays); \
-  } while (0)
-#define RAYB200_WQ2(KK, SP, PK)                                                           \
-  do {                                                                                    \
-    if (all_nodes && sph) RAYB200_WQ(KK, SP, PK, true, true);                             \
-    else if (all_nodes) RAYB200_WQ(KK, SP, PK, true, false);                              \
-    else if (sph) RAYB200_WQ(KK, SP, PK, false, true);                                    \
-    else RAYB200_WQ(KK, SP, PK, false, false);                                            \
-  } while (0)
-#define RAYB200_WQ3(KK, SP)                                                               \
-  do {                                                                                    \
-    if (packet) RAYB200_WQ2(KK, SP, true); else RAYB200_WQ2(KK, SP, false);               \
-  } while (0)
-  if (k == 1) { if (spread) RAYB200_WQ3(1, true); else RAYB200_WQ3(1, false); }
-  else { if (spread) RAYB200_WQ3(2, true); else RAYB200_WQ3(2, false); }
-#undef RAYB200_WQ3
-#undef RAYB200_WQ2
-#undef RAYB200_WQ
-  if (e == cudaSuccess) (*launches)++;
-  return e;
-}
-
-// Ray queries: the same kernel in ray mode, one CTA per SM (fewer for small batches), planned like a pixel frame
-// without spread samples or packets.  The four variants per K and query kind (closest hit / path, or any hit) are loaded
-// on first use.
-cudaError_t launch_rays(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches) {
-  if (q.n <= 0) return cudaSuccess;
-  const bool all_nodes = p.smem_nodes == p.n_inner, sph = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
-  const bool any_hit = q.occluded != nullptr;
-  const int k = lc.wq_k == 1 ? 1 : 2;
-  const int wthreads = 32 * lc.wq_warps;
-  const int ncap = wq_node_capacity(k, p.max_depth, lc.wq_ncap);
-  const int nring = 1 << (31 - __builtin_clz((unsigned)ncap));
-  const int nlow = lc.wq_low < 0 ? 0 : (lc.wq_low == 0 ? nring / 2 : (lc.wq_low > nring - 96 ? nring - 96 : lc.wq_low));
-  const size_t wsmem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * wq_warp_bytes(k, ncap, false, false);
-  long long ctas = lc.sm_count;
-  const long long useful = ((long long)q.n + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
-  if (ctas > useful) ctas = useful;
-  cudaError_t e = cudaSuccess;
-#define RAYB200_WQR(KK, A, S, AH)                                                                                          \
-  do {                                                                                                                     \
-    e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, false, false, A, S, true, AH>>(lc.max_dynamic_smem);               \
-    if (e == cudaSuccess)                                                                                                  \
-      render_warpqueue_kernel<KK, false, false, A, S, true, AH><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, ncap, 0, 1, nlow, q); \
-  } while (0)
-#define RAYB200_WQR2(KK, AH)                                                                                               \
-  do {                                                                                                                     \
-    if (all_nodes && sph) RAYB200_WQR(KK, true, true, AH);                                                                 \
-    else if (all_nodes) RAYB200_WQR(KK, true, false, AH);                                                                  \
-    else if (sph) RAYB200_WQR(KK, false, true, AH);                                                                        \
-    else RAYB200_WQR(KK, false, false, AH);                                                                                \
-  } while (0)
-  if (any_hit) { if (k == 1) RAYB200_WQR2(1, true); else RAYB200_WQR2(2, true); }
-  else { if (k == 1) RAYB200_WQR2(1, false); else RAYB200_WQR2(2, false); }
-#undef RAYB200_WQR2
-#undef RAYB200_WQR
+  cudaError_t e;
+  if (rays)
+    e = with_flags([&](auto k2, auto any_hit, auto a, auto s) {
+      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, true, any_hit>>(
+          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
+    }, k == 2, q.occluded != nullptr, all_nodes, sph);
+  else
+    e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
+      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s>>(
+          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
+    }, k == 2, spread, packet, all_nodes, sph);
   if (e == cudaSuccess) (*launches)++;
   return e;
 }
 
 // Loads (and opts in to shared memory) the variants the default plan uses - K = 1 / 2, samples spread or not, and the three
 // staging cases: whole scene staged, tree partly staged with / without the packet walk - so that the first timed frame of
-// main.c does not pay CUDA's lazy function loading.  12 of the 32 instantiations, loaded once per process at context
-// creation instead of all kernels of all builds.
+// main.c does not pay CUDA's lazy function loading.  12 of the 32 pixel instantiations, loaded once per process at
+// context creation instead of all kernels of all builds.
 cudaError_t preload_default_kernels(int max_dynamic_smem) {
+  const bool staging[3][3] = {{false, true, true}, {true, false, false}, {false, false, false}};  // packet, all nodes, spheres
   cudaError_t e = cudaSuccess;
-#define RAYB200_PRE(KK, SP, PK, A, S) \
-  if (e == cudaSuccess) e = opt_in_dynamic_smem<render_warpqueue_kernel<KK, SP, PK, A, S>>(max_dynamic_smem)
-#define RAYB200_PRE3(KK, SP) \
-  RAYB200_PRE(KK, SP, false, true, true); RAYB200_PRE(KK, SP, true, false, false); RAYB200_PRE(KK, SP, false, false, false)
-  RAYB200_PRE3(1, false); RAYB200_PRE3(1, true); RAYB200_PRE3(2, false); RAYB200_PRE3(2, true);
-#undef RAYB200_PRE3
-#undef RAYB200_PRE
+  for (int k2 = 0; k2 < 2; k2++)
+    for (int spread = 0; spread < 2; spread++)
+      for (const auto &c : staging)
+        if (e == cudaSuccess)
+          e = with_flags([&](auto kk2, auto sp, auto pk, auto a, auto s) {
+            return opt_in_dynamic_smem<render_warpqueue_kernel<kk2 ? 2 : 1, sp, pk, a, s>>(max_dynamic_smem);
+          }, k2 == 1, spread == 1, c[0], c[1], c[2]);
   return e;
 }
 

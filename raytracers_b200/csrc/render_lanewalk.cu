@@ -386,31 +386,17 @@ cudaError_t launch_lanewalk(const RenderParams &p, const LaunchConfig &lc, cudaS
   if (ctas > useful) ctas = useful;
   const int idle_min = lc.lw_idle_min < 1 ? 1 : (lc.lw_idle_min > 32 ? 32 : lc.lw_idle_min);
   const int max_pass = lc.lw_passes < 1 ? 1 : lc.lw_passes;
-  cudaError_t e = cudaSuccess;
-#define RAYB200_LW(RR, SP, A, S)                                                                                     \
-  do {                                                                                                               \
-    e = opt_in_dynamic_smem<render_lanewalk_kernel<RR, SP, A, S>>(lc.max_dynamic_smem);                              \
-    if (e == cudaSuccess)                                                                                            \
-      render_lanewalk_kernel<RR, SP, A, S><<<(unsigned)ctas, wthreads, wsmem, stream>>>(p, scap, idle_min, max_pass); \
-  } while (0)
-#define RAYB200_LW2(RR, SP)                               \
-  do {                                                    \
-    if (all_nodes && sph) RAYB200_LW(RR, SP, true, true); \
-    else if (all_nodes) RAYB200_LW(RR, SP, true, false);  \
-    else if (sph) RAYB200_LW(RR, SP, false, true);        \
-    else RAYB200_LW(RR, SP, false, false);                \
-  } while (0)
-#define RAYB200_LW3(RR)                                   \
-  do {                                                    \
-    if (spread) RAYB200_LW2(RR, true); else RAYB200_LW2(RR, false); \
-  } while (0)
-  if (lc.lw_slots == 64) RAYB200_LW3(64);
-  else if (lc.lw_slots == 48) RAYB200_LW3(48);
-  else if (lc.lw_slots == 32) RAYB200_LW3(32);
+  const auto with_slots = [&](auto slots) {  // the slot counts that are built: 32, 48, 64
+    return with_flags([&](auto sp, auto a, auto s) {
+      return launch_opted_in<render_lanewalk_kernel<decltype(slots)::value, sp, a, s>>(
+          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, scap, idle_min, max_pass);
+    }, spread, all_nodes, sph);
+  };
+  cudaError_t e;
+  if (lc.lw_slots == 64) e = with_slots(std::integral_constant<int, 64>{});
+  else if (lc.lw_slots == 48) e = with_slots(std::integral_constant<int, 48>{});
+  else if (lc.lw_slots == 32) e = with_slots(std::integral_constant<int, 32>{});
   else return cudaErrorInvalidValue;
-#undef RAYB200_LW3
-#undef RAYB200_LW2
-#undef RAYB200_LW
   if (e == cudaSuccess) (*launches)++;
   return e;
 }

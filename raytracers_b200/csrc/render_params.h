@@ -93,16 +93,16 @@ struct WavefrontBuffers {
 };
 size_t wavefront_sort_bytes(int64_t items);  // cub temp storage for the re-sort (0 in builds without the alternative kernels)
 
+// The launch plan of one frame or ray query: fill_params returns it next to the RenderParams (trace() in api_rays.cu makes
+// the ray queries'), and the launcher of its kernel reads only the fields that kernel uses.
 struct LaunchConfig {
   int kernel;          // ray_b200_kernel
   int blocks_per_sm;
   int sm_count;
-  int smem_budget;     // bytes of dynamic shared memory per CTA for BVH staging
   int refill_min;      // persistent kernel: refill when at least this many lanes are idle
-  int tail_from;       // wavefront: see WavefrontBuffers
-  int wq_warps;        // warp-queue kernel: warps per CTA (one CTA per SM)
+  int wq_warps;        // warp-queue / stream-queue / lane-walk kernels: warps per CTA (one CTA per SM)
   int wq_k;            // warp-queue kernel: rays in flight per warp = 32 * wq_k (1 or 2)
-  int wq_refill;       // warp-queue kernel, spread mode: hand out samples when at least this many slots are idle
+  int wq_refill;       // warp-queue / stream-queue kernels, spread mode: hand out samples when at least this many slots are idle
   int wq_low;          // warp-queue kernel: node batches take the OLDEST queued items while at most this many are queued (0 = half the ring, < 0 = never)
   int wq_packet;       // warp-queue kernel: node steps with at least this many lanes are done packet-style (0 = never)
   int wq_ncap;         // warp-queue kernel: cap on the node-queue capacity (0 = the proved bound, at most 1024)
@@ -112,16 +112,17 @@ struct LaunchConfig {
   int max_dynamic_smem;  // the device's opt-in shared-memory limit (kernels opt in on first launch)
 };
 
+// A frame on the kernel lc.kernel names (render_kernels.cu)
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches);
-// Ray queries: the warp-queue kernel in ray mode (render_kernels.cu), whatever lc.kernel says
-cudaError_t launch_rays(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches);
+// The warp-queue kernel (render_kernels.cu): a pixel frame, or a ray query when q.rays != NULL (whatever lc.kernel says)
+cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
+                             int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
 // build without RAYB200_ALL_KERNELS returns cudaErrorNotSupported)
 cudaError_t launch_lanewalk(const RenderParams &p, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches);
 cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                               int64_t *launches);
-bool alt_kernels_built();
 cudaError_t preload_default_kernels(int max_dynamic_smem);  // render_kernels.cu: the variants of the default plan
 // Probe pass + sort that produce RenderParams::tile_order (see render_kernels.cu).  All buffers are device memory.
 struct TileOrderBuffers {

@@ -5,9 +5,9 @@
 
 cuobjdump -sass of both files, split into functions, names demangled.  A function of OLD must exist in NEW with the
 same instructions and encodings.  The any-hit template parameter of the warp-queue kernel (kAnyHit, default false)
-only changes the symbol names of the pixel and the closest-hit / path instantiations; it is mapped back before the
-comparison, so OLD is a build that has ray mode (kRays) but no any-hit variants.  Functions that exist in NEW only are
-listed.  Exit code 0 = every function of OLD is identical.
+only changes the symbol names of the pixel and the closest-hit / path instantiations; it is mapped out of the names of
+both builds before the comparison, so OLD may be a build from before or after the any-hit variants (it needs ray mode,
+kRays).  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
 """
 import collections
 import re
@@ -48,11 +48,10 @@ def normalise(name):
 
 
 def main():
-    old, new = functions(sys.argv[1]), functions(sys.argv[2])
-    new_n = collections.OrderedDict(((normalise(n), i), b) for (n, i), b in new.items())
+    old, new = ({(normalise(n), i): b for (n, i), b in functions(path).items()} for path in sys.argv[1:3])
     bad = 0
     for key, body in old.items():
-        other = new_n.get(key)
+        other = new.get(key)
         if other is None:
             print(f"MISSING  {key[0]}")
             bad += 1
@@ -60,7 +59,7 @@ def main():
             diff = sum(a != b for a, b in zip(body, other)) + abs(len(body) - len(other))
             print(f"DIFFERS  {key[0]}  ({len(body)} -> {len(other)} lines, {diff} differ)")
             bad += 1
-    added = [n for (n, _) in new_n if (n, 1) not in old]
+    added = [n for (n, _) in new if (n, 1) not in old]
     print(f"{len(old)} functions compared, {bad} not identical; {len(added)} new:")
     for n in added:
         print(f"NEW      {n}")
