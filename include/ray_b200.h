@@ -23,8 +23,8 @@
  * At spp = 1 this is bit-identical to the reference's render.
  *
  * Ray queries ("ray queries" below): rays the caller made are traced against a prepared scene to their closest hit
- * (objs_hit), along their path (ray_colour), bit for bit, or to their first accepted sphere (occlusion), by the same
- * warp-queue kernel in ray mode.
+ * (objs_hit), along their path (ray_colour), bit for bit, to their first accepted sphere (occlusion), or to the k
+ * nearest of their accepted spheres (multi-hit), by the same warp-queue kernel in ray mode.
  */
 #ifndef RAY_B200_EXT_H
 #define RAY_B200_EXT_H
@@ -161,6 +161,23 @@ int ray_b200_trace_paths(struct futhark_context *ctx, const struct futhark_opaqu
  * target - origin (not normalised), and an interval such as (1e-4, 1 - 1e-4), which excludes both end points. */
 int ray_b200_trace_occluded(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
                             const float *rays_dev, int64_t n, float t_min, float t_max, uint8_t *occluded_dev);
+/* Multi-hit (transparency layers, depth complexity, line-of-sight lists): A(r) = the leaves the reference's bvh_fold
+ * (bvh.fut:61-84) reaches, boxes tested against (t_min, t_max) as objs_hit tests them, whose sphere_hit L[i] r t_min
+ * t_max (ray.fut:32-51) is a hit, each with its t (root1 if it lies in the interval, else root2).  As in
+ * ray_b200_trace_occluded there is no epsilon 0.1 and no re-intersection, and a sphere gives at most one record, its
+ * first intersection in the interval.  A(r) is ordered by ascending t, then ascending Morton-sorted leaf (coincident
+ * identical spheres: ascending caller index).  hits_dev[i][j], j < min(k, |A(r)|): the j-th member as struct
+ * ray_b200_hit, t, sphere, p and normal made as ray_b200_trace_hits makes them; the remaining records are t = -1,
+ * sphere = -1, p = normal = 0.  counts_dev[i] = |A(r)|, not capped at k.  The set of reached leaves does not depend
+ * on traversal order, so neither do the records nor the count.  Two identities hold exactly:
+ *   counts_dev[i] > 0  ==  ray_b200_trace_occluded(t_min, t_max) for every ray;
+ *   at t_min = 0.1, record 0 == the ray_b200_trace_hits(0.1, t_max) record, all 8 words, for every ray whose closest
+ *   hit has t < 2^24.
+ * hits_dev: device struct ray_b200_hit[n][k] (record offsets are 64-bit: n * k may pass 2^32); counts_dev: device
+ * int32[n] or NULL.  Further errors: k outside [1, 64]. */
+int ray_b200_trace_multi_hits(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                              const float *rays_dev, int64_t n, float t_min, float t_max, int32_t k,
+                              struct ray_b200_hit *hits_dev, int32_t *counts_dev);
 /* sizeof(struct ray_b200_hit) as the library was compiled (32). */
 int64_t ray_b200_hit_size(void);
 

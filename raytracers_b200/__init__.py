@@ -147,6 +147,7 @@ def load_library(variant=""):
         "ray_b200_trace_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
         "ray_b200_trace_paths": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
         "ray_b200_trace_occluded": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
+        "ray_b200_trace_multi_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, i32, vp, vp]),
         "ray_b200_hit_size": (i64, []),
         "ray_b200_count_work": (C.c_int, [vp, i64, i64, i32, vp, C.POINTER(WorkCounters)]),
         "ray_b200_ipc_alloc": (C.c_int, [vp, i64, pp, vp]),
@@ -630,6 +631,14 @@ class Context:
         self._check(self.lib.ray_b200_trace_occluded(self.handle, prepared.handle, _ptr(rays_dev), int(n), float(t_min),
                                                      float(t_max), _ptr(out_dev)))
 
+    def trace_multi_hits_into(self, rays_dev, n, prepared, k, hits_dev, counts_dev=None, t_min=0.0, t_max=1e9):
+        """The k nearest sphere intersections of n rays in (t_min, t_max): hits_dev = device Hit[n][k], in ascending t
+        (then Morton-sorted leaf), empty records (t = -1, sphere = -1) after the last; counts_dev = device int32[n]
+        (or None) = every sphere the BVH walk reaches that is hit in the interval, not capped at k.  No epsilon, one
+        record per sphere.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_trace_multi_hits(self.handle, prepared.handle, _ptr(rays_dev), int(n), float(t_min),
+                                                       float(t_max), int(k), _ptr(hits_dev), _ptr(counts_dev)))
+
     def _rays_tensor(self, rays):
         import torch
         if not isinstance(rays, torch.Tensor) or rays.device.type != "cuda" or rays.device.index != self.device:
@@ -671,6 +680,19 @@ class Context:
         self.trace_occluded_into(rays.data_ptr(), n, prepared, out.data_ptr(), t_min=t_min, t_max=t_max)
         self.sync()
         return out
+
+    def trace_multi_hits(self, prepared, rays, k, t_min=0.0, t_max=1e9):
+        """The k nearest sphere intersections of a [n, 6] float32 CUDA tensor of rays.  Returns dict(t [n, k],
+        sphere [n, k] int32, p [n, k, 3], normal [n, k, 3], count [n] int32): the first four are views of one [n, k, 8]
+        buffer of Hit records.  Waits for torch's current stream before, and synchronises the context after the query."""
+        torch = self._rays_tensor(rays)
+        n = rays.shape[0]
+        buf = torch.empty((n, int(k), 8), dtype=torch.float32, device=rays.device)
+        count = torch.empty((n,), dtype=torch.int32, device=rays.device)
+        self.trace_multi_hits_into(rays.data_ptr(), n, prepared, k, buf.data_ptr(), count.data_ptr(), t_min=t_min, t_max=t_max)
+        self.sync()
+        return {"t": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "p": buf[..., 2:5], "normal": buf[..., 5:8],
+                "count": count}
 
     def count_work(self, h, w, prepared, spp=1):
         wc = WorkCounters()

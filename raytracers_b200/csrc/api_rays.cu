@@ -1,6 +1,7 @@
 // C ABI, part 5: ray queries (include/ray_b200.h "ray queries") - caller-supplied rays traced against a prepared scene
 // by the warp-queue kernel in ray mode (render_kernels.cu), either to their closest hit (objs_hit), along their whole
-// path (ray_colour), or to their first accepted sphere (occlusion, the any-hit instantiations).
+// path (ray_colour), to their first accepted sphere (occlusion, the any-hit instantiations), or to the k nearest of
+// their accepted spheres (multi-hit, the multi-hit instantiations).
 #include "api_internal.h"
 
 #include <cmath>
@@ -11,10 +12,11 @@ static_assert(sizeof(struct ray_b200_hit) == 32, "struct ray_b200_hit is 32 byte
 
 namespace {
 
-// Validates, plans and enqueues one query on the context's stream (lane 0).  hits != NULL: hit query, occluded != NULL:
-// occlusion query, else path query.
+// Validates, plans and enqueues one query on the context's stream (lane 0).  multi: multi-hit query of k records per ray
+// into hits (and counts, optional), else hits != NULL: hit query, occluded != NULL: occlusion query, else path query.
 int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const float *rays, int64_t n, float t_min, float t_max,
-          int32_t max_depth, ray_b200_hit *hits, float *rgb, int32_t *segments, uint8_t *occluded, const char *what) {
+          int32_t max_depth, ray_b200_hit *hits, float *rgb, int32_t *segments, uint8_t *occluded, bool multi, int32_t k,
+          int32_t *counts, const char *what) {
   if (bad_ctx(ctx)) return 1;
   std::lock_guard<std::mutex> g(ctx->mu);
   if (n < 0 || n > ((int64_t)1 << 30)) { set_error(ctx, "%s: n = %lld is outside [0, 2^30]", what, (long long)n); return 1; }
@@ -23,6 +25,7 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const fl
     return 1;
   }
   if (max_depth < 0 || max_depth > 65535) { set_error(ctx, "%s: max_depth %d is outside [0, 65535]", what, max_depth); return 1; }
+  if (multi && (k < 1 || k > 64)) { set_error(ctx, "%s: k = %d is outside [1, 64]", what, k); return 1; }
   if (n == 0) return 0;
   if (!rays || (!hits && !rgb && !occluded)) { set_error(ctx, "%s: NULL device buffer", what); return 1; }
   if (!p || !p->dev.nodes || !p->dev.perm) { set_error(ctx, "%s: invalid prepared scene", what); return 1; }
@@ -52,6 +55,8 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, const fl
     Q.t_max = one_segment ? t_max : 1000000000.0f;
     Q.max_depth = one_segment ? 1 : max_depth;
     Q.occluded = occluded;
+    Q.k = multi ? k : 0;
+    Q.counts = multi ? counts : nullptr;
     CUDA_TRY(ctx, cudaMemsetAsync(L.work_cursor, 0, 2 * sizeof(int32_t), L.stream));
     CUDA_TRY(ctx, launch_warpqueue(P, Q, lc, L.stream, &ctx->launches));
     CUDA_TRY(ctx, cudaGetLastError());
@@ -71,17 +76,24 @@ extern "C" {
 
 int ray_b200_trace_hits(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev, int64_t n,
                         float t_min, float t_max, struct ray_b200_hit *hits_dev) {
-  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, hits_dev, nullptr, nullptr, nullptr, "trace_hits");
+  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, hits_dev, nullptr, nullptr, nullptr, false, 0, nullptr, "trace_hits");
 }
 
 int ray_b200_trace_paths(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev, int64_t n,
                          int32_t max_depth, float *rgb_dev, int32_t *segments_dev) {
-  return trace(ctx, p, rays_dev, n, 0.0f, 1000000000.0f, max_depth, nullptr, rgb_dev, segments_dev, nullptr, "trace_paths");
+  return trace(ctx, p, rays_dev, n, 0.0f, 1000000000.0f, max_depth, nullptr, rgb_dev, segments_dev, nullptr, false, 0, nullptr,
+               "trace_paths");
 }
 
 int ray_b200_trace_occluded(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev,
                             int64_t n, float t_min, float t_max, uint8_t *occluded_dev) {
-  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, nullptr, nullptr, nullptr, occluded_dev, "trace_occluded");
+  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, nullptr, nullptr, nullptr, occluded_dev, false, 0, nullptr,
+               "trace_occluded");
+}
+
+int ray_b200_trace_multi_hits(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, const float *rays_dev,
+                              int64_t n, float t_min, float t_max, int32_t k, struct ray_b200_hit *hits_dev, int32_t *counts_dev) {
+  return trace(ctx, p, rays_dev, n, t_min, t_max, 1, hits_dev, nullptr, nullptr, nullptr, true, k, counts_dev, "trace_multi_hits");
 }
 
 int64_t ray_b200_hit_size(void) { return (int64_t)sizeof(struct ray_b200_hit); }

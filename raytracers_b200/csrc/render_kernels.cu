@@ -138,6 +138,17 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // queue bounds and the overflow guard hold as they are.  The owner lane writes Q.occluded and frees the slot.
 // Queue discipline of these instantiations: node batches as in the other instantiations, leaf batches from
 // kAnyHitLeafMin items on.
+//
+// Multi-hit ray mode (kMultiHit, a multi-hit query): one segment whose answer is every leaf the boxes admit whose sphere
+// accepts in (t_min, t_max), as the keys bits(t) << 32 | leaf (t >= 0, so bit order is numeric order), of which the Q.k
+// smallest are kept and all are counted.  The set of reached leaves does not depend on the order of the items, and
+// neither do its k smallest keys nor its size.  The list lives in the ray's own k output records (words 0 and 1 of record
+// j = the j-th smallest key so far, sorted); best_t[slot] counts the accepted leaves.  A hit moves the larger keys up one
+// record and drops the k-th when the list is full, so a key above the k-th costs one compare.  Lanes of a leaf batch
+// that hit the same slot insert one at a time (one lane per slot per round, __syncwarp between rounds); slots are
+// warp-private and a ray is claimed once, so no other warp touches the list.  Node batches are those of the closest-hit
+// instantiations: no box is pruned by the k-th t, because the count needs the whole set.  The owner lane turns the keys
+// into hit records (sphere through Q.perm), fills the rest with empty records, writes Q.counts and frees the slot.
 
 // any-hit instantiations: a leaf batch runs as soon as this many leaf items are queued (the other instantiations wait
 // for 32, a full batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured
@@ -148,12 +159,15 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, bool kRays = false, bool kAnyHit = false>
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, bool kRays = false, bool kAnyHit = false,
+          bool kMultiHit = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without the packet walk");
   static_assert(!kAnyHit || kRays, "the any-hit variant is a ray-mode query");
+  static_assert(!kMultiHit || kRays, "the multi-hit variant is a ray-mode query");
+  static_assert(!(kMultiHit && kAnyHit), "a query is either any-hit or multi-hit");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -260,6 +274,63 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     h[0] = t; h[1] = __int_as_float(sphere);
     h[2] = p.x; h[3] = p.y; h[4] = p.z;
     h[5] = n.x; h[6] = n.y; h[7] = n.z;
+    p_item[slot] = -1;
+  };
+  // multi-hit query: the ray's Q.k records (64-bit offsets: n * k records pass 4 GiB)
+  [[maybe_unused]] auto multi_records = [&](const int slot) {
+    return reinterpret_cast<uint32_t *>(Q.hits) + (size_t)p_item[slot] * (size_t)Q.k * 8;
+  };
+  // multi-hit query, one lane per slot at a time: inserts the key (tb, li) into the slot's sorted list of its smallest
+  // keys and counts it.  Keys are unique (a ray reaches a leaf once), so the comparisons are strict.
+  [[maybe_unused]] auto insert_hit = [&](const int slot, const uint32_t tb, const uint32_t li) {
+    const int k = Q.k;
+    const uint32_t c = best_t[slot];
+    best_t[slot] = c + 1u;
+    uint32_t *h = multi_records(slot);
+    int j = c < (uint32_t)k ? (int)c : k;  // the key goes to record j, once every larger key has moved up
+    for (; j > 0; j--) {
+      const uint32_t pt = h[8 * (j - 1)], pl = h[8 * (j - 1) + 1];
+      if (pt < tb || (pt == tb && pl < li)) break;
+      if (j < k) { h[8 * j] = pt; h[8 * j + 1] = pl; }
+    }
+    if (j < k) { h[8 * j] = tb; h[8 * j + 1] = li; }
+  };
+  // multi-hit query, owner lane: the first min(count, k) records hold the sorted keys; each becomes struct ray_b200_hit as
+  // the hit query's finish makes it (t, perm[leaf], point_at_param, normal), the rest are empty (t = -1, sphere = -1,
+  // p = normal = 0), and the count is the full number of accepted leaves
+  [[maybe_unused]] auto finish_multi = [&](const int slot, const uint32_t count) {
+    const int k = Q.k;
+    uint32_t *h = multi_records(slot);
+    const int m = count < (uint32_t)k ? (int)count : k;
+    const float4 ro = ray_o[slot], rd = ray_d[slot];
+    const V3 o = v3(ro.x, ro.y, ro.z), d = v3(rd.x, rd.y, rd.z);
+    // records are 32 bytes: a 16-byte aligned buffer (torch's are) takes two 16-byte stores per record instead of eight
+    // scattered 4-byte ones, which was most of the cost of the mostly empty records of large k
+    const bool aligned16 = (reinterpret_cast<uintptr_t>(Q.hits) & 15u) == 0;
+    for (int j = 0; j < k; j++) {
+      float t = -1.0f;
+      int sphere = -1;
+      V3 p = v3(0.0f, 0.0f, 0.0f), n = p;
+      if (j < m) {
+        const uint32_t leaf = h[8 * j + 1];
+        const float4 g = sc.sphere((int)leaf);
+        t = __uint_as_float(h[8 * j]);
+        sphere = __ldg(Q.perm + leaf);
+        p = vadd(o, vscale(t, d));                                // point_at_param, ray.fut:14-15
+        n = vscale(1.0f / g.w, vsub(p, v3(g.x, g.y, g.z)));       // ray.fut:42-43
+      }
+      if (aligned16) {
+        float4 *r = reinterpret_cast<float4 *>(h + 8 * j);
+        r[0] = make_float4(t, __int_as_float(sphere), p.x, p.y);
+        r[1] = make_float4(p.z, n.x, n.y, n.z);
+      } else {
+        float *r = reinterpret_cast<float *>(h + 8 * j);
+        r[0] = t; r[1] = __int_as_float(sphere);
+        r[2] = p.x; r[3] = p.y; r[4] = p.z;
+        r[5] = n.x; r[6] = n.y; r[7] = n.z;
+      }
+    }
+    if (Q.counts) Q.counts[p_item[slot]] = (int32_t)count;
     p_item[slot] = -1;
   };
   // spread: pixels whose last sample has landed are summed IN SAMPLE ORDER and written; frees the ring entry
@@ -406,13 +477,17 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, t_lo, t_hi)) {
               ray_o[slot] = make_float4(ro.x, ro.y, ro.z, q.a);
               ray_i[slot] = make_float4(q.ix, q.iy, q.iz, 0.0f);
-              best_t[slot] = kItemNoHit;
+              best_t[slot] = kMultiHit ? 0u : kItemNoHit;  // multi-hit: no accepted leaf yet
               go = true;
               break;
             }
             if constexpr (kAnyHit) {  // the root box already misses: not occluded
               Q.occluded[p_item[slot]] = 0;
               p_item[slot] = -1;
+              continue;
+            }
+            if constexpr (kMultiHit) {  // the root box already misses: k empty records, count 0
+              finish_multi(slot, 0u);
               continue;
             }
             if (kRays && Q.hits) {
@@ -478,6 +553,34 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         }
         ltop -= n;
         if (hit) best_t[slot] = 0u;  // any value but kItemNoHit: occluded
+        return;
+      }
+      if constexpr (kMultiHit) {
+        // sphere_hit L[i] r t_min t_max with the query's own t_min (no epsilon), then every hit into its slot's list
+        if (kFull || lane < n) {
+          const uint32_t it = lstk[ltop - 1 - lane];
+          slot = (int)(it >> kSlotShift);
+          li = (int)(it & kIndexMask);
+          const float4 ro = ray_o[slot], rd = ray_d[slot];
+          const float4 g = sc.sphere(li);
+          Ray r;
+          r.o = v3(ro.x, ro.y, ro.z);
+          r.d = v3(rd.x, rd.y, rd.z);
+          const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, t_lo, t_hi);
+          hit = t >= 0.0f;
+          tb = __float_as_uint(t);
+        }
+        ltop -= n;
+        if (__any_sync(kFullMask, hit)) {
+          // lanes that hit the same slot insert in rounds, the r-th lane of each slot's group in round r
+          const unsigned peers = __match_any_sync(kFullMask, hit ? slot : -1);
+          const int rank = __popc(peers & lt_mask);
+          const int rounds = (int)__reduce_max_sync(kFullMask, hit ? (unsigned)rank + 1u : 0u);
+          for (int round = 0; round < rounds; round++) {
+            if (hit && rank == round) insert_hit(slot, tb, (uint32_t)li);
+            __syncwarp();
+          }
+        }
         return;
       }
       if (kFull || lane < n) {
@@ -674,6 +777,10 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         p_item[slot] = -1;
         continue;
       }
+      if constexpr (kMultiHit) {
+        finish_multi(slot, best_t[slot]);
+        continue;
+      }
       const float4 ro = ray_o[slot], rd = ray_d[slot], pl = p_light[slot];
       const uint32_t bt = best_t[slot];
       Ray r;
@@ -771,7 +878,8 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
 }
 
 // K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query when q.rays is set:
-// the same kernel in ray mode, without spread samples or packets, closest hit / path or (q.occluded set) any hit.
+// the same kernel in ray mode, without spread samples or packets, closest hit / path, (q.occluded set) any hit or
+// (q.k > 0) multi-hit.
 cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
                              int64_t *launches) {
   const bool rays = q.rays != nullptr;
@@ -792,7 +900,12 @@ cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const Lau
   const long long useful = (work + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
   if (ctas > useful) ctas = useful;
   cudaError_t e;
-  if (rays)
+  if (rays && q.k > 0)
+    e = with_flags([&](auto k2, auto a, auto s) {
+      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, true, false, true>>(
+          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
+    }, k == 2, all_nodes, sph);
+  else if (rays)
     e = with_flags([&](auto k2, auto any_hit, auto a, auto s) {
       return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, true, any_hit>>(
           lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);

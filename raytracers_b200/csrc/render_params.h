@@ -65,12 +65,14 @@ struct RayQuery {
   const float *rays;        // [n][6]: origin.xyz, dir.xyz
   float *rgb;               // path query: [n][3] colour of ray_colour (ray.fut:126-148)
   int32_t *segments;        // path query, optional: [n] objs_hit calls of the path
-  float *hits;              // hit query (non-NULL = hit mode): [n][8] struct ray_b200_hit
+  float *hits;              // hit query (non-NULL = hit mode): [n][8] struct ray_b200_hit; multi-hit query: [n][k][8]
   const int32_t *perm;      // Morton-sorted leaf -> index into the caller's sphere array
   int32_t n;
   float t_min, t_max;       // hit / occlusion query: the call's interval; path query: (0, 1e9) as ray_colour passes it
   int32_t max_depth;        // path query: the depth limit of ray_colour (1 for a hit or occlusion query)
   uint8_t *occluded;        // occlusion query (non-NULL = the any-hit instantiations): [n] 0 / 1
+  int32_t k;                // multi-hit query (> 0 = the multi-hit instantiations): records per ray, in [1, 64]
+  int32_t *counts;          // multi-hit query, optional: [n] accepted leaves per ray, not capped at k
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.

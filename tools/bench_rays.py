@@ -11,14 +11,18 @@
 - rays_irreg_occluded_4M, rays_random1M_occluded_4M: the random rays of the hit workloads through trace_occluded with the
   interval (0.1, 1e9);
 - shadow_irreg_1000: irreg's 1000x1000 camera rays through trace_hits, then a segment from every hit point to a point
-  light above the scene (direction = light - point, interval (1e-4, 1 - 1e-4)) through trace_occluded.
-An occlusion record has trace_hits' time on the same rays and interval beside its own (`hits_ms`) and the fraction of
-rays occluded; its Mrays/s counts one ray per query.
+  light above the scene (direction = light - point, interval (1e-4, 1 - 1e-4)) through trace_occluded;
+- rays_irreg_multi{1,4,16}_4M, rays_random1M_multi4_4M: the random rays of the hit workloads through trace_multi_hits
+  with k = 1, 4, 16 (irreg) and k = 4 (1 M spheres), interval (0.1, 1e9);
+- depth_irreg_1000_multi8: irreg's 1000x1000 camera rays through trace_multi_hits with k = 8 and the interval (0, 1e9),
+  a depth-complexity query.
+An occlusion or multi-hit record has trace_hits' time on the same rays and interval beside its own (`hits_ms`), and the
+fraction of rays occluded or the mean count of a multi-hit query; its Mrays/s counts one ray per query.
 Random rays come from a fixed seed: origins uniform in the scene's bounding box expanded by 10 % per side, directions
 uniform on the sphere, so every run sees the same inputs.  `ms` = the median of 3 queries (CUDA events of the context,
 after one warm-up query that loads the kernel); Mrays/s = objs_hit calls / kernel time (one per ray for a hit query, the
 segments trace_paths reports for a path query); `parity` = differing values against the CPU oracle
-(tests/ray_query_oracle.py, tests/occlusion_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
+(tests/ray_query_oracle.py, tests/occlusion_oracle.py, tests/multi_hit_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
 """
 import argparse
 import json
@@ -49,6 +53,7 @@ def main():
     import numpy as np
     import torch
 
+    import multi_hit_oracle as MQ
     import occlusion_oracle as OQ
     import ray_query_oracle as Q
     import raytracers_b200 as R
@@ -71,19 +76,24 @@ def main():
         return sorted(ms)[1]
 
     out = {}
-    for tag, name, n_spheres, hh, ww, mode in (("rays_irreg_paths_4M", "irreg", None, 1000, 1000, "paths"),
-                                               ("rays_irreg_hits_4M", "irreg", None, 1000, 1000, "hits"),
-                                               ("rays_random1M_hits_4M", "random", 1000000, 2000, 2000, "hits"),
-                                               ("camera_rays_irreg_1000", "irreg", None, 1000, 1000, "camera"),
-                                               ("rays_irreg_occluded_4M", "irreg", None, 1000, 1000, "occluded"),
-                                               ("rays_random1M_occluded_4M", "random", 1000000, 2000, 2000, "occluded"),
-                                               ("shadow_irreg_1000", "irreg", None, 1000, 1000, "shadow")):
+    for tag, name, n_spheres, hh, ww, mode, k in (("rays_irreg_paths_4M", "irreg", None, 1000, 1000, "paths", 0),
+                                                  ("rays_irreg_hits_4M", "irreg", None, 1000, 1000, "hits", 0),
+                                                  ("rays_random1M_hits_4M", "random", 1000000, 2000, 2000, "hits", 0),
+                                                  ("camera_rays_irreg_1000", "irreg", None, 1000, 1000, "camera", 0),
+                                                  ("rays_irreg_occluded_4M", "irreg", None, 1000, 1000, "occluded", 0),
+                                                  ("rays_random1M_occluded_4M", "random", 1000000, 2000, 2000, "occluded", 0),
+                                                  ("shadow_irreg_1000", "irreg", None, 1000, 1000, "shadow", 0),
+                                                  ("rays_irreg_multi1_4M", "irreg", None, 1000, 1000, "multi", 1),
+                                                  ("rays_irreg_multi4_4M", "irreg", None, 1000, 1000, "multi", 4),
+                                                  ("rays_irreg_multi16_4M", "irreg", None, 1000, 1000, "multi", 16),
+                                                  ("rays_random1M_multi4_4M", "random", 1000000, 2000, 2000, "multi", 4),
+                                                  ("depth_irreg_1000_multi8", "irreg", None, 1000, 1000, "depth", 8)):
         if args.only and tag not in args.only.split(","):
             continue
         sc = ctx.scene(name, n=n_spheres)
         pr = ctx.prepare_scene(hh, ww, sc)
-        t_min, t_max = (1e-4, 1 - 1e-4) if mode == "shadow" else (0.1, 1e9)
-        if mode in ("camera", "shadow"):
+        t_min, t_max = (1e-4, 1 - 1e-4) if mode == "shadow" else ((0.0, 1e9) if mode == "depth" else (0.1, 1e9))
+        if mode in ("camera", "shadow", "depth"):
             rays = R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6)
         else:
             rays = random_rays(np, sc.arrays()[0], args.rays, args.seed)
@@ -100,8 +110,14 @@ def main():
         seg = torch.empty((cnt,), dtype=torch.int32, device="cuda")
         hits = torch.empty((cnt, 8), dtype=torch.float32, device="cuda")
         occ = torch.empty((cnt,), dtype=torch.bool, device="cuda")
+        multi = torch.empty((cnt, max(k, 1), 8), dtype=torch.float32, device="cuda")
+        counts = torch.empty((cnt,), dtype=torch.int32, device="cuda")
         torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
-        if mode in ("occluded", "shadow"):
+        if mode in ("multi", "depth"):
+            ms = timed(lambda: ctx.trace_multi_hits_into(d_rays.data_ptr(), cnt, pr, k, multi.data_ptr(), counts.data_ptr(),
+                                                         t_min=t_min, t_max=t_max))
+            segments = cnt
+        elif mode in ("occluded", "shadow"):
             ms = timed(lambda: ctx.trace_occluded_into(d_rays.data_ptr(), cnt, pr, occ.data_ptr(), t_min=t_min, t_max=t_max))
             segments = cnt
         elif mode == "hits":
@@ -111,19 +127,28 @@ def main():
             ms = timed(lambda: ctx.trace_paths_into(d_rays.data_ptr(), cnt, pr, rgb.data_ptr(), seg.data_ptr()))
             segments = int(seg.sum(dtype=torch.int64))
         rec = {"rays": cnt, "ms": round(ms, 3), "segments": segments, "Mrays_s": round(segments / ms / 1e3, 1)}
-        if mode in ("occluded", "shadow"):   # the closest-hit query on the same rays and interval, timed the same way
+        if mode in ("occluded", "shadow", "multi", "depth"):   # the closest-hit query on the same rays and interval, timed the same way
             rec["t_min"], rec["t_max"] = t_min, t_max
             rec["hits_ms"] = round(timed(lambda: ctx.trace_hits_into(d_rays.data_ptr(), cnt, pr, hits.data_ptr(), t_min=t_min, t_max=t_max)), 3)
+        if mode in ("occluded", "shadow"):
             rec["hits_over_occluded"] = round(rec["hits_ms"] / rec["ms"], 3)
             rec["occluded_fraction"] = round(float(occ.float().mean()), 4)
+        if mode in ("multi", "depth"):
+            rec["k"] = k
+            rec["multi_over_hits"] = round(rec["ms"] / rec["hits_ms"], 3)
+            rec["mean_count"] = round(float(counts.double().mean()), 3)
+            rec["max_count"] = int(counts.max())
         if mode == "camera":   # the fused path: the render call on the same frame
             fr = torch.empty((hh, ww), dtype=torch.int32, device="cuda")
             rec["render_ms"] = round(timed(lambda: ctx.render_into(fr.data_ptr(), hh, ww, pr, spp=1)), 3)
             q = (np.float32(255.99) * rgb.cpu().numpy()).astype(np.int32)
             rec["quantised_equals_render_pixels"] = bool(((q[:, 0] << 16 | q[:, 1] << 8 | q[:, 2]).reshape(hh, ww) == fr.cpu().numpy()).all())
         sub = np.linspace(0, cnt - 1, 4096).astype(np.int64)
-        o = (OQ if mode in ("occluded", "shadow") else Q).prepare(name, hh, ww, n=n_spheres)
-        if mode in ("occluded", "shadow"):
+        o = (OQ if mode in ("occluded", "shadow") else MQ if mode in ("multi", "depth") else Q).prepare(name, hh, ww, n=n_spheres)
+        if mode in ("multi", "depth"):
+            want, want_counts = o.trace_multi_hits(rays[sub], k, t_min, t_max)
+            rec["parity"] = int((bits(multi.cpu().numpy()[sub]) != bits(want)).sum()) + int((counts.cpu().numpy()[sub] != want_counts).sum())
+        elif mode in ("occluded", "shadow"):
             rec["parity"] = int((occ.cpu().numpy()[sub] != o.trace_occluded(rays[sub], t_min, t_max)).sum())
         elif mode == "hits":
             rec["parity"] = int((bits(hits.cpu().numpy()[sub]) != bits(o.trace_hits(rays[sub]))).sum())
@@ -131,7 +156,7 @@ def main():
             want_rgb, want_seg = o.trace_paths(rays[sub])
             rec["parity"] = int((bits(rgb.cpu().numpy()[sub]) != bits(want_rgb)).sum()) + int((seg.cpu().numpy()[sub] != want_seg).sum())
         out[tag] = rec
-        del d_rays, rgb, seg, hits, occ
+        del d_rays, rgb, seg, hits, occ, multi, counts
         pr.free(); sc.free()
     ctx.close()
     print(json.dumps({"gpu": gpu[0] if gpu else None, "power_limit_w": float(gpu[1]) if len(gpu) > 1 else None,

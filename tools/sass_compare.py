@@ -4,10 +4,11 @@
     python tools/sass_compare.py OLD.so NEW.so
 
 cuobjdump -sass of both files, split into functions, names demangled.  A function of OLD must exist in NEW with the
-same instructions and encodings.  The any-hit template parameter of the warp-queue kernel (kAnyHit, default false)
-only changes the symbol names of the pixel and the closest-hit / path instantiations; it is mapped out of the names of
-both builds before the comparison, so OLD may be a build from before or after the any-hit variants (it needs ray mode,
-kRays).  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
+same instructions and encodings.  The any-hit and multi-hit template parameters of the warp-queue kernel (kAnyHit and
+kMultiHit, default false) only change the symbol names of the instantiations that leave them false; they are mapped out
+of the names of both builds before the comparison, so OLD may be a build from before or after the any-hit or multi-hit
+variants (it needs ray mode, kRays).  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD
+is identical.
 """
 import collections
 import re
@@ -42,9 +43,14 @@ def functions(path):
 
 
 def normalise(name):
+    # render_warpqueue_kernel<K, kSpread, kPacket, kAllNodes, kSpheres, kRays, kAnyHit, false>(...)
+    # -> the name the same instantiation had before the multi-hit parameter existed, then
     # render_warpqueue_kernel<K, kSpread, kPacket, kAllNodes, kSpheres, kRays, false>(...)
-    # -> the name the same instantiation had before the any-hit parameter existed
-    return re.sub(r"render_warpqueue_kernel<((?:[^,<>]+, ){5}[^,<>]+), false>\(", r"render_warpqueue_kernel<\1>(", name)
+    # -> the name it had before the any-hit parameter existed
+    for n_before in (7, 6):
+        name = re.sub(r"render_warpqueue_kernel<((?:[^,<>]+, ){%d}[^,<>]+), false>\(" % (n_before - 1),
+                      r"render_warpqueue_kernel<\1>(", name)
+    return name
 
 
 def main():
