@@ -380,6 +380,16 @@ cudaError_t with_flags(F &&f, bool b, B... rest) {
   if (b) return with_flags([&](auto... c) { return f(std::true_type{}, c...); }, rest...);
   return with_flags([&](auto... c) { return f(std::false_type{}, c...); }, rest...);
 }
+// ... and with_query(f, q) calls f(std::integral_constant<Query, q>{}) for the ray-query kinds (Query::kPixels is not one)
+template <class F>
+cudaError_t with_query(F &&f, Query q) {
+  switch (q) {
+    case Query::kClosest: return f(std::integral_constant<Query, Query::kClosest>{});
+    case Query::kAnyHit: return f(std::integral_constant<Query, Query::kAnyHit>{});
+    case Query::kMultiHit: return f(std::integral_constant<Query, Query::kMultiHit>{});
+    default: return cudaErrorInvalidValue;
+  }
+}
 
 // Opts Kern in to the device's dynamic shared memory on first use, then launches it.
 template <auto Kern, class... Args>

@@ -123,51 +123,52 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // finished sample's colour is parked in an L2-resident buffer so that the pixel is summed in SAMPLE
 // ORDER when its last sample lands, which keeps the result bit-identical to the sequential definition.
 //
-// Ray mode (kRays, include/ray_b200.h "ray queries"): the work items are the caller's rays instead of pixels.  A claim c
-// is ray c (no tile order), a slot is filled from Q.rays, boxes and spheres are tested against the query's (t_min, t_max)
-// instead of the literal (0, 1e9), the depth limit is Q.max_depth, and a finished path writes Q.rgb / Q.segments.  A hit
-// query (Q.hits != NULL, warp-uniform) is a path query of one segment whose owner lane writes the hit record instead of
-// shading.  Rays of a batch are not coherent: ray mode has no packet walk and no spread samples.  Q is unused otherwise.
+// The query kind (kQuery, render_params.h Query) says what is traced.  Query::kPixels: camera rays of a frame, as above;
+// Q is unused.  Every other kind is a ray query (include/ray_b200.h "ray queries"), "ray mode" below: the work items are
+// the caller's rays instead of pixels.  A claim c is ray c (no tile order), a slot is filled from Q.rays, and boxes are
+// tested against the query's (t_min, t_max) instead of the literal (0, 1e9).  Rays of a batch are not coherent: ray mode
+// has no packet walk and no spread samples.
 //
-// Any-hit ray mode (kAnyHit, an occlusion query): one segment whose answer is "does some leaf the boxes admit accept its
-// sphere in (t_min, t_max)".  That is an OR over the set of reached leaves, so it is order-free like the closest-hit fold,
-// and it may stop early.  best_t[slot] is a "found" flag (kItemNoHit = nothing yet) set by a plain shared store: every
-// writer stores the same value.  Once a slot is marked, its leaf items skip the sphere test and its node items push no
-// children, which prunes the rest of that ray's tree; items already queued cost one pop each.  The drain still runs the
-// queues dry before a slot is refilled, so no stale item reaches a reused slot, and skipping only removes pushes, so the
-// queue bounds and the overflow guard hold as they are.  The owner lane writes Q.occluded and frees the slot.
-// Queue discipline of these instantiations: node batches as in the other instantiations, leaf batches from
+// Query::kClosest, a path or hit query: the closest-hit fold of a frame, spheres tested with epsilon 0.1 whatever t_min
+// is (ray.fut:79), the depth limit is Q.max_depth, and a finished path writes Q.rgb / Q.segments.  A hit query
+// (Q.hits != NULL, warp-uniform) is a path query of one segment whose owner lane writes the hit record instead of shading.
+//
+// Query::kAnyHit, an occlusion query: one segment whose answer is "does some leaf the boxes admit accept its sphere in
+// (t_min, t_max)", with the query's own t_min (no epsilon).  That is an OR over the set of reached leaves, so it is
+// order-free like the closest-hit fold, and it may stop early.  best_t[slot] is a "found" flag (kItemNoHit = nothing yet)
+// set by a plain shared store: every writer stores the same value.  Once a slot is marked, its leaf items skip the sphere
+// test and its node items push no children, which prunes the rest of that ray's tree; items already queued cost one pop
+// each.  The drain still runs the queues dry before a slot is refilled, so no stale item reaches a reused slot, and
+// skipping only removes pushes, so the queue bounds and the overflow guard hold as they are.  The owner lane writes
+// Q.occluded and frees the slot.  Queue discipline of this kind: node batches as for the other kinds, leaf batches from
 // kAnyHitLeafMin items on.
 //
-// Multi-hit ray mode (kMultiHit, a multi-hit query): one segment whose answer is every leaf the boxes admit whose sphere
-// accepts in (t_min, t_max), as the keys bits(t) << 32 | leaf (t >= 0, so bit order is numeric order), of which the Q.k
-// smallest are kept and all are counted.  The set of reached leaves does not depend on the order of the items, and
-// neither do its k smallest keys nor its size.  The list lives in the ray's own k output records (words 0 and 1 of record
-// j = the j-th smallest key so far, sorted); best_t[slot] counts the accepted leaves.  A hit moves the larger keys up one
-// record and drops the k-th when the list is full, so a key above the k-th costs one compare.  Lanes of a leaf batch
-// that hit the same slot insert one at a time (one lane per slot per round, __syncwarp between rounds); slots are
+// Query::kMultiHit, a multi-hit query: one segment whose answer is every leaf the boxes admit whose sphere accepts in
+// (t_min, t_max), again with no epsilon, as the keys bits(t) << 32 | leaf (t >= 0, so bit order is numeric order), of
+// which the Q.k smallest are kept and all are counted.  The set of reached leaves does not depend on the order of the
+// items, and neither do its k smallest keys nor its size.  The list lives in the ray's own k output records (words 0 and
+// 1 of record j = the j-th smallest key so far, sorted); best_t[slot] counts the accepted leaves.  A hit moves the larger
+// keys up one record and drops the k-th when the list is full, so a key above the k-th costs one compare.  Lanes of a leaf
+// batch that hit the same slot insert one at a time (one lane per slot per round, __syncwarp between rounds); slots are
 // warp-private and a ray is claimed once, so no other warp touches the list.  Node batches are those of the closest-hit
-// instantiations: no box is pruned by the k-th t, because the count needs the whole set.  The owner lane turns the keys
-// into hit records (sphere through Q.perm), fills the rest with empty records, writes Q.counts and frees the slot.
+// kinds: no box is pruned by the k-th t, because the count needs the whole set.  The owner lane turns the keys into hit
+// records (sphere through Q.perm), fills the rest with empty records, writes Q.counts and frees the slot.
 
-// any-hit instantiations: a leaf batch runs as soon as this many leaf items are queued (the other instantiations wait
-// for 32, a full batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured
-// against 1, 8 and 32, and newest-first node batches (wq_low = -1) against the default, in DESIGN.md §5.
+// Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
+// batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
+// 32, and newest-first node batches (wq_low = -1) against the default, in DESIGN.md §5.
 #ifndef RAYB200_ANYHIT_LEAF_MIN
 #define RAYB200_ANYHIT_LEAF_MIN 16
 #endif
 constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, bool kRays = false, bool kAnyHit = false,
-          bool kMultiHit = false>
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
-  static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without the packet walk");
-  static_assert(!kAnyHit || kRays, "the any-hit variant is a ray-mode query");
-  static_assert(!kMultiHit || kRays, "the multi-hit variant is a ray-mode query");
-  static_assert(!(kMultiHit && kAnyHit), "a query is either any-hit or multi-hit");
+  constexpr bool kRays = kQuery != Query::kPixels;  // ray mode
+  static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -477,20 +478,19 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, t_lo, t_hi)) {
               ray_o[slot] = make_float4(ro.x, ro.y, ro.z, q.a);
               ray_i[slot] = make_float4(q.ix, q.iy, q.iz, 0.0f);
-              best_t[slot] = kMultiHit ? 0u : kItemNoHit;  // multi-hit: no accepted leaf yet
+              best_t[slot] = kQuery == Query::kMultiHit ? 0u : kItemNoHit;  // multi-hit: no accepted leaf yet
               go = true;
               break;
             }
-            if constexpr (kAnyHit) {  // the root box already misses: not occluded
+            // the root box already misses: a one-segment query has its answer
+            if constexpr (kQuery == Query::kAnyHit) {  // not occluded
               Q.occluded[p_item[slot]] = 0;
               p_item[slot] = -1;
               continue;
-            }
-            if constexpr (kMultiHit) {  // the root box already misses: k empty records, count 0
+            } else if constexpr (kQuery == Query::kMultiHit) {  // k empty records, count 0
               finish_multi(slot, 0u);
               continue;
-            }
-            if (kRays && Q.hits) {
+            } else if (kQuery == Query::kClosest && Q.hits) {  // no hit
               finish_hit(slot, -1.0f, -1, v3(0.0f, 0.0f, 0.0f), v3(0.0f, 0.0f, 0.0f));
               continue;
             }
@@ -530,49 +530,36 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     // Both batch bodies exist twice: a full-warp version (32 items, no lane predicate: the four push flags stay in
     // predicate registers) used while the queues are deep enough, and a partial one for the drain.
     auto leaf_batch = [&](auto full_tag, const int n_part) {
-      // closest_hit (ray.fut:78-81) for up to 32 (ray, sphere) pairs
+      // up to 32 (ray, sphere) pairs: closest_hit (ray.fut:78-81) for pixels and closest-hit queries; sphere_hit L[i] r
+      // t_min t_max with the query's own t_min (no epsilon) for any-hit and multi-hit queries
       constexpr bool kFull = decltype(full_tag)::value;
+      constexpr bool kEpsilon = kQuery == Query::kPixels || kQuery == Query::kClosest;
       const int n = kFull ? 32 : n_part;
       bool hit = false;
       uint32_t tb = 0;
       int slot = 0, li = 0;
-      if constexpr (kAnyHit) {
-        // sphere_hit L[i] r t_min t_max with the query's own t_min (no epsilon); items of a marked ray are skipped
-        if (kFull || lane < n) {
-          const uint32_t it = lstk[ltop - 1 - lane];
-          slot = (int)(it >> kSlotShift);
-          li = (int)(it & kIndexMask);
-          if (best_t[slot] == kItemNoHit) {
-            const float4 ro = ray_o[slot], rd = ray_d[slot];
-            const float4 g = sc.sphere(li);
-            Ray r;
-            r.o = v3(ro.x, ro.y, ro.z);
-            r.d = v3(rd.x, rd.y, rd.z);
-            hit = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, t_lo, t_hi) >= 0.0f;
-          }
-        }
-        ltop -= n;
-        if (hit) best_t[slot] = 0u;  // any value but kItemNoHit: occluded
-        return;
-      }
-      if constexpr (kMultiHit) {
-        // sphere_hit L[i] r t_min t_max with the query's own t_min (no epsilon), then every hit into its slot's list
-        if (kFull || lane < n) {
-          const uint32_t it = lstk[ltop - 1 - lane];
-          slot = (int)(it >> kSlotShift);
-          li = (int)(it & kIndexMask);
+      if (kFull || lane < n) {
+        const uint32_t it = lstk[ltop - 1 - lane];
+        slot = (int)(it >> kSlotShift);
+        li = (int)(it & kIndexMask);
+        if (kQuery != Query::kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: items of a marked ray are skipped
           const float4 ro = ray_o[slot], rd = ray_d[slot];
           const float4 g = sc.sphere(li);
           Ray r;
           r.o = v3(ro.x, ro.y, ro.z);
           r.d = v3(rd.x, rd.y, rd.z);
-          const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, t_lo, t_hi);
+          const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, kEpsilon ? 0.1f : t_lo, t_hi);  // epsilon: ray.fut:79
           hit = t >= 0.0f;
           tb = __float_as_uint(t);
         }
-        ltop -= n;
+      }
+      ltop -= n;
+      if constexpr (kQuery == Query::kAnyHit) {
+        if (hit) best_t[slot] = 0u;  // any value but kItemNoHit: occluded
+      } else if constexpr (kQuery == Query::kMultiHit) {
         if (__any_sync(kFullMask, hit)) {
-          // lanes that hit the same slot insert in rounds, the r-th lane of each slot's group in round r
+          // every hit into its slot's list: lanes that hit the same slot insert in rounds, the r-th lane of each slot's
+          // group in round r
           const unsigned peers = __match_any_sync(kFullMask, hit ? slot : -1);
           const int rank = __popc(peers & lt_mask);
           const int rounds = (int)__reduce_max_sync(kFullMask, hit ? (unsigned)rank + 1u : 0u);
@@ -581,23 +568,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             __syncwarp();
           }
         }
-        return;
+      } else {
+        fold_hit(best_t, best_l, slot, hit, tb, (uint32_t)li);
       }
-      if (kFull || lane < n) {
-        const uint32_t it = lstk[ltop - 1 - lane];
-        slot = (int)(it >> kSlotShift);
-        li = (int)(it & kIndexMask);
-        const float4 ro = ray_o[slot], rd = ray_d[slot];
-        const float4 g = sc.sphere(li);
-        Ray r;
-        r.o = v3(ro.x, ro.y, ro.z);
-        r.d = v3(rd.x, rd.y, rd.z);
-        const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, 0.1f, t_hi);  // epsilon 0.1 whatever t_min is (ray.fut:79)
-        hit = t >= 0.0f;
-        tb = __float_as_uint(t);
-      }
-      ltop -= n;
-      fold_hit(best_t, best_l, slot, hit, tb, (uint32_t)li);
     };
     auto node_batch = [&](auto full_tag, const bool bottom, const int n_part) {
       // one BVH2C node step (both children's boxes) for up to 32 (ray, node) pairs, taken from the top of the queue
@@ -611,7 +584,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const uint32_t it = nstk[ring(kDeque && bottom ? nhead + lane : ntop + ~lane)];
         tag = it & ~kIndexMask;
         const int slot = (int)(it >> kSlotShift), cur = (int)(it & kIndexMask);
-        if (!kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: a marked ray pushes nothing, its subtree is pruned
+        if (kQuery != Query::kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: a marked ray pushes nothing, its subtree is pruned
           const float4 ro = ray_o[slot], ri = ray_i[slot];
           float4 q0, q1, q2, q3;
           sc.node(cur, q0, q1, q2, q3);
@@ -661,7 +634,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     auto drain = [&]() {
       __syncwarp();
       const int nroom = ncap - 96;
-      constexpr int kLeafMin = kAnyHit ? kAnyHitLeafMin : 32;  // leaf items that make a leaf batch due
+      constexpr int kLeafMin = kQuery == Query::kAnyHit ? kAnyHitLeafMin : 32;  // leaf items that make a leaf batch due
       for (;;) {
         // the common case first and alone in its loop: full node batches while nothing else is due (the general
         // dispatch below costs ~12 instructions per batch).  One copy of the batch body for both pop directions.
@@ -772,12 +745,11 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     for (int k = 0; k < K; k++) {
       if (!((trav >> k) & 1u)) continue;
       const int slot = lane + 32 * k;
-      if constexpr (kAnyHit) {
+      if constexpr (kQuery == Query::kAnyHit) {
         Q.occluded[p_item[slot]] = best_t[slot] != kItemNoHit ? 1 : 0;
         p_item[slot] = -1;
         continue;
-      }
-      if constexpr (kMultiHit) {
+      } else if constexpr (kQuery == Query::kMultiHit) {
         finish_multi(slot, best_t[slot]);
         continue;
       }
@@ -790,7 +762,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       int depth = __float_as_int(pl.w);
       const int j = bt == kItemNoHit ? -1 : (int)best_l[slot];
       const float tb = __uint_as_float(bt);
-      if (kRays && Q.hits) {
+      if (kQuery == Query::kClosest && Q.hits) {
         // objs_hit, second half (ray.fut:83-85) with the query's t_min; a failed re-intersection is no hit
         float t = -1.0f;
         V3 p = v3(0.0f, 0.0f, 0.0f), n = p;
@@ -874,15 +846,14 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   }
   if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
   if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  return launch_warpqueue(p, RayQuery{}, lc, stream, launches);                   // RAY_B200_KERNEL_WARPQUEUE
+  return launch_warpqueue(p, Query::kPixels, RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
 }
 
-// K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query when q.rays is set:
-// the same kernel in ray mode, without spread samples or packets, closest hit / path, (q.occluded set) any hit or
-// (q.k > 0) multi-hit.
-cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
+// K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query of kind `kind`: the
+// same kernel in ray mode, without spread samples or packets.
+cudaError_t launch_warpqueue(const RenderParams &p, Query kind, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
                              int64_t *launches) {
-  const bool rays = q.rays != nullptr;
+  const bool rays = kind != Query::kPixels;
   const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
   // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
   // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
@@ -900,16 +871,13 @@ cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const Lau
   const long long useful = (work + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
   if (ctas > useful) ctas = useful;
   cudaError_t e;
-  if (rays && q.k > 0)
-    e = with_flags([&](auto k2, auto a, auto s) {
-      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, true, false, true>>(
-          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
-    }, k == 2, all_nodes, sph);
-  else if (rays)
-    e = with_flags([&](auto k2, auto any_hit, auto a, auto s) {
-      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, true, any_hit>>(
-          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
-    }, k == 2, q.occluded != nullptr, all_nodes, sph);
+  if (rays)
+    e = with_query([&](auto query) {
+      return with_flags([&](auto k2, auto a, auto s) {
+        return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, query>>(
+            lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
+      }, k == 2, all_nodes, sph);
+    }, kind);
   else
     e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
       return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s>>(

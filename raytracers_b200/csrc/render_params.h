@@ -58,9 +58,14 @@ struct RenderParams {
   unsigned long long *warp_trace;
 };
 
-// Ray queries (include/ray_b200.h "ray queries"): the warp-queue kernel's ray-mode instantiations trace caller-supplied
-// rays instead of camera rays.  A block of its own, passed after the kernel's scalar parameters: new fields at the end of
-// RenderParams would move those parameters, and with them the constant-bank offsets in every pixel instantiation's code.
+// What the warp-queue kernel traces (its template parameter kQuery): camera rays of a frame, or the caller's rays of a
+// ray query (include/ray_b200.h "ray queries") to their closest hit or along their path (RayQuery::hits != NULL tells
+// the two apart at run time), to their first accepted sphere (occlusion) or to their k nearest ones (multi-hit).
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit };
+
+// Ray queries: the warp-queue kernel's ray-mode instantiations trace caller-supplied rays instead of camera rays.  A block
+// of its own, passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those
+// parameters, and with them the constant-bank offsets in every pixel instantiation's code.
 struct RayQuery {
   const float *rays;        // [n][6]: origin.xyz, dir.xyz
   float *rgb;               // path query: [n][3] colour of ray_colour (ray.fut:126-148)
@@ -68,10 +73,10 @@ struct RayQuery {
   float *hits;              // hit query (non-NULL = hit mode): [n][8] struct ray_b200_hit; multi-hit query: [n][k][8]
   const int32_t *perm;      // Morton-sorted leaf -> index into the caller's sphere array
   int32_t n;
-  float t_min, t_max;       // hit / occlusion query: the call's interval; path query: (0, 1e9) as ray_colour passes it
-  int32_t max_depth;        // path query: the depth limit of ray_colour (1 for a hit or occlusion query)
-  uint8_t *occluded;        // occlusion query (non-NULL = the any-hit instantiations): [n] 0 / 1
-  int32_t k;                // multi-hit query (> 0 = the multi-hit instantiations): records per ray, in [1, 64]
+  float t_min, t_max;       // hit / occlusion / multi-hit query: the call's interval; path query: (0, 1e9) as ray_colour passes it
+  int32_t max_depth;        // path query: the depth limit of ray_colour (1 for the one-segment queries)
+  uint8_t *occluded;        // occlusion query: [n] 0 / 1
+  int32_t k;                // multi-hit query: records per ray, in [1, 64]
   int32_t *counts;          // multi-hit query, optional: [n] accepted leaves per ray, not capped at k
 };
 
@@ -117,8 +122,9 @@ struct LaunchConfig {
 // A frame on the kernel lc.kernel names (render_kernels.cu)
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches);
-// The warp-queue kernel (render_kernels.cu): a pixel frame, or a ray query when q.rays != NULL (whatever lc.kernel says)
-cudaError_t launch_warpqueue(const RenderParams &p, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
+// The warp-queue kernel (render_kernels.cu): a pixel frame (kind = Query::kPixels, q unused), or a ray query of that kind
+// (whatever lc.kernel says)
+cudaError_t launch_warpqueue(const RenderParams &p, Query kind, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
                              int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
 // build without RAYB200_ALL_KERNELS returns cudaErrorNotSupported)

@@ -2,20 +2,21 @@
 //
 // The literal restatement of the reference in oracle/oracle.cpp is compiled into this translation unit unchanged (it is
 // included below), so every oracle_* entry of liboracle.so exists here too and operates on this library's own handles.
-// On top of it: objs_hit for caller-supplied rays and intervals (ray.fut:76-86) reporting the winning leaf, ray_colour
-// with any depth limit (ray.fut:126-148), and the camera rays of oracle_render.  tests/ray_query_oracle.py compiles it
-// with oracle/Makefile's flags (strict f32: no FMA contraction, no -march, no fast-math).
+// On top of it: the reference's stackless bvh_fold walk for caller-supplied rays and intervals, folded three ways:
+// objs_hit (ray.fut:76-86) reporting the winning leaf, "some reached leaf accepts its sphere in (t_min, t_max)" (the
+// occlusion query) and "every reached leaf that accepts" (the multi-hit query); ray_colour with any depth limit
+// (ray.fut:126-148); and the camera rays of oracle_render.  tests/ray_query_oracle.py compiles it with
+// oracle/Makefile's flags (strict f32: no FMA contraction, no -march, no fast-math).
 #include "../oracle/oracle.cpp"
 
 #include <functional>
 
 namespace {
 
-// ray.fut:76-86 objs_hit with bvh.fut:61-84 bvh_fold inlined literally, as oracle.cpp's objs_hit, plus acc_j: the
-// winning leaf in Morton order (-1 = none).
-bool objs_hit_leaf(const Bvh &bvh, const Ray &r, float t_min, float t_max, Hit *out, int32_t *leaf) {
-  int32_t acc_j = -1;
-  float acc_t = t_max;
+// bvh.fut:61-84 bvh_fold inlined literally, as oracle.cpp's objs_hit walks it, with the boxes tested against
+// (t_min, t_max) (ray.fut:77, the original t range); op(i) is the fold operator "op acc i L[i]" of every reached leaf i.
+template <class Op>
+void bvh_fold(const Bvh &bvh, const Ray &r, float t_min, float t_max, Op &&op) {
   int32_t cur = 0;
   Ptr prev = inner_ptr(-1);
   while (cur != -1) {                                                  // bvh.fut:64
@@ -26,19 +27,52 @@ bool objs_hit_leaf(const Bvh &bvh, const Ray &r, float t_min, float t_max, Hit *
     Ptr child = {0, 0};
     if (from_left) { rec = true; child = node.right; }                 // bvh.fut:70-71
     else if (!from_right) {                                            // bvh.fut:73-76
-      if (aabb_hit(node.aabb, r, t_min, t_max)) { rec = true; child = node.left; }   // ray.fut:77 (original t range)
+      if (aabb_hit(node.aabb, r, t_min, t_max)) { rec = true; child = node.left; }
     }
     if (!rec) { prev = inner_ptr(cur); cur = node.parent; }            // bvh.fut:79-80
     else if (child.tag == 1) { prev = inner_ptr(cur); cur = child.idx; }  // bvh.fut:83
     else {                                                             // bvh.fut:84: op acc i L[i]
-      Hit h;
-      if (sphere_hit(bvh.L[child.idx], r, scene_epsilon, acc_t, &h)) { acc_j = child.idx; acc_t = h.t; }  // ray.fut:78-81
+      op(child.idx);
       prev = child;
     }
   }
+}
+
+// ray.fut:76-86 objs_hit, as oracle.cpp's objs_hit, plus acc_j: the winning leaf in Morton order (-1 = none).
+bool objs_hit_leaf(const Bvh &bvh, const Ray &r, float t_min, float t_max, Hit *out, int32_t *leaf) {
+  int32_t acc_j = -1;
+  float acc_t = t_max;
+  bvh_fold(bvh, r, t_min, t_max, [&](int32_t i) {
+    Hit h;
+    if (sphere_hit(bvh.L[i], r, scene_epsilon, acc_t, &h)) { acc_j = i; acc_t = h.t; }  // ray.fut:78-81
+  });
   *leaf = acc_j;
   if (acc_j >= 0) return sphere_hit(bvh.L[acc_j], r, t_min, acc_t + 1.0f, out);   // ray.fut:83-85
   return false;
+}
+
+// The fold operator "acc or sphere_hit L[i] r t_min t_max" (ray.fut:32-51): some reached leaf accepts in the interval.
+// The OR short-circuits the sphere test once acc is set; the walk itself is not cut short.
+bool objs_occluded(const Bvh &bvh, const Ray &r, float t_min, float t_max) {
+  bool acc = false;
+  bvh_fold(bvh, r, t_min, t_max, [&](int32_t i) {
+    Hit h;
+    acc = acc || sphere_hit(bvh.L[i], r, t_min, t_max, &h);
+  });
+  return acc;
+}
+
+struct Accepted { float t; int32_t leaf; Hit h; };
+
+// The fold operator "acc ++ [(t, i)] if sphere_hit L[i] r t_min t_max" (ray.fut:32-51): every reached leaf that
+// accepts in the interval, in walk order.
+std::vector<Accepted> objs_accepted(const Bvh &bvh, const Ray &r, float t_min, float t_max) {
+  std::vector<Accepted> acc;
+  bvh_fold(bvh, r, t_min, t_max, [&](int32_t i) {
+    Hit h;
+    if (sphere_hit(bvh.L[i], r, t_min, t_max, &h)) acc.push_back({h.t, i, h});
+  });
+  return acc;
 }
 
 // Runs fn(first, end) over spans of 64 rays on `threads` threads (<= 0: all cores).
@@ -121,6 +155,53 @@ void oracle_camera_ray(void *pv, int64_t h, int64_t w, int32_t spp, int64_t j, i
   const Ray r = get_ray(p->cam, u, v);
   const float o[6] = {r.origin.x, r.origin.y, r.origin.z, r.dir.x, r.dir.y, r.dir.z};
   std::copy(o, o + 6, out6);
+}
+
+// Occlusion per ray of rays (n x 6: origin.xyz, dir.xyz): out[i] = 1 if some leaf the walk reaches accepts its sphere
+// in (t_min, t_max), else 0.
+int oracle_trace_occluded(void *pv, const float *rays, int64_t n, float t_min, float t_max, uint8_t *out, int32_t threads) {
+  Prepared *p = (Prepared *)pv;
+  if (!p || n < 0) return 1;
+  for_spans(n, threads, [&](int64_t i0, int64_t i1) {
+    for (int64_t i = i0; i < i1; i++) {
+      const float *q = rays + 6 * i;
+      out[i] = objs_occluded(p->objs, Ray{{q[0], q[1], q[2]}, {q[3], q[4], q[5]}}, t_min, t_max) ? 1 : 0;
+    }
+  });
+  return 0;
+}
+
+// Multi-hit per ray of rays (n x 6: origin.xyz, dir.xyz): the accepted leaves stable-sorted by (t, leaf), the first k as
+// out8[i][j] = struct ray_b200_hit (t, bits(perm[leaf]), p.xyz, normal.xyz from sphere_hit's own Hit), the rest t = -1,
+// sphere = -1, p = normal = 0; counts[i] = the number of accepted leaves (counts may be NULL).
+int oracle_trace_multi_hits(void *pv, const float *rays, int64_t n, float t_min, float t_max, int32_t k, float *out8,
+                            int32_t *counts, int32_t threads) {
+  Prepared *p = (Prepared *)pv;
+  if (!p || n < 0 || k < 1) return 1;
+  for_spans(n, threads, [&](int64_t i0, int64_t i1) {
+    for (int64_t i = i0; i < i1; i++) {
+      const float *q = rays + 6 * i;
+      std::vector<Accepted> acc = objs_accepted(p->objs, Ray{{q[0], q[1], q[2]}, {q[3], q[4], q[5]}}, t_min, t_max);
+      std::stable_sort(acc.begin(), acc.end(), [](const Accepted &a, const Accepted &b) {
+        return a.t < b.t || (a.t == b.t && a.leaf < b.leaf);
+      });
+      for (int32_t j = 0; j < k; j++) {
+        float *o = out8 + 8 * ((size_t)i * (size_t)k + (size_t)j);
+        if ((size_t)j < acc.size()) {
+          const Hit &h = acc[j].h;
+          const int32_t sphere = p->objs.perm[(size_t)acc[j].leaf];
+          o[0] = h.t; memcpy(o + 1, &sphere, 4);
+          o[2] = h.p.x; o[3] = h.p.y; o[4] = h.p.z; o[5] = h.normal.x; o[6] = h.normal.y; o[7] = h.normal.z;
+        } else {
+          const int32_t none = -1;
+          o[0] = -1.0f; memcpy(o + 1, &none, 4);
+          for (int c = 2; c < 8; c++) o[c] = 0.0f;
+        }
+      }
+      if (counts) counts[i] = (int32_t)acc.size();
+    }
+  });
+  return 0;
 }
 
 }  // extern "C"

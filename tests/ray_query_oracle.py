@@ -1,9 +1,9 @@
 """ctypes binding of the ray-query oracle (tests/ray_query_oracle.cpp).  TEST INFRASTRUCTURE ONLY.
 
 The library is compiled on first use into a fresh temporary directory with oracle/Makefile's flags, so a read-only
-checkout works.  It contains the whole CPU oracle (oracle/oracle.cpp, included unchanged) plus objs_hit / ray_colour for
-caller-supplied rays; its handles are its own, not liboracle.so's.  Used by tests/test_ray_queries.py,
-__graft_entry__.smoke() and tools/bench_rays.py.
+checkout works.  It contains the whole CPU oracle (oracle/oracle.cpp, included unchanged) plus the four ray queries
+(objs_hit, ray_colour, occlusion and multi-hit) for caller-supplied rays; its handles are its own, not liboracle.so's.
+Used by the ray-query tests, __graft_entry__.smoke() and tools/bench_rays.py.
 """
 import ctypes as C
 import os
@@ -48,6 +48,10 @@ def lib():
         L.oracle_trace_hits.argtypes = [vp, vp, i64, f32, f32, vp, i32]
         L.oracle_trace_paths.restype = C.c_int
         L.oracle_trace_paths.argtypes = [vp, vp, i64, i32, vp, vp, i32]
+        L.oracle_trace_occluded.restype = C.c_int
+        L.oracle_trace_occluded.argtypes = [vp, vp, i64, f32, f32, vp, i32]
+        L.oracle_trace_multi_hits.restype = C.c_int
+        L.oracle_trace_multi_hits.argtypes = [vp, vp, i64, f32, f32, i32, vp, vp, i32]
         L.oracle_camera_ray.argtypes = [vp, i64, i64, i32, i64, i64, i32, vp]
         _lib = L
     return _lib
@@ -84,6 +88,28 @@ class Prepared:
         if lib().oracle_trace_paths(self._h, _p(r), r.shape[0], int(max_depth), _p(rgb), _p(seg), int(threads)) != 0:
             raise RuntimeError("oracle_trace_paths failed")
         return rgb, seg
+
+    def trace_occluded(self, rays, t_min=0.0, t_max=1e9, threads=0):
+        """Occlusion of every ray of float32[n][6]: bool[n], True if the bvh_fold walk (bvh.fut:61-84, boxes against
+        (t_min, t_max)) reaches a leaf whose sphere_hit L[i] r t_min t_max (ray.fut:32-51) is a hit."""
+        r = np.ascontiguousarray(rays, np.float32).reshape(-1, 6)
+        out = np.empty(r.shape[0], np.uint8)
+        if lib().oracle_trace_occluded(self._h, _p(r), r.shape[0], float(t_min), float(t_max), _p(out), int(threads)) != 0:
+            raise RuntimeError("oracle_trace_occluded failed")
+        return out.view(np.bool_)
+
+    def trace_multi_hits(self, rays, k, t_min=0.0, t_max=1e9, threads=0):
+        """The multi-hit query of every ray of float32[n][6]: (float32[n][k][8] records as struct ray_b200_hit, int32[n]
+        counts).  The records are the leaves the bvh_fold walk (bvh.fut:61-84, boxes against (t_min, t_max)) reaches
+        whose sphere_hit L[i] r t_min t_max (ray.fut:32-51) is a hit, stable-sorted by (t, leaf), the first k of them;
+        empty records (t = -1, sphere = -1, p = normal = 0) after the last.  counts = all accepted leaves."""
+        r = np.ascontiguousarray(rays, np.float32).reshape(-1, 6)
+        out = np.empty((r.shape[0], int(k), 8), np.float32)
+        counts = np.empty(r.shape[0], np.int32)
+        if lib().oracle_trace_multi_hits(self._h, _p(r), r.shape[0], float(t_min), float(t_max), int(k), _p(out), _p(counts),
+                                         int(threads)) != 0:
+            raise RuntimeError("oracle_trace_multi_hits failed")
+        return out, counts
 
     def camera_ray(self, h, w, j, i, s=0, spp=1):
         """get_ray (ray.fut:109-114) for sample s of pixel (row j, column i) of an h x w frame, as render makes it."""

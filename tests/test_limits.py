@@ -21,18 +21,7 @@ import pytest
 
 import limit_scenes as LS
 import ray_query_oracle as Q
-from test_ray_queries import bits_differ, hits_differ, quantise
-
-GiB = 1 << 30
-
-
-def _torch():
-    import torch
-    return torch
-
-
-def _dev(a):
-    return _torch().from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
+from ray_query_cases import GiB, _dev, _torch, bits_differ, hits_differ, quantise
 
 
 class DeviceUse:

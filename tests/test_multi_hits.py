@@ -7,10 +7,9 @@ import numpy as np
 import pytest
 
 import limit_scenes as LS
-import multi_hit_oracle as M   # tests/multi_hit_oracle.py: the CPU oracle of the multi-hit query
-import occlusion_oracle as OQ  # tests/occlusion_oracle.py: the CPU oracle of the occlusion query
-from test_occlusion import GiB, INTERVALS, PLANS, RANDOM_SCENES, SEGMENT, T24, _dev, _gpu_case, _np, _shadow_case, _torch, max_hit_t
-from test_ray_queries import ALONG_Z, TWO_CAM, TWO_SPHERES, hits_differ, random_rays
+import ray_query_oracle as Q   # tests/ray_query_oracle.py: the CPU oracle of the ray queries
+from ray_query_cases import (ALONG_Z, GiB, INTERVALS, PLANS, RANDOM_SCENES, SEGMENT, T24, TWO_CAM, TWO_SPHERES, _dev,
+                             _gpu_case, _np, _shadow_case, _torch, hits_differ, max_hit_t, random_rays)
 
 # ------------------------------------------------------------------------------------------ helpers
 
@@ -107,14 +106,14 @@ def test_multi_hits_is_bound(R):
 
 
 def test_oracle_two_sphere_known_answers():
-    pr = M.prepare_custom(TWO_SPHERES, TWO_CAM, 64, 64)
+    pr = Q.prepare_custom(TWO_SPHERES, TWO_CAM, 64, 64)
     check_two_sphere(lambda r, k, lo, hi: pr.trace_multi_hits(r, k, lo, hi))
 
 
 @pytest.mark.parametrize("name", ["rgbbox", "irreg"])
 def test_oracle_self_consistency(R, name):
-    pr = M.prepare(name, 64, 64)
-    occ = OQ.prepare(name, 64, 64)
+    pr = Q.prepare(name, 64, 64)
+    occ = Q.prepare(name, 64, 64)
     spheres, _ = R.host_scene(name)
     perm = pr.perm(spheres.shape[0])
     leaf_of_sphere = np.empty_like(perm)
@@ -162,7 +161,7 @@ def test_random_rays_equal_oracle(R, name, n_spheres):
     ctx, sc, pr = _gpu_case(R, name, n=n_spheres)
     with ctx:
         rays = random_rays(sc.arrays()[0], 8192, seed=43)
-        o = M.prepare(name, 500, 500, n=n_spheres)
+        o = Q.prepare(name, 500, 500, n=n_spheres)
         d = _dev(rays)
         several = False
         for t_min, t_max in INTERVALS:
@@ -194,7 +193,7 @@ def test_random_rays_on_the_million_sphere_scene(R):
         ctx.trace_multi_hits_into(d.data_ptr(), rays.shape[0], pr, k, hits.data_ptr(), counts.data_ptr(), t_min=0.1)
         ctx.sync()
         sub = slice(0, None, 16)
-        want = M.prepare("random", 2000, 2000, n=1000000).trace_multi_hits(rays[sub], k, 0.1, 1e9)
+        want = Q.prepare("random", 2000, 2000, n=1000000).trace_multi_hits(rays[sub], k, 0.1, 1e9)
         assert_equal((_np(hits)[sub], _np(counts)[sub]), want, "1M")
         assert (want[1] > k).any() and 0.02 < (want[1] > 0).mean() < 0.98
 
@@ -211,7 +210,7 @@ def test_plan_variants_give_identical_results(R, name):
             rays = np.concatenate([random_rays(sc.arrays()[0], 3000, seed=53), _shadow_case(R, ctx, sc, pr, h, w)])
             d = _dev(rays)
             results.append([gpu_multi(ctx, pr, d, k, lo, hi) for lo, hi in intervals for k in (1, 8)])
-    o = M.prepare(name, h, w)
+    o = Q.prepare(name, h, w)
     want = [o.trace_multi_hits(rays, k, lo, hi) for lo, hi in intervals for k in (1, 8)]
     for kw, got in zip(PLANS, results):
         for j in range(len(want)):
@@ -234,7 +233,7 @@ def test_batch_sizes(R, n):
         assert ctx.launch_count() == before + 1
         assert ctx.last_render_ms() > 0
         sub = slice(None) if n < 1000 else slice(0, None, 997)
-        want = M.prepare("irreg", 500, 500).trace_multi_hits(rays[sub], 4, 0.1, 1e9)
+        want = Q.prepare("irreg", 500, 500).trace_multi_hits(rays[sub], 4, 0.1, 1e9)
         assert_equal((got[0][sub], got[1][sub]), want, n)
 
 
@@ -243,7 +242,7 @@ def test_edge_rays_equal_oracle(R):
     ctx, sc, pr = _gpu_case(R, "rgbbox")
     with ctx:
         spheres = sc.arrays()[0]
-        o = M.prepare("rgbbox", 500, 500)
+        o = Q.prepare("rgbbox", 500, 500)
         c, rad = spheres[:, :3], spheres[:, 6:7]
         rays = [[0, 0, 0, 0, 0, 0], [0, 0, 0, 1, 0, 0], [0, 0, 0, 0, -1, 0], [0, 0, 0, 0, 0, 1],   # all-zero, axis-aligned
                 [0, 30, 30, 0, -1, -1], [1, 2, 3, -0.0, 0.0, 1], [0, 0, 0, 1, 1, 0], [-30, -30, -30, 1, 1, 1],
@@ -290,7 +289,7 @@ def test_tie_groups_keep_the_lowest_caller_indices(R):
     and the count is the whole group, on every plan: no schedule may leak into the result."""
     s, groups = LS.tie_groups()
     rays = LS.tie_rays(len(groups))
-    o = M.prepare_custom(s, LS.TIE_CAM, 96, 128)
+    o = Q.prepare_custom(s, LS.TIE_CAM, 96, 128)
     k = 64
     want = o.trace_multi_hits(rays, k)
     assert max(len(g) for g in groups) > k   # premise: some list is truncated
@@ -311,7 +310,7 @@ def test_tie_groups_keep_the_lowest_caller_indices(R):
 def test_comb_tree_depth_48(R):
     s, _ = LS.comb_scene(1 << 18)
     rays = LS.comb_query_rays(122, seed=3)
-    o = M.prepare_custom(s, LS.COMB_CAM, 48, 64)
+    o = Q.prepare_custom(s, LS.COMB_CAM, 48, 64)
     intervals = [(0.0, 1e9), (0.1, 1e9), (1.0, 100.0), (0.0, 1.5)]
     want = {(iv, k): o.trace_multi_hits(rays, k, *iv) for iv in intervals for k in (1, 8)}
     assert (want[((0.0, 1e9), 8)][1] > 0).all() and not want[((0.0, 1.5), 8)][1].any()
@@ -353,7 +352,7 @@ def test_records_past_4GiB(R):
         idx = np.unique(np.concatenate([rng.integers(0, N22, 3000), np.arange(N22 - 64, N22)]))
         it = torch.from_numpy(idx).cuda()
         got = (hits[it].cpu().numpy().view(np.float32), counts[it].cpu().numpy())
-        want = M.prepare("irreg", 500, 500).trace_multi_hits(rays[idx], k)
+        want = Q.prepare("irreg", 500, 500).trace_multi_hits(rays[idx], k)
         assert_equal(got, want, "past 4 GiB")
         assert (want[1] > 1).any()
 
@@ -392,7 +391,7 @@ def test_validation_errors_leave_the_context_usable(R):
         assert ctx.launch_count() == before
         ctx.trace_multi_hits_into(rp, 0, pr, 4, None, None)   # n == 0 does nothing, NULL buffers included
         assert ctx.launch_count() == before
-        o = M.prepare("rgbbox", 500, 500)
+        o = Q.prepare("rgbbox", 500, 500)
         ctx.trace_multi_hits_into(rp, 64, pr, 64, hp, None)   # counts are optional
         ctx.sync()
         assert records_differ(_np(hits), o.trace_multi_hits(_np(rays), 64)[0]) == 0
@@ -410,7 +409,7 @@ def test_records_at_4_byte_alignment(R):
         rays = random_rays(sc.arrays()[0], 5000, seed=73)
         d = _dev(rays)
         k = 5
-        want = M.prepare("irreg", 500, 500).trace_multi_hits(rays, k, 0.1, 1e9)
+        want = Q.prepare("irreg", 500, 500).trace_multi_hits(rays, k, 0.1, 1e9)
         for offset in (1, 2, 3):   # floats
             raw = torch.empty((rays.shape[0] * k * 8 + 4,), dtype=torch.float32, device="cuda")
             counts = torch.empty((rays.shape[0],), dtype=torch.int32, device="cuda")
@@ -433,7 +432,7 @@ def test_freed_scene_in_flight_and_frames_unchanged(R, golden):
         frame_scene = ctx.prepare_scene(h, w, sc)
         rays = random_rays(sc.arrays()[0], 20000, seed=67)
         k = 6
-        want = M.prepare("rgbbox", h, w).trace_multi_hits(rays, k, 0.1, 50.0)
+        want = Q.prepare("rgbbox", h, w).trace_multi_hits(rays, k, 0.1, 50.0)
         frames = [torch.empty((h, w), dtype=torch.int32, device="cuda") for _ in range(4)]
         outs = []
         for j in range(4):

@@ -6,42 +6,12 @@ import numpy as np
 import pytest
 
 import limit_scenes as LS
-import occlusion_oracle as Q   # tests/occlusion_oracle.py: the CPU oracle of the occlusion query
-from test_ray_queries import ALONG_Z, TWO_CAM, TWO_SPHERES, random_rays
-
-GiB = 1 << 30
-T24 = np.float32(1 << 24)
+import ray_query_oracle as Q   # tests/ray_query_oracle.py: the CPU oracle of the ray queries
+from ray_query_cases import (ALONG_Z, GiB, INTERVALS, PLANS, RANDOM_SCENES, SEGMENT, T24, TWO_CAM, TWO_SPHERES, _dev,
+                             _gpu_case, _np, _shadow_case, _torch, light_above, max_hit_t, random_rays, segment_rays)
 
 # ------------------------------------------------------------------------------------------ helpers
 
-
-def max_hit_t(spheres, rays):
-    """An upper bound of every t at which a ray can meet a sphere: a hit point lies on some sphere, so
-    t * |d| <= |o - c| + r for that sphere.  Rays with d = 0 never hit (their discriminant is 0)."""
-    s = np.asarray(spheres, np.float64)
-    r = np.asarray(rays, np.float64)
-    dist = np.linalg.norm(r[:, None, :3] - s[None, :, :3], axis=2).max(1) + s[:, 6].max()
-    dn = np.linalg.norm(r[:, 3:6], axis=1)
-    ok = dn > 0
-    return float((dist[ok] / dn[ok]).max()) if ok.any() else 0.0
-
-
-def light_above(spheres):
-    """A point light above the middle of the scene's bounding box, one box height above its top."""
-    s = np.asarray(spheres, np.float32)
-    lo = (s[:, :3] - s[:, 6:7]).min(0)
-    hi = (s[:, :3] + s[:, 6:7]).max(0)
-    return np.float32([(lo[0] + hi[0]) / 2, hi[1] + (hi[1] - lo[1]), (lo[2] + hi[2]) / 2])
-
-
-def segment_rays(points, target):
-    """Point-to-point visibility rays: origin = point, direction = target - point (not normalised), so that the
-    interval (1e-4, 1 - 1e-4) covers the open segment."""
-    p = np.asarray(points, np.float32)
-    return np.ascontiguousarray(np.concatenate([p, np.asarray(target, np.float32)[None] - p], 1), np.float32)
-
-
-SEGMENT = (1e-4, 1 - 1e-4)
 
 # (ray, t_min, t_max, occluded) on the two-sphere scene: A = centre 0, radius 1 (roots 4 and 6 along ALONG_Z),
 # B = centre (0, 0, 10), radius 1 (roots 14 and 16)
@@ -115,29 +85,6 @@ def test_segment_rays_of_the_shadow_workload(R):
 
 # ------------------------------------------------------------------------------------------ GPU
 
-def _torch():
-    import torch
-    return torch
-
-
-def _dev(a):
-    return _torch().from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
-
-
-def _gpu_case(R, name, h=500, w=500, n=None, seed=1, **ctx_kw):
-    ctx = R.Context(device=0, **ctx_kw)
-    sc = ctx.scene(name, n=n, seed=seed)
-    return ctx, sc, ctx.prepare_scene(h, w, sc)
-
-
-def _np(t):
-    return t.cpu().numpy()
-
-
-INTERVALS = [(0.0, 1e9), (0.1, 1e9), (1.0, 100.0), (2.5, 1e9), (40.0, 7.0)]
-RANDOM_SCENES = [("rgbbox", None), ("irreg", None), ("random", 30000)]
-
-
 @pytest.mark.gpu
 def test_two_sphere_known_answers_on_gpu(R):
     with R.Context(device=0) as ctx:
@@ -185,13 +132,6 @@ def test_random_rays_on_the_million_sphere_scene(R):
         assert 0.02 < want.mean() < 0.98
 
 
-def _shadow_case(R, ctx, sc, pr, h, w):
-    """Camera rays through trace_hits, then segments from every hit point to the light."""
-    hits = ctx.trace_hits(pr, _dev(R.camera_rays(pr.info()["camera"], h, w).reshape(-1, 6)))
-    t = _np(hits["t"])
-    return segment_rays(_np(hits["p"])[t >= 0], light_above(sc.arrays()[0]))
-
-
 @pytest.mark.gpu
 def test_shadow_rays(R):
     h, w = 500, 500
@@ -211,10 +151,6 @@ def test_shadow_rays(R):
             occ = _np(ctx.trace_occluded(pr, d, t_min=0.1, t_max=t_max))
             hit = _np(ctx.trace_hits(pr, d, t_min=0.1, t_max=t_max)["t"]) >= 0
             assert int((occ != hit).sum()) == 0, t_max
-
-
-PLANS = [{}, {"wq_k": 1}, {"wq_k": 2}, {"wq_warps": 3}, {"wq_warps": 5}, {"stage_cap": 1024}, {"wq_low": -1},
-         {"wq_low": 64}, {"wq_ncap": 256}]
 
 
 @pytest.mark.gpu

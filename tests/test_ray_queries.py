@@ -7,51 +7,9 @@ import numpy as np
 import pytest
 
 import ray_query_oracle as Q   # tests/ray_query_oracle.py: the CPU oracle of the ray queries
+from ray_query_cases import ALONG_Z, TWO_CAM, TWO_SPHERES, _dev, _gpu_case, _torch, bits_differ, hits_differ, quantise, random_rays
 
 # ------------------------------------------------------------------------------------------ helpers
-
-
-def bits_differ(a, b):
-    """Number of float32 values whose bits differ (any NaN equals any NaN)."""
-    a = np.ascontiguousarray(a, np.float32).ravel()
-    b = np.ascontiguousarray(b, np.float32).ravel()
-    assert a.shape == b.shape
-    na, nb = np.isnan(a), np.isnan(b)
-    return int(((na != nb) | (~na & (a.view(np.uint32) != b.view(np.uint32)))).sum())
-
-
-def hits_differ(got, want):
-    """[n, 8] hit records: the sphere column as int32, the rest by bits."""
-    got = np.ascontiguousarray(got, np.float32)
-    want = np.ascontiguousarray(want, np.float32)
-    bad = int((got[:, 1].view(np.int32) != want[:, 1].view(np.int32)).sum())
-    return bad + bits_differ(got[:, [0, 2, 3, 4, 5, 6, 7]], want[:, [0, 2, 3, 4, 5, 6, 7]])
-
-
-def quantise(rgb):
-    """colour_to_pixel (ray.fut:158-162) of float32 [..., 3]."""
-    q = (np.float32(255.99) * np.asarray(rgb, np.float32)).astype(np.int32)
-    return (q[..., 0] << 16) | (q[..., 1] << 8) | q[..., 2]
-
-
-def random_rays(spheres, n, seed):
-    """Origins uniform in the scene's bounding box expanded by 10 % per side, directions uniform on the sphere."""
-    s = np.asarray(spheres, np.float32)
-    lo = (s[:, :3] - s[:, 6:7]).min(0)
-    hi = (s[:, :3] + s[:, 6:7]).max(0)
-    ext = 0.1 * (hi - lo)
-    rng = np.random.default_rng(seed)
-    o = rng.uniform(lo - ext, hi + ext, (n, 3)).astype(np.float32)
-    d = rng.standard_normal((n, 3)).astype(np.float32)
-    d /= np.linalg.norm(d, axis=1, keepdims=True).astype(np.float32)
-    return np.ascontiguousarray(np.concatenate([o, d], 1), np.float32)
-
-
-# A hand-built scene with exactly representable answers.  Sphere A (centre 0, radius 1) is second in the caller's array
-# and first in Morton order, so a hit on it reports sphere 1; sphere B (centre (0,0,10), radius 1) is first.
-TWO_SPHERES = np.array([[0, 0, 10, 0.5, 0.5, 0.5, 1], [0, 0, 0, 0.8, 0.6, 0.4, 1]], np.float32)
-TWO_CAM = np.array([0, 0, -20, 0, 0, 0, 60], np.float32)
-ALONG_Z = [0, 0, -5, 0, 0, 1]
 
 
 def two_sphere_cases():
@@ -135,21 +93,6 @@ def test_oracle_two_sphere_known_answers():
 
 
 # ------------------------------------------------------------------------------------------ GPU
-
-def _torch():
-    import torch
-    return torch
-
-
-def _dev(a):
-    return _torch().from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
-
-
-def _gpu_case(R, name, h=500, w=500, n=None, seed=1, **ctx_kw):
-    ctx = R.Context(device=0, **ctx_kw)
-    sc = ctx.scene(name, n=n, seed=seed)
-    return ctx, sc, ctx.prepare_scene(h, w, sc)
-
 
 def _oracle_for(name, h=500, w=500, n=None, seed=1):
     return Q.prepare(name, h, w, n=n, seed=seed)

@@ -22,7 +22,7 @@ Random rays come from a fixed seed: origins uniform in the scene's bounding box 
 uniform on the sphere, so every run sees the same inputs.  `ms` = the median of 3 queries (CUDA events of the context,
 after one warm-up query that loads the kernel); Mrays/s = objs_hit calls / kernel time (one per ray for a hit query, the
 segments trace_paths reports for a path query); `parity` = differing values against the CPU oracle
-(tests/ray_query_oracle.py, tests/occlusion_oracle.py, tests/multi_hit_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
+(tests/ray_query_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
 """
 import argparse
 import json
@@ -53,8 +53,6 @@ def main():
     import numpy as np
     import torch
 
-    import multi_hit_oracle as MQ
-    import occlusion_oracle as OQ
     import ray_query_oracle as Q
     import raytracers_b200 as R
 
@@ -144,7 +142,7 @@ def main():
             q = (np.float32(255.99) * rgb.cpu().numpy()).astype(np.int32)
             rec["quantised_equals_render_pixels"] = bool(((q[:, 0] << 16 | q[:, 1] << 8 | q[:, 2]).reshape(hh, ww) == fr.cpu().numpy()).all())
         sub = np.linspace(0, cnt - 1, 4096).astype(np.int64)
-        o = (OQ if mode in ("occluded", "shadow") else MQ if mode in ("multi", "depth") else Q).prepare(name, hh, ww, n=n_spheres)
+        o = Q.prepare(name, hh, ww, n=n_spheres)
         if mode in ("multi", "depth"):
             want, want_counts = o.trace_multi_hits(rays[sub], k, t_min, t_max)
             rec["parity"] = int((bits(multi.cpu().numpy()[sub]) != bits(want)).sum()) + int((counts.cpu().numpy()[sub] != want_counts).sum())

@@ -4,11 +4,10 @@
     python tools/sass_compare.py OLD.so NEW.so
 
 cuobjdump -sass of both files, split into functions, names demangled.  A function of OLD must exist in NEW with the
-same instructions and encodings.  The any-hit and multi-hit template parameters of the warp-queue kernel (kAnyHit and
-kMultiHit, default false) only change the symbol names of the instantiations that leave them false; they are mapped out
-of the names of both builds before the comparison, so OLD may be a build from before or after the any-hit or multi-hit
-variants (it needs ray mode, kRays).  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD
-is identical.
+same instructions and encodings.  The warp-queue kernel's instantiations are matched by one canonical key, (K, spread,
+packet, all-nodes, spheres, query kind), parsed from every form its template has had: five parameters (pixel frames
+only), six (kRays), seven (kAnyHit), eight (kMultiHit) and the query-kind enum (Query).  So OLD and NEW may be builds of
+any of them.  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
 """
 import collections
 import re
@@ -42,19 +41,29 @@ def functions(path):
     return collections.OrderedDict(((d[n], i), b) for (n, i), b in out.items())
 
 
-def normalise(name):
-    # render_warpqueue_kernel<K, kSpread, kPacket, kAllNodes, kSpheres, kRays, kAnyHit, false>(...)
-    # -> the name the same instantiation had before the multi-hit parameter existed, then
-    # render_warpqueue_kernel<K, kSpread, kPacket, kAllNodes, kSpheres, kRays, false>(...)
-    # -> the name it had before the any-hit parameter existed
-    for n_before in (7, 6):
-        name = re.sub(r"render_warpqueue_kernel<((?:[^,<>]+, ){%d}[^,<>]+), false>\(" % (n_before - 1),
-                      r"render_warpqueue_kernel<\1>(", name)
-    return name
+WARPQUEUE = re.compile(r"render_warpqueue_kernel<([^<>]*)>\(")
+KINDS = ("pixels", "closest", "any-hit", "multi-hit")   # the values of the Query enum, in order
+
+
+def canonical(name):
+    """The key of a warp-queue instantiation, whatever the form of its template; other names as they are."""
+    m = WARPQUEUE.search(name)
+    if not m:
+        return name
+    args = [a.strip() for a in m.group(1).split(",")]
+    k, (spread, packet, all_nodes, spheres), rest = args[0], args[1:5], args[5:]
+    enum = re.fullmatch(r"\(.*Query\)(\d+)", rest[0]) if rest else None
+    if enum:   # <K, kSpread, kPacket, kAllNodes, kSpheres, (Query)N>
+        kind = KINDS[int(enum.group(1))]
+    else:      # <K, kSpread, kPacket, kAllNodes, kSpheres[, kRays[, kAnyHit[, kMultiHit]]]>, false when absent
+        rays, any_hit, multi_hit = [a == "true" for a in rest] + [False] * (3 - len(rest))
+        kind = KINDS[0 if not rays else 2 if any_hit else 3 if multi_hit else 1]
+    return (f"render_warpqueue_kernel[K={k}, spread={spread}, packet={packet}, all_nodes={all_nodes}, spheres={spheres}, "
+            f"query={kind}]")
 
 
 def main():
-    old, new = ({(normalise(n), i): b for (n, i), b in functions(path).items()} for path in sys.argv[1:3])
+    old, new = ({(canonical(n), i): b for (n, i), b in functions(path).items()} for path in sys.argv[1:3])
     bad = 0
     for key, body in old.items():
         other = new.get(key)
