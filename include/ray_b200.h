@@ -24,7 +24,8 @@
  *
  * Ray queries ("ray queries" below): rays the caller made are traced against a prepared scene to their closest hit
  * (objs_hit), along their path (ray_colour), bit for bit, to their first accepted sphere (occlusion), or to the k
- * nearest of their accepted spheres (multi-hit), by the same warp-queue kernel in ray mode.
+ * nearest of their accepted spheres (multi-hit), by the same warp-queue kernel in ray mode.  The last three also take
+ * rays that carry their own (t_min, t_max) (struct ray_b200_ray, the *_ranged entry points).
  */
 #ifndef RAY_B200_EXT_H
 #define RAY_B200_EXT_H
@@ -180,6 +181,33 @@ int ray_b200_trace_multi_hits(struct futhark_context *ctx, const struct futhark_
                               struct ray_b200_hit *hits_dev, int32_t *counts_dev);
 /* sizeof(struct ray_b200_hit) as the library was compiled (32). */
 int64_t ray_b200_hit_size(void);
+/* Ranged queries: rays that carry their own interval, as Embree's tnear / tfar, OptiX's tmin / tmax and DXR's RayDesc do
+ * (shadow rays to many lights with unit directions and t_max = each light's distance, per-ray near / far clipping, the
+ * closest hit over two prepared scenes by tracing the second with t_max = the first one's t).  rays_dev: device
+ * struct ray_b200_ray[n], 4-byte aligned (a 16-byte aligned buffer is read with 16-byte loads).
+ * The answer for ray i is exactly what the per-call entry point returns for that ray alone, called with
+ * (rays[i].t_min, rays[i].t_max).
+ * A ray whose t_min is not finite and >= 0 (-0.0 is valid), or whose t_max is not finite, is not an error (the host does
+ * not read the rays): it gets the empty answer that t_max <= t_min gives, t = -1 / sphere = -1 / p = normal = 0,
+ * occluded = 0, k empty records and a count of 0, and the other rays are unaffected.  Errors are those of the per-call
+ * entry points without the interval checks: n outside [0, 2^30], a NULL buffer with n > 0, an invalid prepared scene,
+ * k outside [1, 64].  There is no ranged trace_paths: ray_colour uses (0, 1e9) for every segment.
+ * Continuing a multi-hit list past k from the last record's t is not exact: a sphere that straddles the new t_min gives
+ * its second root, records at exactly that t are dropped (the interval is open), and the stale boxes of the fixed-sweep
+ * refit make the set of reached leaves depend on the interval. */
+struct ray_b200_ray {
+  float o[3];   float t_min;   /* origin, near end of the interval */
+  float d[3];   float t_max;   /* direction (need not be normalised), far end */
+};              /* 32 bytes */
+int ray_b200_trace_hits_ranged(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                               const struct ray_b200_ray *rays_dev, int64_t n, struct ray_b200_hit *hits_dev);
+int ray_b200_trace_occluded_ranged(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                                   const struct ray_b200_ray *rays_dev, int64_t n, uint8_t *occluded_dev);
+int ray_b200_trace_multi_hits_ranged(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                                     const struct ray_b200_ray *rays_dev, int64_t n, int32_t k,
+                                     struct ray_b200_hit *hits_dev, int32_t *counts_dev);
+/* sizeof(struct ray_b200_ray) as the library was compiled (32). */
+int64_t ray_b200_ray_size(void);
 
 /* ---- multi-GPU tile sharding (one process per GPU; the gather itself is NCCL, done by the host) -- */
 /* Number of 8x4 tiles rank `rank` of `world` owns for an h x w image, and the padded per-rank count

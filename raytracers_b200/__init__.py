@@ -20,7 +20,7 @@ import os
 
 import numpy as np
 
-__all__ = ["Context", "RayError", "Hit", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
+__all__ = ["Context", "RayError", "Hit", "Ray", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
            "host_camera", "host_lbvh", "host_sample_offsets", "camera_rays"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -67,7 +67,17 @@ class Hit(C.Structure):
     _fields_ = [("t", C.c_float), ("sphere", C.c_int32), ("p", C.c_float * 3), ("normal", C.c_float * 3)]
 
 
+class Ray(C.Structure):
+    """struct ray_b200_ray (include/ray_b200.h): a ray with its own interval, 32 bytes; the rows of an [n, 8] float32
+    tensor of rays (origin, t_min, direction, t_max)."""
+    _fields_ = [("o", C.c_float * 3), ("t_min", C.c_float), ("d", C.c_float * 3), ("t_max", C.c_float)]
+
+
 _libs = {}
+
+
+def _or(value, default):
+    return default if value is None else value
 
 
 def load_library(variant=""):
@@ -149,6 +159,10 @@ def load_library(variant=""):
         "ray_b200_trace_occluded": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
         "ray_b200_trace_multi_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, i32, vp, vp]),
         "ray_b200_hit_size": (i64, []),
+        "ray_b200_trace_hits_ranged": (C.c_int, [vp, vp, vp, i64, vp]),
+        "ray_b200_trace_occluded_ranged": (C.c_int, [vp, vp, vp, i64, vp]),
+        "ray_b200_trace_multi_hits_ranged": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_ray_size": (i64, []),
         "ray_b200_count_work": (C.c_int, [vp, i64, i64, i32, vp, C.POINTER(WorkCounters)]),
         "ray_b200_ipc_alloc": (C.c_int, [vp, i64, pp, vp]),
         "ray_b200_ipc_free": (C.c_int, [vp, vp]),
@@ -639,31 +653,60 @@ class Context:
         self._check(self.lib.ray_b200_trace_multi_hits(self.handle, prepared.handle, _ptr(rays_dev), int(n), float(t_min),
                                                        float(t_max), int(k), _ptr(hits_dev), _ptr(counts_dev)))
 
-    def _rays_tensor(self, rays):
+    def trace_hits_ranged_into(self, rays_dev, n, prepared, hits_dev):
+        """trace_hits_into for rays that carry their own interval: rays_dev = device Ray[n] (float[n][8]: origin, t_min,
+        direction, t_max), 4-byte aligned.  A ray whose interval the per-call form would reject (t_min not finite and
+        >= 0, t_max not finite) gets the empty record.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_trace_hits_ranged(self.handle, prepared.handle, _ptr(rays_dev), int(n), _ptr(hits_dev)))
+
+    def trace_occluded_ranged_into(self, rays_dev, n, prepared, out_dev):
+        """trace_occluded_into for rays that carry their own interval (device Ray[n]); an invalid interval gives 0."""
+        self._check(self.lib.ray_b200_trace_occluded_ranged(self.handle, prepared.handle, _ptr(rays_dev), int(n), _ptr(out_dev)))
+
+    def trace_multi_hits_ranged_into(self, rays_dev, n, prepared, k, hits_dev, counts_dev=None):
+        """trace_multi_hits_into for rays that carry their own interval (device Ray[n]); an invalid interval gives k
+        empty records and a count of 0."""
+        self._check(self.lib.ray_b200_trace_multi_hits_ranged(self.handle, prepared.handle, _ptr(rays_dev), int(n), int(k),
+                                                              _ptr(hits_dev), _ptr(counts_dev)))
+
+    def _rays_tensor(self, rays, ranged_ok=False, t_min=None, t_max=None):
+        """Checks a tensor of rays: [n, 6] (origin, direction) or, where ranged_ok, [n, 8] (Ray: origin, t_min,
+        direction, t_max), which carries its own interval and so takes no t_min= / t_max=.  Returns (torch, ranged)."""
         import torch
+        widths = (6, 8) if ranged_ok else (6,)
+        shapes = " or ".join(f"[n, {w}]" for w in widths)
+        if isinstance(rays, torch.Tensor) and (rays.dim() != 2 or rays.shape[1] not in widths):
+            raise ValueError(f"rays must be a contiguous float32 tensor of shape {shapes}, got {rays.dtype} {tuple(rays.shape)}")
+        ranged = isinstance(rays, torch.Tensor) and rays.shape[1] == 8
+        if ranged and (t_min is not None or t_max is not None):
+            raise ValueError("rays of shape [n, 8] carry their own (t_min, t_max): pass t_min= / t_max= only with [n, 6] rays")
         if not isinstance(rays, torch.Tensor) or rays.device.type != "cuda" or rays.device.index != self.device:
             raise ValueError(f"rays must be a CUDA tensor on cuda:{self.device}")
-        if rays.dtype != torch.float32 or rays.dim() != 2 or rays.shape[1] != 6 or not rays.is_contiguous():
-            raise ValueError(f"rays must be a contiguous float32 tensor of shape [n, 6], got {rays.dtype} {tuple(rays.shape)}")
+        if rays.dtype != torch.float32 or not rays.is_contiguous():
+            raise ValueError(f"rays must be a contiguous float32 tensor of shape {shapes}, got {rays.dtype} {tuple(rays.shape)}")
         # the rays may still be in flight on torch's stream, which the context's own stream is not ordered after
         torch.cuda.current_stream(rays.device).synchronize()
-        return torch
+        return torch, ranged
 
-    def trace_hits(self, prepared, rays, t_min=0.0, t_max=1e9):
-        """Closest hits of a [n, 6] float32 CUDA tensor of rays.  Returns dict(t [n], sphere [n] int32, p [n, 3],
-        normal [n, 3]): views of one [n, 8] buffer of Hit records.  t = -1 and sphere = -1 where a ray hits nothing.
-        Waits for torch's current stream before, and synchronises the context after the query."""
-        torch = self._rays_tensor(rays)
+    def trace_hits(self, prepared, rays, t_min=None, t_max=None):
+        """Closest hits of a [n, 6] float32 CUDA tensor of rays in (t_min, t_max) (default (0, 1e9)), or of a [n, 8] one
+        whose rays carry their own interval (Ray; no t_min= / t_max= then).  Returns dict(t [n], sphere [n] int32,
+        p [n, 3], normal [n, 3]): views of one [n, 8] buffer of Hit records.  t = -1 and sphere = -1 where a ray hits
+        nothing.  Waits for torch's current stream before, and synchronises the context after the query."""
+        torch, ranged = self._rays_tensor(rays, True, t_min, t_max)
         n = rays.shape[0]
         buf = torch.empty((n, 8), dtype=torch.float32, device=rays.device)
-        self.trace_hits_into(rays.data_ptr(), n, prepared, buf.data_ptr(), t_min=t_min, t_max=t_max)
+        if ranged:
+            self.trace_hits_ranged_into(rays.data_ptr(), n, prepared, buf.data_ptr())
+        else:
+            self.trace_hits_into(rays.data_ptr(), n, prepared, buf.data_ptr(), t_min=_or(t_min, 0.0), t_max=_or(t_max, 1e9))
         self.sync()
         return {"t": buf[:, 0], "sphere": buf[:, 1].view(torch.int32), "p": buf[:, 2:5], "normal": buf[:, 5:8]}
 
     def trace_paths(self, prepared, rays, max_depth=50):
         """Colours of a [n, 6] float32 CUDA tensor of rays: (rgb [n, 3] float32, segments [n] int32 = objs_hit calls of
         every path).  Waits for torch's current stream before, and synchronises the context after the query."""
-        torch = self._rays_tensor(rays)
+        torch, _ = self._rays_tensor(rays)
         n = rays.shape[0]
         rgb = torch.empty((n, 3), dtype=torch.float32, device=rays.device)
         seg = torch.empty((n,), dtype=torch.int32, device=rays.device)
@@ -671,25 +714,34 @@ class Context:
         self.sync()
         return rgb, seg
 
-    def trace_occluded(self, prepared, rays, t_min=0.0, t_max=1e9):
-        """Occlusion of a [n, 6] float32 CUDA tensor of rays: torch.bool [n].  Waits for torch's current stream before,
-        and synchronises the context after the query."""
-        torch = self._rays_tensor(rays)
+    def trace_occluded(self, prepared, rays, t_min=None, t_max=None):
+        """Occlusion of a [n, 6] float32 CUDA tensor of rays in (t_min, t_max) (default (0, 1e9)), or of a [n, 8] one
+        whose rays carry their own interval: torch.bool [n].  Waits for torch's current stream before, and synchronises
+        the context after the query."""
+        torch, ranged = self._rays_tensor(rays, True, t_min, t_max)
         n = rays.shape[0]
         out = torch.empty((n,), dtype=torch.bool, device=rays.device)
-        self.trace_occluded_into(rays.data_ptr(), n, prepared, out.data_ptr(), t_min=t_min, t_max=t_max)
+        if ranged:
+            self.trace_occluded_ranged_into(rays.data_ptr(), n, prepared, out.data_ptr())
+        else:
+            self.trace_occluded_into(rays.data_ptr(), n, prepared, out.data_ptr(), t_min=_or(t_min, 0.0), t_max=_or(t_max, 1e9))
         self.sync()
         return out
 
-    def trace_multi_hits(self, prepared, rays, k, t_min=0.0, t_max=1e9):
-        """The k nearest sphere intersections of a [n, 6] float32 CUDA tensor of rays.  Returns dict(t [n, k],
-        sphere [n, k] int32, p [n, k, 3], normal [n, k, 3], count [n] int32): the first four are views of one [n, k, 8]
-        buffer of Hit records.  Waits for torch's current stream before, and synchronises the context after the query."""
-        torch = self._rays_tensor(rays)
+    def trace_multi_hits(self, prepared, rays, k, t_min=None, t_max=None):
+        """The k nearest sphere intersections of a [n, 6] float32 CUDA tensor of rays in (t_min, t_max) (default
+        (0, 1e9)), or of a [n, 8] one whose rays carry their own interval.  Returns dict(t [n, k], sphere [n, k] int32,
+        p [n, k, 3], normal [n, k, 3], count [n] int32): the first four are views of one [n, k, 8] buffer of Hit records.
+        Waits for torch's current stream before, and synchronises the context after the query."""
+        torch, ranged = self._rays_tensor(rays, True, t_min, t_max)
         n = rays.shape[0]
         buf = torch.empty((n, int(k), 8), dtype=torch.float32, device=rays.device)
         count = torch.empty((n,), dtype=torch.int32, device=rays.device)
-        self.trace_multi_hits_into(rays.data_ptr(), n, prepared, k, buf.data_ptr(), count.data_ptr(), t_min=t_min, t_max=t_max)
+        if ranged:
+            self.trace_multi_hits_ranged_into(rays.data_ptr(), n, prepared, k, buf.data_ptr(), count.data_ptr())
+        else:
+            self.trace_multi_hits_into(rays.data_ptr(), n, prepared, k, buf.data_ptr(), count.data_ptr(), t_min=_or(t_min, 0.0),
+                                       t_max=_or(t_max, 1e9))
         self.sync()
         return {"t": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "p": buf[..., 2:5], "normal": buf[..., 5:8],
                 "count": count}

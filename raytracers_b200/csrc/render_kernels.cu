@@ -153,6 +153,15 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // warp-private and a ray is claimed once, so no other warp touches the list.  Node batches are those of the closest-hit
 // kinds: no box is pruned by the k-th t, because the count needs the whole set.  The owner lane turns the keys into hit
 // records (sphere through Q.perm), fills the rest with empty records, writes Q.counts and frees the slot.
+//
+// kRanged (ray mode, hit / occlusion / multi-hit queries): every ray carries its own interval.  Q.rays is [n][8]
+// (struct ray_b200_ray: origin, t_min, direction, t_max), and the per-slot interval takes the place of the query's
+// (t_min, t_max) in the root test, the node batch, the leaf batch and the closest-hit finish.  An invalid interval (t_min
+// not finite and >= 0, or t_max not finite) becomes (0, 0), which no box passes (tmin >= 0 >= tmax), so the root-miss
+// exits write the empty answer.  No shared memory is added: the interval takes the .w words of the slot's float4s that
+// the node batch loads anyway, ray_o.w = t_min and ray_i.w = t_max, and a = dot(d, d), which box tests do not use, moves
+// to ray_d.w (the leaf batch loads ray_d).  Ranged variants exist only as a separate template instantiation, so the
+// per-call variants keep their code.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -163,12 +172,13 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels>
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   constexpr bool kRays = kQuery != Query::kPixels;  // ray mode
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
+  static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -198,9 +208,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     gt_mask = lane == 31 ? 0u : ~((2u << lane) - 1u);
   }
   unsigned char *wbase = smem_raw + ((staging_bytes(P) + 127) & ~(size_t)127) + (size_t)warp * wq_warp_bytes(K, ncap_arg, kPacket, kSpread);
-  float4 *ray_o = reinterpret_cast<float4 *>(wbase);   // {o.xyz, a = dot d d}
-  float4 *ray_i = ray_o + R;                           // {1/d.xyz, 0}
-  float4 *ray_d = ray_i + R;                           // {d.xyz, 0}
+  float4 *ray_o = reinterpret_cast<float4 *>(wbase);   // {o.xyz, a = dot d d}     kRanged: {o.xyz, t_min}
+  float4 *ray_i = ray_o + R;                           // {1/d.xyz, 0}             kRanged: {1/d.xyz, t_max}
+  float4 *ray_d = ray_i + R;                           // {d.xyz, 0}               kRanged: {d.xyz, a} (t_max until the root test)
   float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth)}   owner lane only
   float4 *p_sum = p_light + R;                         // pixel-bound samples: {sum.rgb, bits(sample)}
   int *p_ms = reinterpret_cast<int *>(p_light + R);    // spread samples: ring entry << 16 | sample (4 bytes per slot instead of 16)
@@ -217,7 +227,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
 
   const int total = kRays ? Q.n : (int)(P.local_tiles * kTilePixels);
   const int total_claims = kRays ? Q.n : P.n_chunks << 11;
-  // the query's interval (ray mode) or the literal one of ray_colour (ray.fut:130)
+  // the query's interval (ray mode; kRanged: each slot's own instead) or the literal one of ray_colour (ray.fut:130)
   const float t_lo = kRays ? Q.t_min : 0.0f, t_hi = kRays ? Q.t_max : 1000000000.0f;
   const int spp = P.spp;
 #pragma unroll
@@ -393,7 +403,23 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               const int c = base + rank++;
               const int item = c < total_claims ? (kRays ? c : claim_to_item(P, c)) : total;
               int pi, pj;
-              if (kRays && item < total) {
+              if (kRanged && item < total) {
+                // struct ray_b200_ray (64-bit offset: n reaches 2^30); a 16-byte aligned buffer takes two 16-byte loads
+                const float *rp = Q.rays + 8 * (size_t)item;
+                float4 a, b;
+                if ((reinterpret_cast<uintptr_t>(Q.rays) & 15u) == 0) {
+                  a = reinterpret_cast<const float4 *>(rp)[0];
+                  b = reinterpret_cast<const float4 *>(rp)[1];
+                } else {
+                  a = make_float4(rp[0], rp[1], rp[2], rp[3]);
+                  b = make_float4(rp[4], rp[5], rp[6], rp[7]);
+                }
+                // the empty answer for an interval the per-call entry points reject: (0, 0) passes no box
+                const bool valid = isfinite(a.w) && a.w >= 0.0f && isfinite(b.w);
+                p_item[slot] = item;
+                ray_o[slot] = make_float4(a.x, a.y, a.z, valid ? a.w : 0.0f);
+                ray_d[slot] = make_float4(b.x, b.y, b.z, valid ? b.w : 0.0f);
+              } else if (kRays && item < total) {
                 const float *rp = Q.rays + 6 * (size_t)item;
                 p_item[slot] = item;
                 ray_o[slot] = make_float4(rp[0], rp[1], rp[2], 0.0f);
@@ -475,9 +501,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             r.o = v3(ro.x, ro.y, ro.z);
             r.d = v3(rd.x, rd.y, rd.z);
             const RayInv q = ray_invariants(r);
-            if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, t_lo, t_hi)) {
-              ray_o[slot] = make_float4(ro.x, ro.y, ro.z, q.a);
-              ray_i[slot] = make_float4(q.ix, q.iy, q.iz, 0.0f);
+            const float lo = kRanged ? ro.w : t_lo, hi = kRanged ? rd.w : t_hi;
+            if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, lo, hi)) {
+              if constexpr (kRanged) {
+                ray_i[slot] = make_float4(q.ix, q.iy, q.iz, hi);
+                ray_d[slot] = make_float4(rd.x, rd.y, rd.z, q.a);
+              } else {
+                ray_o[slot] = make_float4(ro.x, ro.y, ro.z, q.a);
+                ray_i[slot] = make_float4(q.ix, q.iy, q.iz, 0.0f);
+              }
               best_t[slot] = kQuery == Query::kMultiHit ? 0u : kItemNoHit;  // multi-hit: no accepted leaf yet
               go = true;
               break;
@@ -490,7 +522,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             } else if constexpr (kQuery == Query::kMultiHit) {  // k empty records, count 0
               finish_multi(slot, 0u);
               continue;
-            } else if (kQuery == Query::kClosest && Q.hits) {  // no hit
+            } else if (kQuery == Query::kClosest && (kRanged || Q.hits)) {  // no hit (paths have no ranged form)
               finish_hit(slot, -1.0f, -1, v3(0.0f, 0.0f, 0.0f), v3(0.0f, 0.0f, 0.0f));
               continue;
             }
@@ -548,7 +580,13 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
           Ray r;
           r.o = v3(ro.x, ro.y, ro.z);
           r.d = v3(rd.x, rd.y, rd.z);
-          const float t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, kEpsilon ? 0.1f : t_lo, t_hi);  // epsilon: ray.fut:79
+          float a = ro.w, lo = kEpsilon ? 0.1f : t_lo, hi = t_hi;  // epsilon: ray.fut:79
+          if constexpr (kRanged) {
+            a = rd.w;
+            hi = ray_i[slot].w;
+            if (!kEpsilon) lo = ro.w;
+          }
+          const float t = sphere_t(g.x, g.y, g.z, g.w, r, a, lo, hi);
           hit = t >= 0.0f;
           tb = __float_as_uint(t);
         }
@@ -595,8 +633,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
           q.ix = ri.x; q.iy = ri.y; q.iz = ri.z; q.a = ro.w;
           lptr = __float_as_int(q0.w);
           rptr = __float_as_int(q1.w);
-          const bool hl = box_hit(q0.x, q0.y, q0.z, q1.x, q1.y, q1.z, r, q, t_lo, t_hi);
-          const bool hr = box_hit(q2.x, q2.y, q2.z, q3.x, q3.y, q3.z, r, q, t_lo, t_hi);
+          const float lo = kRanged ? ro.w : t_lo, hi = kRanged ? ri.w : t_hi;
+          const bool hl = box_hit(q0.x, q0.y, q0.z, q1.x, q1.y, q1.z, r, q, lo, hi);
+          const bool hr = box_hit(q2.x, q2.y, q2.z, q3.x, q3.y, q3.z, r, q, lo, hi);
           pl_leaf = lptr < 0;          // a leaf child has no box in the reference: always visited
           pr_leaf = rptr < 0;
           pl_node = hl && !pl_leaf;
@@ -762,13 +801,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       int depth = __float_as_int(pl.w);
       const int j = bt == kItemNoHit ? -1 : (int)best_l[slot];
       const float tb = __uint_as_float(bt);
-      if (kQuery == Query::kClosest && Q.hits) {
-        // objs_hit, second half (ray.fut:83-85) with the query's t_min; a failed re-intersection is no hit
+      if (kQuery == Query::kClosest && (kRanged || Q.hits)) {
+        // objs_hit, second half (ray.fut:83-85) with the query's (kRanged: the ray's) t_min; a failed re-intersection is
+        // no hit
         float t = -1.0f;
         V3 p = v3(0.0f, 0.0f, 0.0f), n = p;
         if (j >= 0) {
           const float4 g = sc.sphere(j);
-          t = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, Q.t_min, tb + 1.0f);
+          t = kRanged ? sphere_t(g.x, g.y, g.z, g.w, r, rd.w, ro.w, tb + 1.0f)
+                      : sphere_t(g.x, g.y, g.z, g.w, r, ro.w, Q.t_min, tb + 1.0f);
           if (t >= 0.0f) {
             p = vadd(r.o, vscale(t, r.d));                            // point_at_param, ray.fut:14-15
             n = vscale(1.0f / g.w, vsub(p, v3(g.x, g.y, g.z)));       // ray.fut:42-43
@@ -846,13 +887,13 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   }
   if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
   if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  return launch_warpqueue(p, Query::kPixels, RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
+  return launch_warpqueue(p, Query::kPixels, false, RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
 }
 
 // K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query of kind `kind`: the
-// same kernel in ray mode, without spread samples or packets.
-cudaError_t launch_warpqueue(const RenderParams &p, Query kind, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
-                             int64_t *launches) {
+// same kernel in ray mode, without spread samples or packets; `ranged`: its rays carry their own intervals.
+cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
+                             cudaStream_t stream, int64_t *launches) {
   const bool rays = kind != Query::kPixels;
   const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
   // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
@@ -873,10 +914,10 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, const RayQuery &
   cudaError_t e;
   if (rays)
     e = with_query([&](auto query) {
-      return with_flags([&](auto k2, auto a, auto s) {
-        return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, query>>(
+      return with_flags([&](auto k2, auto a, auto s, auto rg) {
+        return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, query, rg>>(
             lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
-      }, k == 2, all_nodes, sph);
+      }, k == 2, all_nodes, sph, ranged);
     }, kind);
   else
     e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {

@@ -67,13 +67,14 @@ enum class Query { kPixels, kClosest, kAnyHit, kMultiHit };
 // of its own, passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those
 // parameters, and with them the constant-bank offsets in every pixel instantiation's code.
 struct RayQuery {
-  const float *rays;        // [n][6]: origin.xyz, dir.xyz
+  const float *rays;        // [n][6]: origin.xyz, dir.xyz; ranged query: [n][8] = struct ray_b200_ray
   float *rgb;               // path query: [n][3] colour of ray_colour (ray.fut:126-148)
   int32_t *segments;        // path query, optional: [n] objs_hit calls of the path
   float *hits;              // hit query (non-NULL = hit mode): [n][8] struct ray_b200_hit; multi-hit query: [n][k][8]
   const int32_t *perm;      // Morton-sorted leaf -> index into the caller's sphere array
   int32_t n;
-  float t_min, t_max;       // hit / occlusion / multi-hit query: the call's interval; path query: (0, 1e9) as ray_colour passes it
+  float t_min, t_max;       // hit / occlusion / multi-hit query: the call's interval (unused when ranged: each ray has
+                            // its own); path query: (0, 1e9) as ray_colour passes it
   int32_t max_depth;        // path query: the depth limit of ray_colour (1 for the one-segment queries)
   uint8_t *occluded;        // occlusion query: [n] 0 / 1
   int32_t k;                // multi-hit query: records per ray, in [1, 64]
@@ -123,9 +124,9 @@ struct LaunchConfig {
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches);
 // The warp-queue kernel (render_kernels.cu): a pixel frame (kind = Query::kPixels, q unused), or a ray query of that kind
-// (whatever lc.kernel says)
-cudaError_t launch_warpqueue(const RenderParams &p, Query kind, const RayQuery &q, const LaunchConfig &lc, cudaStream_t stream,
-                             int64_t *launches);
+// (whatever lc.kernel says); `ranged`: q.rays is [n][8] with an interval per ray (hit, occlusion and multi-hit queries)
+cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
+                             cudaStream_t stream, int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
 // build without RAYB200_ALL_KERNELS returns cudaErrorNotSupported)
 cudaError_t launch_lanewalk(const RenderParams &p, const LaunchConfig &lc, cudaStream_t stream, int64_t *launches);

@@ -15,14 +15,24 @@
 - rays_irreg_multi{1,4,16}_4M, rays_random1M_multi4_4M: the random rays of the hit workloads through trace_multi_hits
   with k = 1, 4, 16 (irreg) and k = 4 (1 M spheres), interval (0.1, 1e9);
 - depth_irreg_1000_multi8: irreg's 1000x1000 camera rays through trace_multi_hits with k = 8 and the interval (0, 1e9),
-  a depth-complexity query.
+  a depth-complexity query;
+- rays_{irreg,random1M}_{hits,occluded,multi4}_ranged_4M: the random rays of the hit workloads, each carrying the interval
+  (0.1, 1e9), through the ranged entry points (k = 4), with the per-call entry point on the same rays and interval beside
+  it (`percall_ms`): the cost of carrying the interval per ray;
+- lights4_irreg_1000: irreg's 1000x1000 camera rays through trace_hits, then from every hit point a shadow ray toward one
+  of four lights above the scene, chosen per ray, with a unit direction and the interval (1e-2, distance - 1e-4),
+  through trace_occluded_ranged; beside it (`segment_ms`) the same segments in the per-call form (direction = light -
+  point, (1e-4, 1 - 1e-4)) through trace_occluded.  The two forms round differently, so each has its own parity.
+  In these records both times are the smaller of two medians, the two forms alternated (ranged, per-call, ranged,
+  per-call).
 An occlusion or multi-hit record has trace_hits' time on the same rays and interval beside its own (`hits_ms`), and the
 fraction of rays occluded or the mean count of a multi-hit query; its Mrays/s counts one ray per query.
 Random rays come from a fixed seed: origins uniform in the scene's bounding box expanded by 10 % per side, directions
 uniform on the sphere, so every run sees the same inputs.  `ms` = the median of 3 queries (CUDA events of the context,
 after one warm-up query that loads the kernel); Mrays/s = objs_hit calls / kernel time (one per ray for a hit query, the
 segments trace_paths reports for a path query); `parity` = differing values against the CPU oracle
-(tests/ray_query_oracle.py) on 4096 rays spread over the batch.  The card's name and power limit are read in the same run.
+(tests/ray_query_oracle.py; tests/ray_interval_oracle.py for the ranged queries) on 4096 rays spread over the batch.
+The card's name and power limit are read in the same run.
 """
 import argparse
 import json
@@ -44,6 +54,77 @@ def random_rays(np, spheres, count, seed):
     return np.ascontiguousarray(np.concatenate([o, d / np.linalg.norm(d, axis=1, keepdims=True)], 1), np.float32)
 
 
+def ranged_workload(np, torch, R, Q, RQ, ctx, timed, bits, name, n_spheres, hh, ww, sc, pr, mode, k, args):
+    """One workload of rays that carry their own interval (struct ray_b200_ray), with the per-call form beside it."""
+    o = Q.prepare(name, hh, ww, n=n_spheres)            # the per-call queries
+    ro = RQ.prepare(name, hh, ww, n=n_spheres)          # the ranged ones
+    if mode == "lights":
+        cam = torch.from_numpy(R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6)).cuda()
+        hit = ctx.trace_hits(pr, cam)
+        p = hit["p"].cpu().numpy()[hit["t"].cpu().numpy() >= 0]
+        s = sc.arrays()[0]
+        lo, hi = (s[:, :3] - s[:, 6:7]).min(0), (s[:, :3] + s[:, 6:7]).max(0)
+        c, ext = (lo + hi) / 2, hi - lo
+        lights = np.float32([[c[0] + sx * ext[0] / 4, hi[1] + max(ext[0], ext[2]) / 4, c[2] + sz * ext[2] / 4]
+                             for sx in (-1, 1) for sz in (-1, 1)])   # the construction of tests/test_ray_intervals.py
+        v = lights[np.random.default_rng(args.seed).integers(0, 4, p.shape[0])] - p
+        dist = np.sqrt((v * v).sum(1, dtype=np.float32)).astype(np.float32)
+        rays8 = np.concatenate([p, np.full((p.shape[0], 1), 1e-2, np.float32), v / dist[:, None], (dist - np.float32(1e-4))[:, None]], 1)
+        rays6 = np.concatenate([p, v], 1)   # the per-call segment form of the same rays
+        t_min, t_max = 1e-4, 1 - 1e-4
+    else:
+        rays6 = random_rays(np, sc.arrays()[0], args.rays, args.seed)
+        t_min, t_max = 0.1, 1e9
+        rays8 = np.concatenate([rays6[:, :3], np.full((rays6.shape[0], 1), t_min, np.float32), rays6[:, 3:],
+                                np.full((rays6.shape[0], 1), t_max, np.float32)], 1)
+    rays6, rays8 = np.ascontiguousarray(rays6, np.float32), np.ascontiguousarray(rays8, np.float32)
+    cnt = rays8.shape[0]
+    d6, d8 = torch.from_numpy(rays6).cuda(), torch.from_numpy(rays8).cuda()
+    kk = max(k, 1)
+    out6 = torch.empty((cnt, kk, 8), dtype=torch.float32, device="cuda")
+    out8 = torch.empty((cnt, kk, 8), dtype=torch.float32, device="cuda")
+    c6 = torch.empty((cnt,), dtype=torch.int32, device="cuda")
+    c8 = torch.empty((cnt,), dtype=torch.int32, device="cuda")
+    occ6 = torch.empty((cnt,), dtype=torch.bool, device="cuda")
+    occ8 = torch.empty((cnt,), dtype=torch.bool, device="cuda")
+    torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
+    if mode == "hits_r":
+        ranged_q = lambda: ctx.trace_hits_ranged_into(d8.data_ptr(), cnt, pr, out8.data_ptr())
+        per_call = lambda: ctx.trace_hits_into(d6.data_ptr(), cnt, pr, out6.data_ptr(), t_min=t_min, t_max=t_max)
+    elif mode == "multi_r":
+        ranged_q = lambda: ctx.trace_multi_hits_ranged_into(d8.data_ptr(), cnt, pr, k, out8.data_ptr(), c8.data_ptr())
+        per_call = lambda: ctx.trace_multi_hits_into(d6.data_ptr(), cnt, pr, k, out6.data_ptr(), c6.data_ptr(), t_min=t_min, t_max=t_max)
+    else:
+        ranged_q = lambda: ctx.trace_occluded_ranged_into(d8.data_ptr(), cnt, pr, occ8.data_ptr())
+        per_call = lambda: ctx.trace_occluded_into(d6.data_ptr(), cnt, pr, occ6.data_ptr(), t_min=t_min, t_max=t_max)
+    # alternated, so that both forms see the same clocks: ranged, per-call, ranged, per-call
+    ms, ms_call = timed(ranged_q), timed(per_call)
+    ms, ms_call = min(ms, timed(ranged_q)), min(ms_call, timed(per_call))
+    rec = {"rays": cnt, "ms": round(ms, 3), "Mrays_s": round(cnt / ms / 1e3, 1)}
+    rec["percall_ms" if mode != "lights" else "segment_ms"] = round(ms_call, 3)
+    rec["ranged_over_percall" if mode != "lights" else "ranged_over_segment"] = round(ms / ms_call, 3)
+    if mode != "lights":
+        rec["t_min"], rec["t_max"] = t_min, t_max
+    sub = np.linspace(0, cnt - 1, 4096).astype(np.int64)
+    if mode == "hits_r":
+        rec["parity"] = int((bits(out8[:, 0].cpu().numpy()[sub]) != bits(ro.trace_hits_ranged(rays8[sub]))).sum())
+        rec["percall_parity"] = int((bits(out6[:, 0].cpu().numpy()[sub]) != bits(o.trace_hits(rays6[sub], t_min, t_max))).sum())
+    elif mode == "multi_r":
+        want, want_c = ro.trace_multi_hits_ranged(rays8[sub], k)
+        rec["parity"] = int((bits(out8.cpu().numpy()[sub]) != bits(want)).sum()) + int((c8.cpu().numpy()[sub] != want_c).sum())
+        want, want_c = o.trace_multi_hits(rays6[sub], k, t_min, t_max)
+        rec["percall_parity"] = int((bits(out6.cpu().numpy()[sub]) != bits(want)).sum()) + int((c6.cpu().numpy()[sub] != want_c).sum())
+        rec["k"], rec["mean_count"] = k, round(float(c8.double().mean()), 3)
+    else:
+        occ8, occ6 = occ8.cpu().numpy(), occ6.cpu().numpy()
+        rec["parity"] = int((occ8[sub] != ro.trace_occluded_ranged(rays8[sub])).sum())
+        rec["percall_parity" if mode != "lights" else "segment_parity"] = int((occ6[sub] != o.trace_occluded(rays6[sub], t_min, t_max)).sum())
+        rec["occluded_fraction"] = round(float(occ8.mean()), 4)
+        if mode == "lights":
+            rec["segment_occluded_fraction"] = round(float(occ6.mean()), 4)
+    return rec
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rays", type=int, default=1 << 22)
@@ -54,6 +135,7 @@ def main():
     import torch
 
     import ray_query_oracle as Q
+    import ray_interval_oracle as RQ
     import raytracers_b200 as R
 
     def bits(a):
@@ -85,12 +167,23 @@ def main():
                                                   ("rays_irreg_multi4_4M", "irreg", None, 1000, 1000, "multi", 4),
                                                   ("rays_irreg_multi16_4M", "irreg", None, 1000, 1000, "multi", 16),
                                                   ("rays_random1M_multi4_4M", "random", 1000000, 2000, 2000, "multi", 4),
-                                                  ("depth_irreg_1000_multi8", "irreg", None, 1000, 1000, "depth", 8)):
+                                                  ("depth_irreg_1000_multi8", "irreg", None, 1000, 1000, "depth", 8),
+                                                  ("rays_irreg_hits_ranged_4M", "irreg", None, 1000, 1000, "hits_r", 0),
+                                                  ("rays_irreg_occluded_ranged_4M", "irreg", None, 1000, 1000, "occluded_r", 0),
+                                                  ("rays_irreg_multi4_ranged_4M", "irreg", None, 1000, 1000, "multi_r", 4),
+                                                  ("rays_random1M_hits_ranged_4M", "random", 1000000, 2000, 2000, "hits_r", 0),
+                                                  ("rays_random1M_occluded_ranged_4M", "random", 1000000, 2000, 2000, "occluded_r", 0),
+                                                  ("rays_random1M_multi4_ranged_4M", "random", 1000000, 2000, 2000, "multi_r", 4),
+                                                  ("lights4_irreg_1000", "irreg", None, 1000, 1000, "lights", 0)):
         if args.only and tag not in args.only.split(","):
             continue
         sc = ctx.scene(name, n=n_spheres)
         pr = ctx.prepare_scene(hh, ww, sc)
         t_min, t_max = (1e-4, 1 - 1e-4) if mode == "shadow" else ((0.0, 1e9) if mode == "depth" else (0.1, 1e9))
+        if mode in ("hits_r", "occluded_r", "multi_r", "lights"):
+            out[tag] = ranged_workload(np, torch, R, Q, RQ, ctx, timed, bits, name, n_spheres, hh, ww, sc, pr, mode, k, args)
+            pr.free(); sc.free()
+            continue
         if mode in ("camera", "shadow", "depth"):
             rays = R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6)
         else:
