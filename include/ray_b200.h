@@ -127,6 +127,28 @@ int ray_b200_render_into(struct futhark_context *ctx, int32_t *out_pix_dev, floa
  * This is the call bench.py's e2e leg times. */
 int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, float *out_rgb_host, int64_t h,
                          int64_t w, int32_t spp, const struct futhark_opaque_prepared_scene *p);
+/* Progressive rendering: samples [s_begin, s_end) of every pixel of an h x w frame, added to a running sum, so that a
+ * caller can show a preview after a few samples and refine it without re-tracing anything.
+ * accum_dev: device float[h][w][3], row-major.  On entry, when s_begin > 0, it holds each pixel's running sum (for
+ * example from earlier calls); it is not read when s_begin == 0.  On return it holds sum + colour_{s_begin} + ... +
+ * colour_{s_end-1}, added one sample at a time in sample order in f32.  When s_begin == 0 the sum starts as colour_0
+ * itself, not 0 + colour_0 (this keeps -0.0).  out_pix_dev / out_rgb_dev (each may be NULL): the frame at spp = s_end,
+ * exactly what ray_b200_render_into(spp = s_end) writes.
+ *   Exactness: any chain of calls [0, a), [a, b), ..., [y, S) on one buffer leaves the same accum as one call [0, S), bit
+ *   for bit, and its pixels and float framebuffer equal ray_b200_render_into(spp = S) (NaN-aware: a NaN is some NaN).
+ *   The sum read at s_begin > 0 is whatever the caller left in the buffer; the result is the f32 arithmetic above on it.
+ *   Sample s is sample s of the spp semantics above, whatever the chunking.
+ *   The call is asynchronous on the context's stream; stream order, the pipeline lanes, freeing the prepared scene while
+ *   the call is in flight, ray_b200_context_last_render_ms and ray_b200_context_launch_count (one launch per call) behave
+ *   as for ray_b200_render_into.  With a shard set (world > 1) only this rank's pixels of accum and of the outputs are
+ *   read or written, in the row-major layout; there is no tile-major form.
+ *   It runs on the warp-queue kernel whatever RAY_KERNEL or the context's kernel says (every kernel's frames are
+ *   bit-identical).
+ *   Errors (nonzero return, futhark_context_get_error; the context stays usable): every error of ray_b200_render_into
+ *   (an s_end it would reject as spp, a RAY_GPUS > 1 context, ...), s_begin < 0, s_end <= s_begin, accum_dev == NULL. */
+int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, int64_t h, int64_t w,
+                               int32_t s_begin, int32_t s_end, int32_t *out_pix_dev, float *out_rgb_dev,
+                               const struct futhark_opaque_prepared_scene *p);
 /* Like futhark_entry_render but with explicit spp (library-owned result). */
 int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d **out0, int64_t h, int64_t w,
                               int32_t spp, const struct futhark_opaque_prepared_scene *p);

@@ -149,6 +149,7 @@ def load_library(variant=""):
         "ray_b200_prepared_device_bytes": (i64, [vp, vp]),
         "ray_b200_render_into": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_host": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
+        "ray_b200_render_accumulate": (C.c_int, [vp, vp, i64, i64, i32, i32, vp, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
         "ray_b200_shard_tiles_padded": (i64, [i64, i64, i32]),
@@ -545,6 +546,35 @@ class Context:
 
     def render_into(self, out_pix_dev, h, w, prepared, spp=1, out_rgb_dev=None):
         self._check(self.lib.ray_b200_render_into(self.handle, _ptr(out_pix_dev), _ptr(out_rgb_dev), int(h), int(w), int(spp), prepared.handle))
+
+    def render_accumulate_into(self, accum_dev, h, w, prepared, s_begin, s_end, out_pix_dev=None, out_rgb_dev=None):
+        """Progressive rendering (ray_b200_render_accumulate): adds samples [s_begin, s_end) of every pixel to the running
+        sums in accum_dev (device float[h][w][3]; not read when s_begin == 0), in sample order, and writes the frame at
+        spp = s_end to out_pix_dev (device int32[h][w]) / out_rgb_dev (device float[h][w][3]) where given.  A chain of
+        calls [0, a), [a, b), ... equals one render at the total spp, bit for bit.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_render_accumulate(self.handle, _ptr(accum_dev), int(h), int(w), int(s_begin), int(s_end),
+                                                        _ptr(out_pix_dev), _ptr(out_rgb_dev), prepared.handle))
+
+    def render_accumulate(self, prepared, accum, s_begin, s_end, want_rgb=False):
+        """Adds samples [s_begin, s_end) of every pixel to accum, a contiguous float32 CUDA tensor [h, w, 3] on the
+        context's device that holds the running sums of samples [0, s_begin) (not read when s_begin == 0), and returns
+        the frame at spp = s_end: int32 [h, w] pixels, and with want_rgb also the float32 [h, w, 3] framebuffer, as
+        (pixels, rgb).  With a shard set, the pixels of other ranks are 0.  Waits for torch's current stream before, and
+        synchronises the context after the call."""
+        import torch
+        if not isinstance(accum, torch.Tensor) or accum.device.type != "cuda" or accum.device.index != self.device:
+            raise ValueError(f"accum must be a CUDA tensor on cuda:{self.device}")
+        if accum.dtype != torch.float32 or accum.dim() != 3 or accum.shape[2] != 3 or not accum.is_contiguous():
+            raise ValueError(f"accum must be a contiguous float32 tensor of shape [h, w, 3], got {accum.dtype} {tuple(accum.shape)}")
+        h, w = int(accum.shape[0]), int(accum.shape[1])
+        pix = torch.zeros((h, w), dtype=torch.int32, device=accum.device)
+        rgb = torch.zeros((h, w, 3), dtype=torch.float32, device=accum.device) if want_rgb else None
+        # accum may still be in flight on torch's stream, which the context's own stream is not ordered after
+        torch.cuda.current_stream(accum.device).synchronize()
+        self.render_accumulate_into(accum.data_ptr(), h, w, prepared, s_begin, s_end, pix.data_ptr(),
+                                    rgb.data_ptr() if rgb is not None else None)
+        self.sync()
+        return (pix, rgb) if want_rgb else pix
 
     def render_host(self, h, w, prepared, spp=1, want_rgb=False, out=None):
         pix = out if out is not None else np.empty((h, w), np.int32)

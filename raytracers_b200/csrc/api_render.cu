@@ -69,9 +69,13 @@ static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
   return lc;
 }
 
-// Fills the kernel parameter block for one frame, and the frame's launch plan.
+// Fills the kernel parameter block for one frame, and the frame's launch plan.  With `accum` the launch is one chunk of
+// a progressive frame: spp samples from accum->s_begin on, planned as a frame of spp samples (spread or pixel-bound by
+// the chunk length), read from the offset table of the whole frame at the chunk's first sample and scaled by
+// 1/s_end; it runs on the warp-queue kernel whatever the context's kernel is.
 int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
-                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc) {
+                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc,
+                const RayQuery *accum) {
   if (!p || !p->dev.nodes) { set_error(ctx, "render: invalid prepared scene"); return 1; }
   if (h <= 0 || w <= 0 || h > 65536 || w > 65536 || ((h + 3) / 4) * ((w + 7) / 8) > ((int64_t)1 << 25)) {
     // work items are 32-bit: at most 2^30 (padded) pixels per frame
@@ -81,13 +85,14 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   if (spp < 1) { set_error(ctx, "render: spp must be >= 1"); return 1; }
   if (world < 1 || rank < 0 || rank >= world) { set_error(ctx, "render: bad shard %d/%d", rank, world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
-  if (ensure_offsets(ctx, spp)) return 1;
+  const int32_t s_begin = accum ? accum->s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
+  if (ensure_offsets(ctx, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
   // h, w only set the pixel grid (ray.fut:246-247) — exactly as in the reference.
   memcpy(P.cam, &p->cam, sizeof P.cam);
-  P.W = (int32_t)w; P.H = (int32_t)h; P.spp = spp; P.inv_spp = 1.0f / (float)spp;
-  P.offsets = ctx->offsets;
+  P.W = (int32_t)w; P.H = (int32_t)h; P.spp = spp; P.inv_spp = 1.0f / (float)s_end;
+  P.offsets = ctx->offsets + 2 * (size_t)s_begin;
   P.out_pix = out_pix; P.out_rgb = out_rgb; P.tile_major = tile_major ? 1 : 0;
   P.rank = rank; P.world = world;
   P.tiles_x = (int32_t)((w + kTileW - 1) / kTileW); P.tiles_y = (int32_t)((h + kTileH - 1) / kTileH);
@@ -117,7 +122,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   // shared-memory staging plan: BFS prefix of the node array, then the sphere records if they all fit.
   // The warp-queue kernel runs one CTA per SM and gives the staging area whatever its queues leave.
   int64_t budget = std::min<int64_t>(ctx->cfg.smem_budget, ctx->max_smem_optin - 1024) - 128;
-  int kern = resolve_kernel(ctx);
+  int kern = accum ? RAY_B200_KERNEL_WARPQUEUE : resolve_kernel(ctx);
   if (kern == RAY_B200_KERNEL_LANEWALK && spp > 1) {
     // K5 traces one sample per slot and needs the finished-sample buffer (0.54 MB per sample on an H100); without it (spreading
     // switched off, or a sample count whose buffer exceeds the budget) the frame runs on the warp-queue kernel
@@ -330,8 +335,9 @@ static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64
 
 // Enqueues one frame with launch plan `lc` (fill_params) on lane `lane_id` (0 = the context's stream).  `timed`: bracket
 // it with the context's timing events.  `ff`: peer-frame protocol of the frame (api_internal.h).
+// `accum`: a chunk of a progressive frame (fill_params), launched without a claim-order pass: see below.
 int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff,
-              const futhark_opaque_prepared_scene *scene) {
+              const futhark_opaque_prepared_scene *scene, const RayQuery *accum) {
   futhark_context::Lane &L = ctx->lanes[lane_id];
   if (lane_id == 0) L.stream = ctx->stream;
   if (lc.kernel == RAY_B200_KERNEL_WAVEFRONT && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
@@ -353,9 +359,11 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
     if (!have && lc.kernel == RAY_B200_KERNEL_LANEWALK) { set_error(ctx, "render: out of device memory for the finished-sample buffer (%zu bytes)", need); return 1; }
   }
   // heavy-first claim order (warp-queue kernel): worth its probe pass when a frame is long enough to have a tail to lose
-  // — more than one sample per pixel — and pointless when every tile is claimed in the first wave anyway
+  // — more than one sample per pixel — and pointless when every tile is claimed in the first wave anyway.
+  // A chunk of a progressive frame uses neither this nor the learned order below: it is one launch in the plain permuted
+  // order, and it leaves the scene's learned order as it found it (DESIGN.md, progressive rendering).
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = !accum && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -370,7 +378,7 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   bool record_order = false;
   // (Frames of more than 2^24 tile-samples do not end on their longest paths any more, and un-mixing cheap and expensive
   // tiles costs them more than the shorter tail saves.)
-  if (!heavy_first && scene && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
+  if (!heavy_first && !accum && scene && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
       P.local_tiles < (1ll << 26) && (ctx->cfg.learn_order > 1 || P.local_tiles * (int64_t)P.spp <= ((int64_t)1 << 24))) {
     auto &oc = scene->order_cache;
     const bool same = oc.state == 1 && oc.h == P.H && oc.w == P.W && oc.spp == P.spp && oc.rank == P.rank && oc.world == P.world && oc.tiles == P.local_tiles;
@@ -416,7 +424,7 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
   if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches);
   {
-    const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches);
+    const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches, accum);
     if (le == cudaErrorNotSupported) {
       set_error(ctx, "render: kernel %d is not part of this build (libray_b200.so carries mega / warpqueue; the alternatives "
                      "persistent / wavefront / streamqueue / lanewalk are in libray_b200_all.so, built with RAYB200_ALL_KERNELS)", lc.kernel);
@@ -495,6 +503,24 @@ int ray_b200_render_into(struct futhark_context *ctx, int32_t *out_pix_dev, floa
   LaunchConfig lc;
   if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc)) return 1;
   return do_render(ctx, P, lc, 0, true, nullptr, p);
+}
+
+int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, int64_t h, int64_t w, int32_t s_begin,
+                               int32_t s_end, int32_t *out_pix_dev, float *out_rgb_dev,
+                               const struct futhark_opaque_prepared_scene *p) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!ctx->peers.empty()) { set_error(ctx, "render_accumulate: not available on a single-process multi-GPU context (RAY_GPUS > 1)"); return 1; }
+  if (s_begin < 0 || s_end <= s_begin) { set_error(ctx, "render_accumulate: bad sample range [%d, %d)", s_begin, s_end); return 1; }
+  if (!accum_dev) { set_error(ctx, "render_accumulate: accum_dev is required"); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  RayQuery acc{};
+  acc.accum = accum_dev;
+  acc.s_begin = s_begin;
+  RenderParams P;
+  LaunchConfig lc;
+  if (fill_params(ctx, p, h, w, s_end - s_begin, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc, &acc)) return 1;
+  return do_render(ctx, P, lc, 0, true, nullptr, p, &acc);
 }
 
 int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, float *out_rgb_host, int64_t h, int64_t w, int32_t spp,

@@ -177,10 +177,13 @@ __device__ __forceinline__ bool advance_path(const Scene &sc, const RenderParams
 }
 
 // get_ray for sample s of pixel (row j, column i): ray.fut:150-154 with pixel j i -> trace_ray (height-j) i
-// (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).
+// (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).  kAccum (a chunk of a progressive frame):
+// s is relative to the chunk, P.offsets starts at its first sample and is read even when P.spp == 1; at s = 0 of the
+// frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.
+template <bool kAccum = false>
 __device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s) {
   float u, v;
-  if (P.spp == 1) {
+  if (!kAccum && P.spp == 1) {
     u = (float)i / (float)P.W;
     v = (float)(P.H - j) / (float)P.H;
   } else {
@@ -225,11 +228,19 @@ __device__ __forceinline__ int claim_to_item(const RenderParams &P, int c) {
   return (perm << 11) | (c & 2047);
 }
 
+// kAccum: the sum of a progressive frame's samples [0, s_end), always scaled by P.inv_spp = 1/s_end (1 * x = x when
+// s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only)
+template <bool kAccum = false>
 __device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum) {
-  const V3 col = (P.spp == 1) ? sum : vscale(P.inv_spp, sum);
+  const V3 col = (!kAccum && P.spp == 1) ? sum : vscale(P.inv_spp, sum);
   const int pix = pack_pixel(col);
-  if (P.tile_major) P.out_pix[k] = pix;
-  else P.out_pix[(size_t)j * P.W + i] = pix;
+  if constexpr (kAccum) {
+    if (P.out_pix) P.out_pix[(size_t)j * P.W + i] = pix;
+  } else if (P.tile_major) {
+    P.out_pix[k] = pix;
+  } else {
+    P.out_pix[(size_t)j * P.W + i] = pix;
+  }
   if (P.out_rgb) {
     float *q = P.out_rgb + 3 * ((size_t)j * P.W + i);
     q[0] = col.x; q[1] = col.y; q[2] = col.z;

@@ -162,6 +162,16 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // the node batch loads anyway, ray_o.w = t_min and ray_i.w = t_max, and a = dot(d, d), which box tests do not use, moves
 // to ray_d.w (the leaf batch loads ray_d).  Ranged variants exist only as a separate template instantiation, so the
 // per-call variants keep their code.
+//
+// kAccum (pixel mode, progressive rendering, include/ray_b200.h ray_b200_render_accumulate): the launch traces samples
+// [Q.s_begin, Q.s_begin + P.spp) of every pixel.  Everything that counts samples is chunk-relative: P.spp is the chunk
+// length (it sizes cbuf and bounds p_ms's 16-bit sample, as spp does for a whole frame), P.offsets starts at the
+// chunk's first sample and is read for every sample (primary_ray<true>), and sample rel of the chunk is sample
+// s_begin + rel of the frame.  Q.accum holds each pixel's f32 sum of samples [0, s_begin): with s_begin > 0 the in-order
+// sum starts from it (p_sum at the pixel-bound refill, the first term of finalize_pixels), with s_begin == 0 from sample
+// 0's colour itself, as in a whole frame.  Where the pixel is written (scaled by P.inv_spp = 1/s_end,
+// write_pixel<true>), its owner stores the new sum back to Q.accum in place.  So a chain of chunks computes the same f32
+// additions in the same order as one frame of s_end samples.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -172,13 +182,15 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false>
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false,
+          bool kAccum = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   constexpr bool kRays = kQuery != Query::kPixels;  // ray mode
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
+  static_assert(!kAccum || !kRays, "progressive rendering accumulates the samples of pixels");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -239,6 +251,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   int open_seq = 0, disp_seq = 0, disp_s = 0;  // spread dispenser (warp-uniform): pixels opened / next sample to hand out
   float4 *cbuf = nullptr;                      // spread: [kWqRing][spp] finished-sample colours of this warp
   if (kSpread) cbuf = P.sample_buf + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * kWqRing * (size_t)spp;
+  // kAccum: the running sum of pixel (row pj, column pi), row-major as the frame (64-bit offsets: 2^30 pixels pass 4 GiB)
+  [[maybe_unused]] auto accum_of = [&](const int pi, const int pj) { return Q.accum + 3 * ((size_t)pj * P.W + pi); };
 
   // A path in `slot` has ended with `colour`.
   auto finish_path = [&](const int slot, const V3 colour, const int segs) {
@@ -263,18 +277,23 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       const int item = p_item[slot];
       const float4 ps = p_sum[slot];
       int s = __float_as_int(ps.w);
-      const V3 sum = (s == 0) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
+      // (kAccum: s counts the chunk's samples; only sample 0 of the frame starts the sum, later chunks start from accum)
+      const V3 sum = (s == 0 && (!kAccum || Q.s_begin == 0)) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
       s++;
       int pi, pj;
       item_pixel(P, item, pi, pj);
       if (s < spp) {
-        const Ray nr = primary_ray(P, pi, pj, s);
+        const Ray nr = primary_ray<kAccum>(P, pi, pj, s);
         ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
         ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
         p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
         p_sum[slot] = make_float4(sum.x, sum.y, sum.z, __int_as_float(s));
       } else {
-        write_pixel(P, item, pi, pj, sum);
+        write_pixel<kAccum>(P, item, pi, pj, sum);
+        if constexpr (kAccum) {
+          float *a = accum_of(pi, pj);
+          a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
+        }
         p_item[slot] = -1;
       }
     }
@@ -355,16 +374,36 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       float sum = 0.0f;
       if (ready && ch < 3) {
         const float *c = reinterpret_cast<const float *>(cbuf + (size_t)m * spp) + ch;
-        sum = __ldcg(c);
+        if constexpr (kAccum) {
+          // a later chunk adds its samples to the running sum of the earlier ones, the first chunk starts at its sample 0
+          int s = 1, pi, pj;
+          if (Q.s_begin > 0 && item_pixel(P, ring_item[m], pi, pj)) {
+            sum = accum_of(pi, pj)[ch];
+            s = 0;
+          } else {
+            sum = __ldcg(c);
+          }
 #pragma unroll 4
-        for (int s = 1; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+          for (; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+        } else {
+          sum = __ldcg(c);
+#pragma unroll 4
+          for (int s = 1; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+        }
       }
       const float g = __shfl_down_sync(kFullMask, sum, 1), b = __shfl_down_sync(kFullMask, sum, 2);
       if (ready && ch == 0) {
         const int item = ring_item[m];
         int pi, pj;
-        if (item_pixel(P, item, pi, pj)) write_pixel(P, item, pi, pj, v3(sum, g, b));
-        else if (P.tile_major) P.out_pix[item] = 0;
+        if (item_pixel(P, item, pi, pj)) {
+          write_pixel<kAccum>(P, item, pi, pj, v3(sum, g, b));
+          if constexpr (kAccum) {
+            float *a = accum_of(pi, pj);
+            a[0] = sum; a[1] = g; a[2] = b;
+          }
+        } else if (P.tile_major) {
+          P.out_pix[item] = 0;
+        }
       }
       __syncwarp();  // every lane of the entry has read ring_done before it is reset
       if (ready && ch == 0) ring_done[m] = -1;
@@ -427,12 +466,21 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                 p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
               } else if (item < total) {
                 if (item_pixel(P, item, pi, pj)) {
-                  const Ray r = primary_ray(P, pi, pj, 0);
+                  const Ray r = primary_ray<kAccum>(P, pi, pj, 0);
                   p_item[slot] = item;
                   ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                   ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
                   p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
-                  p_sum[slot] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
+                  if constexpr (kAccum) {  // a later chunk's sum starts from the running sum of the earlier ones
+                    float4 ps = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
+                    if (Q.s_begin > 0) {
+                      const float *a = accum_of(pi, pj);
+                      ps.x = a[0]; ps.y = a[1]; ps.z = a[2];
+                    }
+                    p_sum[slot] = ps;
+                  } else {
+                    p_sum[slot] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
+                  }
                 } else if (P.tile_major) {
                   P.out_pix[item] = 0;
                 }
@@ -472,7 +520,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               const int item = ring_item[m];
               int pi, pj;
               if (item_pixel(P, item, pi, pj)) {
-                const Ray r = primary_ray(P, pi, pj, s);
+                const Ray r = primary_ray<kAccum>(P, pi, pj, s);
                 p_item[slot] = item;
                 ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                 ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -875,7 +923,7 @@ __global__ void detile_kernel(const int32_t *__restrict__ gathered, int32_t *__r
 // opt in to > 48 KB of dynamic shared memory on first use (launch_opted_in), not at context creation:
 // futhark_context_new does not touch the ~50 template instantiations it will never launch.
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
-                          int64_t *launches) {
+                          int64_t *launches, const RayQuery *accum) {
   const long long items = p.local_tiles * kTilePixels;
   if (items <= 0) return cudaSuccess;
   if (lc.kernel == 1) {  // RAY_B200_KERNEL_MEGA
@@ -887,7 +935,7 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   }
   if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
   if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  return launch_warpqueue(p, Query::kPixels, false, RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
+  return launch_warpqueue(p, Query::kPixels, false, accum ? *accum : RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
 }
 
 // K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query of kind `kind`: the
@@ -896,6 +944,7 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
                              cudaStream_t stream, int64_t *launches) {
   const bool rays = kind != Query::kPixels;
   const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
+  const bool accum = !rays && q.accum != nullptr;   // a chunk of a progressive frame
   // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
   // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
   const long long work = rays ? (long long)q.n : p.local_tiles * kTilePixels * (spread ? (long long)p.spp : 1ll);
@@ -920,10 +969,10 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
       }, k == 2, all_nodes, sph, ranged);
     }, kind);
   else
-    e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s>>(
+    e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s, auto ac) {
+      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, Query::kPixels, false, ac>>(
           lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
-    }, k == 2, spread, packet, all_nodes, sph);
+    }, k == 2, spread, packet, all_nodes, sph, accum);
   if (e == cudaSuccess) (*launches)++;
   return e;
 }

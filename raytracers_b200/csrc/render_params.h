@@ -79,6 +79,11 @@ struct RayQuery {
   uint8_t *occluded;        // occlusion query: [n] 0 / 1
   int32_t k;                // multi-hit query: records per ray, in [1, 64]
   int32_t *counts;          // multi-hit query, optional: [n] accepted leaves per ray, not capped at k
+  // progressive rendering (pixel mode, kernel template parameter kAccum; include/ray_b200.h ray_b200_render_accumulate):
+  // the frame's samples [s_begin, s_begin + P.spp) are added to accum, row-major [H][W][3], the running f32 sum of each
+  // pixel's samples [0, s_begin) (not read when s_begin == 0)
+  float *accum;
+  int32_t s_begin;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
@@ -120,11 +125,13 @@ struct LaunchConfig {
   int max_dynamic_smem;  // the device's opt-in shared-memory limit (kernels opt in on first launch)
 };
 
-// A frame on the kernel lc.kernel names (render_kernels.cu)
+// A frame on the kernel lc.kernel names (render_kernels.cu); `accum` (NULL = a whole frame): a progressive-rendering call's
+// running sums (RayQuery::accum, s_begin), on the warp-queue kernel only
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
-                          int64_t *launches);
-// The warp-queue kernel (render_kernels.cu): a pixel frame (kind = Query::kPixels, q unused), or a ray query of that kind
-// (whatever lc.kernel says); `ranged`: q.rays is [n][8] with an interval per ray (hit, occlusion and multi-hit queries)
+                          int64_t *launches, const RayQuery *accum = nullptr);
+// The warp-queue kernel (render_kernels.cu): a pixel frame (kind = Query::kPixels; q unused unless q.accum is set, which
+// picks the accumulating variants), or a ray query of that kind (whatever lc.kernel says); `ranged`: q.rays is [n][8]
+// with an interval per ray (hit, occlusion and multi-hit queries)
 cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
                              cudaStream_t stream, int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
