@@ -149,6 +149,32 @@ int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, flo
 int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, int64_t h, int64_t w,
                                int32_t s_begin, int32_t s_end, int32_t *out_pix_dev, float *out_rgb_dev,
                                const struct futhark_opaque_prepared_scene *p);
+/* Several views of one prepared scene in one launch, each with its own camera, sharing the scene's BVH: a camera
+ * fly-through over a static scene, a stereo pair, the six faces of a cube map, a batch of poses, or (n_views = 1) the
+ * prepared scene seen from another camera without preparing it again.
+ * cams7_host: host float[n_views][7] = look_from.xyz, look_at.xyz, fov of each view (the cam7 layout of
+ * ray_b200_scene_from_arrays).  out_pix_dev: device int32[n_views][h][w] (required); out_rgb_dev: device
+ * float[n_views][h][w][3] or NULL.
+ *   Exactness: view v's pixels and float framebuffer are bit for bit what ray_b200_render_into(h, w, spp) writes for
+ *   prepare_scene(h, w, S_v), where S_v is the prepared scene's spheres with cams7[v] as its camera.  That camera is
+ *   make_camera of cams7[v] with the aspect ratio f32(w) / f32(h) of this call (ray.fut:243-244), computed on the host
+ *   as prepare_scene computes it (ray_b200_host_camera gives the same 12 floats).  The spp semantics and the
+ *   quantisation rule above hold unchanged.  A NaN camera (a view looking along vup or at its own position) quantises by
+ *   that rule and does not affect the other views; a NaN of the float framebuffer is some NaN.
+ *   The call is asynchronous on the context's stream and is one kernel launch (plus the heavy-first probe when enabled
+ *   and spp > 1, as for ray_b200_render_into).  cams7_host may be reused once the call returns: the library copies the
+ *   camera table to stream-ordered device memory and frees it behind the launch.  ray_b200_context_last_render_ms,
+ *   ray_b200_context_launch_count, the pipeline lanes, and freeing or re-uploading the prepared scene while the call is
+ *   in flight behave as for ray_b200_render_into.
+ *   It runs on the warp-queue kernel whatever RAY_KERNEL or the context's kernel says, and leaves the prepared scene's
+ *   learned claim order untouched: renders before and after it plan and launch exactly as without it.
+ *   Errors (nonzero return, futhark_context_get_error; the context stays usable): every error of ray_b200_render_into
+ *   (image size, spp, an invalid prepared scene, a RAY_GPUS > 1 context), n_views < 1, cams7_host == NULL,
+ *   out_pix_dev == NULL, n_views x tiles(h, w) > 2^25 (at most 2^30 padded pixels over all views, where a tile is 8 x 4
+ *   pixels), and a shard set (world > 1). */
+int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                               const float *cams7_host, int32_t n_views, int64_t h, int64_t w, int32_t spp,
+                               int32_t *out_pix_dev, float *out_rgb_dev);
 /* Like futhark_entry_render but with explicit spp (library-owned result). */
 int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d **out0, int64_t h, int64_t w,
                               int32_t spp, const struct futhark_opaque_prepared_scene *p);

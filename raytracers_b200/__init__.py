@@ -21,7 +21,7 @@ import os
 import numpy as np
 
 __all__ = ["Context", "RayError", "Hit", "Ray", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
-           "host_camera", "host_lbvh", "host_sample_offsets", "camera_rays"]
+           "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 KERNELS = {"auto": 0, "mega": 1, "persistent": 2, "wavefront": 3, "warpqueue": 4, "streamqueue": 5, "lanewalk": 6}
@@ -150,6 +150,7 @@ def load_library(variant=""):
         "ray_b200_render_into": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_host": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_accumulate": (C.c_int, [vp, vp, i64, i64, i32, i32, vp, vp, vp]),
+        "ray_b200_render_views_into": (C.c_int, [vp, vp, vp, i32, i64, i64, i32, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
         "ray_b200_shard_tiles_padded": (i64, [i64, i64, i32]),
@@ -256,6 +257,22 @@ def host_sample_offsets(spp):
     t = np.empty((spp, 2), np.float32)
     load_library().ray_b200_host_sample_offsets(int(spp), _ptr(t))
     return t
+
+
+def camera_table(cams):
+    """The cameras of Context.render_views as the library reads them: a contiguous float32 [V, 7] array (look_from.xyz,
+    look_at.xyz, fov of each view) from any host array-like of shape [V, 7] with a floating-point dtype.  A CUDA tensor
+    raises ValueError (reading it would synchronise the device), and so does any other shape or dtype."""
+    if type(cams).__module__.startswith("torch"):
+        if cams.device.type != "cpu":
+            raise ValueError(f"cams must be a host array of shape [V, 7], got a tensor on {cams.device}")
+        cams = cams.numpy()
+    a = np.asarray(cams)
+    if a.ndim != 2 or a.shape[1] != 7:
+        raise ValueError(f"cams must have shape [V, 7], got {a.shape}")
+    if a.dtype.kind != "f":
+        raise ValueError(f"cams must be floating-point, got {a.dtype}")
+    return np.ascontiguousarray(a, np.float32)
 
 
 def camera_rays(camera, h, w, spp=1):
@@ -573,6 +590,30 @@ class Context:
         torch.cuda.current_stream(accum.device).synchronize()
         self.render_accumulate_into(accum.data_ptr(), h, w, prepared, s_begin, s_end, pix.data_ptr(),
                                     rgb.data_ptr() if rgb is not None else None)
+        self.sync()
+        return (pix, rgb) if want_rgb else pix
+
+    def render_views_into(self, prepared, cams, h, w, spp, out_pix_dev, out_rgb_dev=None):
+        """Several views of one prepared scene in one launch (ray_b200_render_views_into): cams = host [V, 7] cameras
+        (look_from.xyz, look_at.xyz, fov; see camera_table), out_pix_dev = device int32[V][h][w], out_rgb_dev = device
+        float[V][h][w][3] or None.  View v equals render_into of a scene prepared at (h, w) with camera cams[v], bit for
+        bit.  Asynchronous on the context's stream; cams may be reused once the call returns."""
+        c = camera_table(cams)
+        self._check(self.lib.ray_b200_render_views_into(self.handle, prepared.handle, _ptr(c), c.shape[0], int(h), int(w),
+                                                        int(spp), _ptr(out_pix_dev), _ptr(out_rgb_dev)))
+
+    def render_views(self, prepared, cams, h, w, spp=1, want_rgb=False):
+        """Renders V views of one prepared scene (cams: host [V, 7], see camera_table) and returns CUDA int32 [V, h, w]
+        pixels, and with want_rgb also the float32 [V, h, w, 3] framebuffers, as (pixels, rgb).  Waits for torch's current
+        stream before, and synchronises the context after the call."""
+        import torch
+        c = camera_table(cams)
+        dev = torch.device("cuda", self.device)
+        pix = torch.empty((c.shape[0], int(h), int(w)), dtype=torch.int32, device=dev)
+        rgb = torch.empty((c.shape[0], int(h), int(w), 3), dtype=torch.float32, device=dev) if want_rgb else None
+        # the outputs' memory may still be in use on torch's stream, which the context's own stream is not ordered after
+        torch.cuda.current_stream(dev).synchronize()
+        self.render_views_into(prepared, c, h, w, spp, pix.data_ptr(), rgb.data_ptr() if rgb is not None else None)
         self.sync()
         return (pix, rgb) if want_rgb else pix
 

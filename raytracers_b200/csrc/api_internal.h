@@ -168,10 +168,12 @@ inline int64_t tiles_of_rank(int64_t h, int64_t w, int32_t rank, int32_t world) 
 int resolve_kernel(const futhark_context *ctx);
 // The parameter block of one frame and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
 // slots, ...), which the caller hands to do_render.  `accum` (progressive rendering, ray_b200_render_accumulate): the
-// frame's samples [accum->s_begin, accum->s_begin + spp) on the warp-queue kernel, scaled by 1/(s_begin + spp).
+// frame's samples [accum->s_begin, accum->s_begin + spp) on the warp-queue kernel, scaled by 1/(s_begin + spp).  `views`
+// (ray_b200_render_views_into; rank 0 of 1): views->n_views frames of h x w, planned as one frame of all their tiles, on
+// the warp-queue kernel; views->view_tiles is set here.
 int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
                 int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc,
-                const RayQuery *accum = nullptr);
+                const RayQuery *accum = nullptr, RayQuery *views = nullptr);
 void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P);  // zeroes P, then its scene half
 // The warp-queue kernel's plan for one launch (pixel frames and ray queries): rays in flight per warp (32 k), warps per
 // CTA, node-queue cap and packet threshold in lc, how much of the scene is staged in shared memory in P.
@@ -189,7 +191,7 @@ struct FrameFlags {
 };
 int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id = 0, bool timed = true,
               const FrameFlags *ff = nullptr, const futhark_opaque_prepared_scene *scene = nullptr,
-              const RayQuery *accum = nullptr);
+              const RayQuery *accum = nullptr, const RayQuery *views = nullptr);
 // api_multigpu.cu: the single-process multi-GPU mode (RAY_GPUS > 1) of futhark_entry_render
 int create_helper_contexts(futhark_context *ctx, const futhark_context_config *cfg, int ndev);
 int render_multi_device(futhark_context *ctx, futhark_i32_2d *img, int64_t h, int64_t w, int32_t spp, const futhark_opaque_prepared_scene *p);

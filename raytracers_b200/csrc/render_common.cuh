@@ -176,12 +176,23 @@ __device__ __forceinline__ bool advance_path(const Scene &sc, const RenderParams
   return shade_segment(sc, P, r, q.a, j, tb, light, depth, colour);
 }
 
+// get_ray (ray.fut:109-114) of camera c (origin, llc, horizontal, vertical) at (u, v)
+__device__ __forceinline__ Ray camera_ray(const float *c, const float u, const float v) {
+  Ray r;
+  r.o = v3(c[0], c[1], c[2]);
+  // llc + s*horizontal + t*vertical - origin (ray.fut:111-113), per component, left to right
+  r.d = v3(((c[3] + u * c[6]) + v * c[9]) - c[0], ((c[4] + u * c[7]) + v * c[10]) - c[1],
+           ((c[5] + u * c[8]) + v * c[11]) - c[2]);
+  return r;
+}
+
 // get_ray for sample s of pixel (row j, column i): ray.fut:150-154 with pixel j i -> trace_ray (height-j) i
 // (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).  kAccum (a chunk of a progressive frame):
 // s is relative to the chunk, P.offsets starts at its first sample and is read even when P.spp == 1; at s = 0 of the
-// frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.
-template <bool kAccum = false>
-__device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s) {
+// frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  kViews (a views launch): the
+// camera is view_cam, the pixel's view's 12 floats of RayQuery::cams, instead of P.cam.
+template <bool kAccum = false, bool kViews = false>
+__device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s, const float *view_cam = nullptr) {
   float u, v;
   if (!kAccum && P.spp == 1) {
     u = (float)i / (float)P.W;
@@ -190,13 +201,13 @@ __device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, 
     u = ((float)i + P.offsets[2 * s]) / (float)P.W;
     v = ((float)(P.H - j) + P.offsets[2 * s + 1]) / (float)P.H;
   }
-  const float *c = P.cam;
-  Ray r;
-  r.o = v3(c[0], c[1], c[2]);
-  // llc + s*horizontal + t*vertical - origin (ray.fut:111-113), per component, left to right
-  r.d = v3(((c[3] + u * c[6]) + v * c[9]) - c[0], ((c[4] + u * c[7]) + v * c[10]) - c[1],
-           ((c[5] + u * c[8]) + v * c[11]) - c[2]);
-  return r;
+  if constexpr (kViews) {  // three 16-byte read-only loads (the table is 16-byte aligned, 48 bytes per view)
+    const float4 *q = reinterpret_cast<const float4 *>(view_cam);
+    const float4 a = __ldg(q), b = __ldg(q + 1), d = __ldg(q + 2);
+    const float c[12] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, d.x, d.y, d.z, d.w};
+    return camera_ray(c, u, v);
+  }
+  return camera_ray(P.cam, u, v);
 }
 
 // item k -> pixel.  Local tile lt = k >> 5 is global tile lt*world + rank; lane position k & 31 inside the 8x4 tile.
@@ -206,6 +217,20 @@ __device__ __forceinline__ bool item_pixel(const RenderParams &P, int k, int &i,
   const unsigned t = (unsigned)(k >> 5) * (unsigned)P.world + (unsigned)P.rank;
   const int sub = k & 31;
   const unsigned ty = t / (unsigned)P.tiles_x, tx = t - ty * (unsigned)P.tiles_x;
+  i = (int)tx * kTileW + (sub & (kTileW - 1));
+  j = (int)ty * kTileH + (sub >> 3);
+  return (long long)t < P.n_tiles && i < P.W && j < P.H;
+}
+
+// kViews: item k -> view v and pixel.  The views' tiles follow each other, view_tiles = tiles_x * tiles_y per view in the
+// row-major tile order of one frame (a views launch has no shards).  Tile t is in tile row r = t / tiles_x over all
+// views, which is row r - v * tiles_y of view v = r / tiles_y: two 32-bit divisions (n_tiles <= 2^25).
+__device__ __forceinline__ bool item_view_pixel(const RenderParams &P, int k, int &v, int &i, int &j) {
+  const unsigned t = (unsigned)(k >> 5);
+  const int sub = k & 31;
+  const unsigned r = t / (unsigned)P.tiles_x, tx = t - r * (unsigned)P.tiles_x;
+  const unsigned vv = r / (unsigned)P.tiles_y, ty = r - vv * (unsigned)P.tiles_y;
+  v = (int)vv;
   i = (int)tx * kTileW + (sub & (kTileW - 1));
   j = (int)ty * kTileH + (sub >> 3);
   return (long long)t < P.n_tiles && i < P.W && j < P.H;
@@ -229,11 +254,21 @@ __device__ __forceinline__ int claim_to_item(const RenderParams &P, int c) {
 }
 
 // kAccum: the sum of a progressive frame's samples [0, s_end), always scaled by P.inv_spp = 1/s_end (1 * x = x when
-// s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only)
-template <bool kAccum = false>
-__device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum) {
+// s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only).  kViews: pixel (i, j) of view
+// `view`, whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the float frames 12 GiB)
+template <bool kAccum = false, bool kViews = false>
+__device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum, int view = 0) {
   const V3 col = (!kAccum && P.spp == 1) ? sum : vscale(P.inv_spp, sum);
   const int pix = pack_pixel(col);
+  if constexpr (kViews) {
+    const size_t px = (size_t)view * (size_t)P.H * (size_t)P.W + (size_t)j * P.W + i;
+    P.out_pix[px] = pix;
+    if (P.out_rgb) {
+      float *q = P.out_rgb + 3 * px;
+      q[0] = col.x; q[1] = col.y; q[2] = col.z;
+    }
+    return;
+  }
   if constexpr (kAccum) {
     if (P.out_pix) P.out_pix[(size_t)j * P.W + i] = pix;
   } else if (P.tile_major) {

@@ -75,6 +75,39 @@ __global__ void __launch_bounds__(256) tile_probe_kernel(const __grid_constant__
   }
 }
 
+// The probe of a views launch (ray_b200_render_views_into): tile_probe_kernel with each tile traced by its view's camera,
+// the 12 floats of `cams` (RayQuery::cams) at its view.
+__global__ void __launch_bounds__(256) tile_probe_views_kernel(const __grid_constant__ RenderParams P, uint32_t *__restrict__ keys,
+                                                               int32_t *__restrict__ ids, const float *__restrict__ cams) {
+  const int probes = P.probes_per_tile;
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long lt = t / probes;
+  const int q = (int)(t - lt * probes);
+  bool alive = false;
+  if (lt < P.local_tiles) {
+    const int sub = q == 0 ? 11 : (q == 1 ? 22 : (q == 2 ? 17 : 5));
+    int v, i, j;
+    if (item_view_pixel(P, (int)(lt << 5) | sub, v, i, j)) {
+      const GlobalScene sc{P.nodes, P.geom};
+      Ray r = primary_ray<false, true>(P, i, j, 0, cams + 12 * (size_t)v);
+      V3 light = v3(1.0f, 1.0f, 1.0f), colour;
+      int depth = 0, segments = 0;
+      WorkCounters wc;
+      do {
+        alive = advance_path<false>(sc, P, r, light, depth, colour, wc);
+      } while (alive && ++segments < P.probe_segments);
+    }
+  }
+  if (probes > 1) alive |= __shfl_xor_sync(kFullMask, alive, 1);
+  if (probes > 2) alive |= __shfl_xor_sync(kFullMask, alive, 2);
+  if (q == 0 && lt < P.local_tiles) {
+    const long long chunk = lt >> 6;
+    const uint32_t pos = (uint32_t)((chunk * P.chunk_stride_inv) % P.n_chunks) << 6 | (uint32_t)(lt & 63);
+    keys[lt] = alive ? pos >> 1 : pos;
+    ids[lt] = (int32_t)lt;
+  }
+}
+
 // Learned claim order: the probe replaced by what the previous frame of the same scene measured (the longest path of every
 // tile, recorded by finish_path).  Tiles with a long path keep their place in the permuted sequence but move in front of
 // all others, so the 50-bounce paths that end a frame are claimed in its first few percent.
@@ -172,6 +205,14 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // 0's colour itself, as in a whole frame.  Where the pixel is written (scaled by P.inv_spp = 1/s_end,
 // write_pixel<true>), its owner stores the new sum back to Q.accum in place.  So a chain of chunks computes the same f32
 // additions in the same order as one frame of s_end samples.
+//
+// kViews (pixel mode, include/ray_b200.h ray_b200_render_views_into): the launch renders Q.n_views frames of one size
+// from one prepared scene.  The work items are the tiles of all views, view after view (P.n_tiles = P.local_tiles =
+// n_views * Q.view_tiles), so the chunk permutation of the claim order mixes the views' sky and ground tiles as it mixes
+// one frame's.  Where a pixel item becomes a pixel (pixel_of: the pixel-bound refill, finish_path's next sample and store,
+// the spread dispenser and finalize_pixels) it also gives its view v; the camera ray reads view v's 12 floats of Q.cams
+// instead of P.cam, and the pixel is stored at offset v * H * W.  Nothing else depends on the view, so every view's
+// pixel sees exactly the arithmetic of a one-view frame whose P.cam is that camera.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -183,7 +224,7 @@ constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
 
 template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false,
-          bool kAccum = false>
+          bool kAccum = false, bool kViews = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
@@ -191,6 +232,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
   static_assert(!kAccum || !kRays, "progressive rendering accumulates the samples of pixels");
+  static_assert(!kViews || (!kRays && !kAccum), "views are whole pixel frames");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -253,6 +295,14 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   if (kSpread) cbuf = P.sample_buf + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * kWqRing * (size_t)spp;
   // kAccum: the running sum of pixel (row pj, column pi), row-major as the frame (64-bit offsets: 2^30 pixels pass 4 GiB)
   [[maybe_unused]] auto accum_of = [&](const int pi, const int pj) { return Q.accum + 3 * ((size_t)pj * P.W + pi); };
+  // pixel item -> (view, column, row), false for a padding pixel; the view is 0 unless kViews
+  auto pixel_of = [&](const int item, int &pv, int &pi, int &pj) {
+    if constexpr (kViews) return item_view_pixel(P, item, pv, pi, pj);
+    pv = 0;
+    return item_pixel(P, item, pi, pj);
+  };
+  // kViews: the camera of view pv (its 12 floats of Q.cams)
+  [[maybe_unused]] auto view_cam = [&](const int pv) -> const float * { return kViews ? Q.cams + 12 * (size_t)pv : nullptr; };
 
   // A path in `slot` has ended with `colour`.
   auto finish_path = [&](const int slot, const V3 colour, const int segs) {
@@ -280,16 +330,16 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       // (kAccum: s counts the chunk's samples; only sample 0 of the frame starts the sum, later chunks start from accum)
       const V3 sum = (s == 0 && (!kAccum || Q.s_begin == 0)) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
       s++;
-      int pi, pj;
-      item_pixel(P, item, pi, pj);
+      int pi, pj, pv;
+      pixel_of(item, pv, pi, pj);
       if (s < spp) {
-        const Ray nr = primary_ray<kAccum>(P, pi, pj, s);
+        const Ray nr = primary_ray<kAccum, kViews>(P, pi, pj, s, view_cam(pv));
         ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
         ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
         p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
         p_sum[slot] = make_float4(sum.x, sum.y, sum.z, __int_as_float(s));
       } else {
-        write_pixel<kAccum>(P, item, pi, pj, sum);
+        write_pixel<kAccum, kViews>(P, item, pi, pj, sum, pv);
         if constexpr (kAccum) {
           float *a = accum_of(pi, pj);
           a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
@@ -394,9 +444,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       const float g = __shfl_down_sync(kFullMask, sum, 1), b = __shfl_down_sync(kFullMask, sum, 2);
       if (ready && ch == 0) {
         const int item = ring_item[m];
-        int pi, pj;
-        if (item_pixel(P, item, pi, pj)) {
-          write_pixel<kAccum>(P, item, pi, pj, v3(sum, g, b));
+        int pi, pj, pv;
+        if (pixel_of(item, pv, pi, pj)) {
+          write_pixel<kAccum, kViews>(P, item, pi, pj, v3(sum, g, b), pv);
           if constexpr (kAccum) {
             float *a = accum_of(pi, pj);
             a[0] = sum; a[1] = g; a[2] = b;
@@ -441,7 +491,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             if (p_item[slot] < 0) {
               const int c = base + rank++;
               const int item = c < total_claims ? (kRays ? c : claim_to_item(P, c)) : total;
-              int pi, pj;
+              int pi, pj, pv;
               if (kRanged && item < total) {
                 // struct ray_b200_ray (64-bit offset: n reaches 2^30); a 16-byte aligned buffer takes two 16-byte loads
                 const float *rp = Q.rays + 8 * (size_t)item;
@@ -465,8 +515,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                 ray_d[slot] = make_float4(rp[3], rp[4], rp[5], 0.0f);
                 p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
               } else if (item < total) {
-                if (item_pixel(P, item, pi, pj)) {
-                  const Ray r = primary_ray<kAccum>(P, pi, pj, 0);
+                if (pixel_of(item, pv, pi, pj)) {
+                  const Ray r = primary_ray<kAccum, kViews>(P, pi, pj, 0, view_cam(pv));
                   p_item[slot] = item;
                   ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                   ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -518,9 +568,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               while (s >= spp) { s -= spp; seq++; }
               const int m = seq & (kWqRing - 1);
               const int item = ring_item[m];
-              int pi, pj;
-              if (item_pixel(P, item, pi, pj)) {
-                const Ray r = primary_ray<kAccum>(P, pi, pj, s);
+              int pi, pj, pv;
+              if (pixel_of(item, pv, pi, pj)) {
+                const Ray r = primary_ray<kAccum, kViews>(P, pi, pj, s, view_cam(pv));
                 p_item[slot] = item;
                 ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                 ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -923,7 +973,7 @@ __global__ void detile_kernel(const int32_t *__restrict__ gathered, int32_t *__r
 // opt in to > 48 KB of dynamic shared memory on first use (launch_opted_in), not at context creation:
 // futhark_context_new does not touch the ~50 template instantiations it will never launch.
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
-                          int64_t *launches, const RayQuery *accum) {
+                          int64_t *launches, const RayQuery *pixq) {
   const long long items = p.local_tiles * kTilePixels;
   if (items <= 0) return cudaSuccess;
   if (lc.kernel == 1) {  // RAY_B200_KERNEL_MEGA
@@ -935,7 +985,7 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   }
   if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
   if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  return launch_warpqueue(p, Query::kPixels, false, accum ? *accum : RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
+  return launch_warpqueue(p, Query::kPixels, false, pixq ? *pixq : RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
 }
 
 // K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query of kind `kind`: the
@@ -945,6 +995,7 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
   const bool rays = kind != Query::kPixels;
   const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
   const bool accum = !rays && q.accum != nullptr;   // a chunk of a progressive frame
+  const bool views = !rays && q.cams != nullptr;    // several views of the scene
   // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
   // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
   const long long work = rays ? (long long)q.n : p.local_tiles * kTilePixels * (spread ? (long long)p.spp : 1ll);
@@ -968,6 +1019,11 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
             lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
       }, k == 2, all_nodes, sph, ranged);
     }, kind);
+  else if (views)
+    e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
+      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, Query::kPixels, false, false, true>>(
+          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
+    }, k == 2, spread, packet, all_nodes, sph);
   else
     e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s, auto ac) {
       return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, Query::kPixels, false, ac>>(
@@ -1001,9 +1057,11 @@ size_t tile_order_sort_bytes(int64_t local_tiles) {
   return bytes;
 }
 
-void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches) {
+void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches,
+                       const RayQuery *views) {
   const long long threads = (long long)p.local_tiles * p.probes_per_tile;
-  tile_probe_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(p, b.keys, b.ids);
+  if (views) tile_probe_views_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(p, b.keys, b.ids, views->cams);
+  else tile_probe_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(p, b.keys, b.ids);
   size_t bytes = b.sort_tmp_bytes;
   cub::DeviceRadixSort::SortPairs(b.sort_tmp, bytes, b.keys, b.keys_sorted, b.ids, b.order, (int)p.local_tiles, 0,
                                   tile_order_key_bits(p.n_chunks), stream);

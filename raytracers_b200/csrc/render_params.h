@@ -84,6 +84,13 @@ struct RayQuery {
   // pixel's samples [0, s_begin) (not read when s_begin == 0)
   float *accum;
   int32_t s_begin;
+  // several views of one prepared scene (pixel mode, kernel template parameter kViews; include/ray_b200.h
+  // ray_b200_render_views_into): n_views frames of P.W x P.H, one after the other.  Work-item tiles
+  // [v * view_tiles, (v + 1) * view_tiles) are view v's tiles in the row-major tile order of one frame; view v is drawn
+  // with the camera cams[v] (device [n_views][12], 16-byte aligned, laid out as RenderParams::cam) and written at pixel
+  // offset v * H * W of the outputs
+  const float *cams;
+  int32_t n_views, view_tiles;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
@@ -125,13 +132,14 @@ struct LaunchConfig {
   int max_dynamic_smem;  // the device's opt-in shared-memory limit (kernels opt in on first launch)
 };
 
-// A frame on the kernel lc.kernel names (render_kernels.cu); `accum` (NULL = a whole frame): a progressive-rendering call's
-// running sums (RayQuery::accum, s_begin), on the warp-queue kernel only
+// A frame on the kernel lc.kernel names (render_kernels.cu); `pixq` (NULL = a whole frame of one view): a progressive-
+// rendering call's running sums (RayQuery::accum, s_begin) or a views call's camera table (RayQuery::cams, n_views,
+// view_tiles), on the warp-queue kernel only
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
-                          int64_t *launches, const RayQuery *accum = nullptr);
+                          int64_t *launches, const RayQuery *pixq = nullptr);
 // The warp-queue kernel (render_kernels.cu): a pixel frame (kind = Query::kPixels; q unused unless q.accum is set, which
-// picks the accumulating variants), or a ray query of that kind (whatever lc.kernel says); `ranged`: q.rays is [n][8]
-// with an interval per ray (hit, occlusion and multi-hit queries)
+// picks the accumulating variants, or q.cams, which picks the views variants), or a ray query of that kind (whatever
+// lc.kernel says); `ranged`: q.rays is [n][8] with an interval per ray (hit, occlusion and multi-hit queries)
 cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
                              cudaStream_t stream, int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
@@ -153,7 +161,9 @@ inline int tile_order_key_bits(int32_t n_chunks) {  // keys are positions < n_ch
   while (bits < 32 && (1ll << bits) < (long long)n_chunks * 64) bits++;
   return bits;
 }
-void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches);
+// `views` (NULL = one view): the probe traces each tile with its view's camera (RayQuery::cams)
+void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches,
+                       const RayQuery *views = nullptr);
 // The same order table from a recorded frame: tiles whose longest path had >= long_path segments first, both groups in
 // the permuted claim sequence (cost = RenderParams::tile_cost of the recorded frame)
 void launch_tile_order_from_cost(const RenderParams &p, const uint32_t *cost, int32_t long_path, const TileOrderBuffers &b,

@@ -5,10 +5,10 @@
 
 cuobjdump -sass of both files, split into functions, names demangled.  A function of OLD must exist in NEW with the
 same instructions and encodings.  The warp-queue kernel's instantiations are matched by one canonical key, (K, spread,
-packet, all-nodes, spheres, query kind, ranged, accum), parsed from every form its template has had: five parameters
-(pixel frames only), six (kRays), seven (kAnyHit), eight (kMultiHit), the query-kind enum (Query), the enum followed by
-kRanged (per-ray intervals) and the enum followed by kRanged and kAccum (progressive rendering); a parameter a form does
-not have is false.  So OLD and NEW may be builds of any of them.  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
+packet, all-nodes, spheres, query kind, ranged, accum, views), parsed from every form its template has had: five
+parameters (pixel frames only), six (kRays), seven (kAnyHit), eight (kMultiHit), the query-kind enum (Query), the enum
+followed by kRanged (per-ray intervals), by kRanged and kAccum (progressive rendering) and by kRanged, kAccum and kViews
+(several views in one launch); a parameter a form does not have is false.  So OLD and NEW may be builds of any of them.  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
 """
 import collections
 import re
@@ -54,16 +54,17 @@ def canonical(name):
     args = [a.strip() for a in m.group(1).split(",")]
     k, (spread, packet, all_nodes, spheres), rest = args[0], args[1:5], args[5:]
     enum = re.fullmatch(r"\(.*Query\)(\d+)", rest[0]) if rest else None
-    ranged = accum = False
-    if enum:   # <K, kSpread, kPacket, kAllNodes, kSpheres, (Query)N[, kRanged[, kAccum]]>
+    ranged = accum = views = False
+    if enum:   # <K, kSpread, kPacket, kAllNodes, kSpheres, (Query)N[, kRanged[, kAccum[, kViews]]]>
         kind = KINDS[int(enum.group(1))]
         ranged = len(rest) > 1 and rest[1] == "true"
         accum = len(rest) > 2 and rest[2] == "true"
+        views = len(rest) > 3 and rest[3] == "true"
     else:      # <K, kSpread, kPacket, kAllNodes, kSpheres[, kRays[, kAnyHit[, kMultiHit]]]>, false when absent
         rays, any_hit, multi_hit = [a == "true" for a in rest] + [False] * (3 - len(rest))
         kind = KINDS[0 if not rays else 2 if any_hit else 3 if multi_hit else 1]
     return (f"render_warpqueue_kernel[K={k}, spread={spread}, packet={packet}, all_nodes={all_nodes}, spheres={spheres}, "
-            f"query={kind}{', ranged' if ranged else ''}{', accum' if accum else ''}]")
+            f"query={kind}{', ranged' if ranged else ''}{', accum' if accum else ''}{', views' if views else ''}]")
 
 
 def main():
