@@ -69,30 +69,31 @@ static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
   return lc;
 }
 
-// Fills the kernel parameter block for one frame, and the frame's launch plan.  With `accum` the launch is one chunk of
-// a progressive frame: spp samples from accum->s_begin on, planned as a frame of spp samples (spread or pixel-bound by
-// the chunk length), read from the offset table of the whole frame at the chunk's first sample and scaled by
-// 1/s_end; it runs on the warp-queue kernel whatever the context's kernel is.  With `views` the launch renders
-// views->n_views frames of h x w: its work items are the tiles of all of them, so the plan (spread or pixel-bound, K,
+// Fills the kernel parameter block for one frame, and the frame's launch plan.  Query::kAccumulate: the launch is one
+// chunk of a progressive frame: spp samples from q->s_begin on, planned as a frame of spp samples (spread or pixel-bound
+// by the chunk length), read from the offset table of the whole frame at the chunk's first sample and scaled by
+// 1/s_end; it runs on the warp-queue kernel whatever the context's kernel is.  Query::kViews: the launch renders
+// q->n_views frames of h x w: its work items are the tiles of all of them, so the plan (spread or pixel-bound, K,
 // staging, the sample buffer) is that of one frame of n_views x tiles(h, w) tiles; it runs on the warp-queue kernel too.
 int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
                 int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc,
-                const RayQuery *accum, RayQuery *views) {
+                Query kind, RayQuery *q) {
+  const bool views = kind == Query::kViews;
   if (!p || !p->dev.nodes) { set_error(ctx, "render: invalid prepared scene"); return 1; }
   if (h <= 0 || w <= 0 || h > 65536 || w > 65536 || ((h + 3) / 4) * ((w + 7) / 8) > ((int64_t)1 << 25)) {
     // work items are 32-bit: at most 2^30 (padded) pixels per frame
     set_error(ctx, "render: bad image size %lldx%lld", (long long)h, (long long)w);
     return 1;
   }
-  if (views && tiles_total(h, w) * views->n_views > ((int64_t)1 << 25)) {
+  if (views && tiles_total(h, w) * q->n_views > ((int64_t)1 << 25)) {
     // ... and per launch: at most 2^30 padded pixels over all views
-    set_error(ctx, "render_views: %d views of %lldx%lld exceed 2^30 padded pixels", views->n_views, (long long)h, (long long)w);
+    set_error(ctx, "render_views: %d views of %lldx%lld exceed 2^30 padded pixels", q->n_views, (long long)h, (long long)w);
     return 1;
   }
   if (spp < 1) { set_error(ctx, "render: spp must be >= 1"); return 1; }
   if (world < 1 || rank < 0 || rank >= world) { set_error(ctx, "render: bad shard %d/%d", rank, world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
-  const int32_t s_begin = accum ? accum->s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
+  const int32_t s_begin = kind == Query::kAccumulate ? q->s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
   if (ensure_offsets(ctx, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
@@ -106,8 +107,8 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   P.n_tiles = tiles_total(h, w);
   P.local_tiles = tiles_of_rank(h, w, rank, world);
   if (views) {  // (the entry point allows no shards)
-    views->view_tiles = (int32_t)P.n_tiles;
-    P.n_tiles = P.local_tiles = P.n_tiles * views->n_views;
+    q->view_tiles = (int32_t)P.n_tiles;
+    P.n_tiles = P.local_tiles = P.n_tiles * q->n_views;
   }
   P.n_chunks = (int32_t)((P.local_tiles + 63) / 64);
   {  // stride ~ golden ratio * n_chunks, made coprime to n_chunks
@@ -133,7 +134,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   // shared-memory staging plan: BFS prefix of the node array, then the sphere records if they all fit.
   // The warp-queue kernel runs one CTA per SM and gives the staging area whatever its queues leave.
   int64_t budget = std::min<int64_t>(ctx->cfg.smem_budget, ctx->max_smem_optin - 1024) - 128;
-  int kern = (accum || views) ? RAY_B200_KERNEL_WARPQUEUE : resolve_kernel(ctx);
+  int kern = kind != Query::kPixels ? RAY_B200_KERNEL_WARPQUEUE : resolve_kernel(ctx);
   if (kern == RAY_B200_KERNEL_LANEWALK && spp > 1) {
     // K5 traces one sample per slot and needs the finished-sample buffer (0.54 MB per sample on an H100); without it (spreading
     // switched off, or a sample count whose buffer exceeds the budget) the frame runs on the warp-queue kernel
@@ -347,10 +348,10 @@ static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64
 
 // Enqueues one frame with launch plan `lc` (fill_params) on lane `lane_id` (0 = the context's stream).  `timed`: bracket
 // it with the context's timing events.  `ff`: peer-frame protocol of the frame (api_internal.h).
-// `accum`: a chunk of a progressive frame (fill_params), launched without a claim-order pass: see below.  `views`: the
-// camera table of a views launch (fill_params; views->cams in device memory), without the learned order.
+// `kind` and `q` as fill_params had them: Query::kAccumulate, a chunk of a progressive frame, is launched without a
+// claim-order pass (see below); Query::kViews, with the camera table q->cams in device memory, without the learned order.
 int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff,
-              const futhark_opaque_prepared_scene *scene, const RayQuery *accum, const RayQuery *views) {
+              const futhark_opaque_prepared_scene *scene, Query kind, const RayQuery *q) {
   futhark_context::Lane &L = ctx->lanes[lane_id];
   if (lane_id == 0) L.stream = ctx->stream;
   if (lc.kernel == RAY_B200_KERNEL_WAVEFRONT && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
@@ -377,7 +378,7 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   // order, and it leaves the scene's learned order as it found it (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = !accum && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = kind != Query::kAccumulate && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -392,7 +393,7 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   bool record_order = false;
   // (Frames of more than 2^24 tile-samples do not end on their longest paths any more, and un-mixing cheap and expensive
   // tiles costs them more than the shorter tail saves.)
-  if (!heavy_first && !accum && !views && scene && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
+  if (!heavy_first && kind == Query::kPixels && scene && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
       P.local_tiles < (1ll << 26) && (ctx->cfg.learn_order > 1 || P.local_tiles * (int64_t)P.spp <= ((int64_t)1 << 24))) {
     auto &oc = scene->order_cache;
     const bool same = oc.state == 1 && oc.h == P.H && oc.w == P.W && oc.spp == P.spp && oc.rank == P.rank && oc.world == P.world && oc.tiles == P.local_tiles;
@@ -436,9 +437,10 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   const bool self_signal = lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK;
   P.frame_flag = (ff && self_signal) ? ff->done_flag : nullptr;
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
-  if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, views);
+  const RayQuery &pq = q ? *q : RayQuery{};
+  if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, kind, pq);
   {
-    const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches, accum ? accum : views);
+    const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches, kind, pq);
     if (le == cudaErrorNotSupported) {
       set_error(ctx, "render: kernel %d is not part of this build (libray_b200.so carries mega / warpqueue; the alternatives "
                      "persistent / wavefront / streamqueue / lanewalk are in libray_b200_all.so, built with RAYB200_ALL_KERNELS)", lc.kernel);
@@ -533,8 +535,8 @@ int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, in
   acc.s_begin = s_begin;
   RenderParams P;
   LaunchConfig lc;
-  if (fill_params(ctx, p, h, w, s_end - s_begin, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc, &acc)) return 1;
-  return do_render(ctx, P, lc, 0, true, nullptr, p, &acc);
+  if (fill_params(ctx, p, h, w, s_end - s_begin, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc, Query::kAccumulate, &acc)) return 1;
+  return do_render(ctx, P, lc, 0, true, nullptr, p, Query::kAccumulate, &acc);
 }
 
 int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
@@ -552,7 +554,7 @@ int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark
   vq.n_views = n_views;
   RenderParams P;
   LaunchConfig lc;
-  if (fill_params(ctx, p, h, w, spp, 0, 1, out_pix_dev, out_rgb_dev, false, P, lc, nullptr, &vq)) return 1;
+  if (fill_params(ctx, p, h, w, spp, 0, 1, out_pix_dev, out_rgb_dev, false, P, lc, Query::kViews, &vq)) return 1;
   // View v's camera is what prepare_scene(h, w) of a scene with camera cams7[v] makes: make_camera with this call's aspect
   // ratio (ray.fut:243-244).  The table goes to stream-ordered device memory, freed behind the launch, so the caller may
   // reuse cams7_host as soon as the call returns.
@@ -571,7 +573,7 @@ int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark
   vq.cams = cams_dev;
   int rc = 0;
   if (ce != cudaSuccess) { set_error(ctx, "render_views_into: camera table upload failed: %s", cudaGetErrorString(ce)); rc = 1; }
-  if (!rc) rc = do_render(ctx, P, lc, 0, true, nullptr, p, nullptr, &vq);
+  if (!rc) rc = do_render(ctx, P, lc, 0, true, nullptr, p, Query::kViews, &vq);
   const cudaError_t fe = cudaFreeAsync(cams_dev, ctx->stream);
   if (!rc && fe != cudaSuccess) { set_error(ctx, "render_views_into: %s", cudaGetErrorString(fe)); rc = 1; }
   return rc;

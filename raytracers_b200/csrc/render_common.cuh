@@ -187,12 +187,13 @@ __device__ __forceinline__ Ray camera_ray(const float *c, const float u, const f
 }
 
 // get_ray for sample s of pixel (row j, column i): ray.fut:150-154 with pixel j i -> trace_ray (height-j) i
-// (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).  kAccum (a chunk of a progressive frame):
-// s is relative to the chunk, P.offsets starts at its first sample and is read even when P.spp == 1; at s = 0 of the
-// frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  kViews (a views launch): the
-// camera is view_cam, the pixel's view's 12 floats of RayQuery::cams, instead of P.cam.
-template <bool kAccum = false, bool kViews = false>
+// (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).  Query::kAccumulate (a chunk of a
+// progressive frame): s is relative to the chunk, P.offsets starts at its first sample and is read even when P.spp == 1;
+// at s = 0 of the frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  Query::kViews:
+// the camera is view_cam, the pixel's view's 12 floats of RayQuery::cams, instead of P.cam.
+template <Query kKind = Query::kPixels>
 __device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s, const float *view_cam = nullptr) {
+  constexpr bool kAccum = kKind == Query::kAccumulate, kViews = kKind == Query::kViews;
   float u, v;
   if (!kAccum && P.spp == 1) {
     u = (float)i / (float)P.W;
@@ -222,9 +223,9 @@ __device__ __forceinline__ bool item_pixel(const RenderParams &P, int k, int &i,
   return (long long)t < P.n_tiles && i < P.W && j < P.H;
 }
 
-// kViews: item k -> view v and pixel.  The views' tiles follow each other, view_tiles = tiles_x * tiles_y per view in the
-// row-major tile order of one frame (a views launch has no shards).  Tile t is in tile row r = t / tiles_x over all
-// views, which is row r - v * tiles_y of view v = r / tiles_y: two 32-bit divisions (n_tiles <= 2^25).
+// Query::kViews: item k -> view v and pixel.  The views' tiles follow each other, view_tiles = tiles_x * tiles_y per view
+// in the row-major tile order of one frame (a views launch has no shards).  Tile t is in tile row r = t / tiles_x over
+// all views, which is row r - v * tiles_y of view v = r / tiles_y: two 32-bit divisions (n_tiles <= 2^25).
 __device__ __forceinline__ bool item_view_pixel(const RenderParams &P, int k, int &v, int &i, int &j) {
   const unsigned t = (unsigned)(k >> 5);
   const int sub = k & 31;
@@ -253,11 +254,12 @@ __device__ __forceinline__ int claim_to_item(const RenderParams &P, int c) {
   return (perm << 11) | (c & 2047);
 }
 
-// kAccum: the sum of a progressive frame's samples [0, s_end), always scaled by P.inv_spp = 1/s_end (1 * x = x when
-// s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only).  kViews: pixel (i, j) of view
-// `view`, whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the float frames 12 GiB)
-template <bool kAccum = false, bool kViews = false>
+// Query::kAccumulate: the sum of a progressive frame's samples [0, s_end), always scaled by P.inv_spp = 1/s_end (1 * x = x
+// when s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only).  Query::kViews: pixel (i, j) of
+// view `view`, whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the float frames 12 GiB)
+template <Query kKind = Query::kPixels>
 __device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum, int view = 0) {
+  constexpr bool kAccum = kKind == Query::kAccumulate, kViews = kKind == Query::kViews;
   const V3 col = (!kAccum && P.spp == 1) ? sum : vscale(P.inv_spp, sum);
   const int pix = pack_pixel(col);
   if constexpr (kViews) {
@@ -418,7 +420,7 @@ cudaError_t opt_in_dynamic_smem(int max_dynamic_smem) {
 
 // Variant dispatch of the host launchers: with_flags(f, b0, b1, ...) calls f(std::bool_constant<b0>{}, ...), so run-time
 // flags pick compile-time template arguments.  f is instantiated for every combination of the flags passed, so a
-// launcher passes only axes whose combinations all exist (K3's ray-mode axes are dispatched apart from its pixel axes).
+// launcher passes only axes whose combinations all exist (K3's ray-query axes are dispatched apart from its pixel axes).
 template <class F>
 cudaError_t with_flags(F &&f) { return f(); }
 template <class F, class... B>
@@ -426,13 +428,16 @@ cudaError_t with_flags(F &&f, bool b, B... rest) {
   if (b) return with_flags([&](auto... c) { return f(std::true_type{}, c...); }, rest...);
   return with_flags([&](auto... c) { return f(std::false_type{}, c...); }, rest...);
 }
-// ... and with_query(f, q) calls f(std::integral_constant<Query, q>{}) for the ray-query kinds (Query::kPixels is not one)
+// ... and with_query(f, q) calls f(std::integral_constant<Query, q>{}) for every kind of Query
 template <class F>
 cudaError_t with_query(F &&f, Query q) {
   switch (q) {
+    case Query::kPixels: return f(std::integral_constant<Query, Query::kPixels>{});
     case Query::kClosest: return f(std::integral_constant<Query, Query::kClosest>{});
     case Query::kAnyHit: return f(std::integral_constant<Query, Query::kAnyHit>{});
     case Query::kMultiHit: return f(std::integral_constant<Query, Query::kMultiHit>{});
+    case Query::kAccumulate: return f(std::integral_constant<Query, Query::kAccumulate>{});
+    case Query::kViews: return f(std::integral_constant<Query, Query::kViews>{});
     default: return cudaErrorInvalidValue;
   }
 }

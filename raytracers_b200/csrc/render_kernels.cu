@@ -43,9 +43,12 @@ __global__ void __launch_bounds__(128) render_mega_kernel(const __grid_constant_
 // ("heavy": possibly 50 bounces) are pulled into its first half: key = position in the permuted sequence, halved for
 // heavy tiles, stable-sorted.  What is claimed in the second half ends within probe_segments traversals.  The probe
 // traces sample 0 of 1, 2 or 4 pixels per 8x4 tile, so its own latency is bounded by the same cap.  The order only
-// changes WHEN a pixel is rendered, never its value.
+// changes WHEN a pixel is rendered, never its value.  The probe of a views launch (Query::kViews) traces each tile with
+// its view's camera, the 12 floats of `cams` (RayQuery::cams) at its view; a whole frame (Query::kPixels) leaves cams
+// unread.
+template <Query kKind>
 __global__ void __launch_bounds__(256) tile_probe_kernel(const __grid_constant__ RenderParams P, uint32_t *__restrict__ keys,
-                                                         int32_t *__restrict__ ids) {
+                                                         int32_t *__restrict__ ids, const float *__restrict__ cams) {
   const int probes = P.probes_per_tile;  // 1, 2 or 4: the lanes of a tile are neighbours in a warp
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long lt = t / probes;
@@ -53,43 +56,11 @@ __global__ void __launch_bounds__(256) tile_probe_kernel(const __grid_constant__
   bool alive = false;
   if (lt < P.local_tiles) {
     const int sub = q == 0 ? 11 : (q == 1 ? 22 : (q == 2 ? 17 : 5));  // pixels (3,1) (6,2) (1,2) (5,0) of the tile
-    int i, j;
-    if (item_pixel(P, (int)(lt << 5) | sub, i, j)) {
-      const GlobalScene sc{P.nodes, P.geom};
-      Ray r = primary_ray(P, i, j, 0);
-      V3 light = v3(1.0f, 1.0f, 1.0f), colour;
-      int depth = 0, segments = 0;
-      WorkCounters wc;
-      do {
-        alive = advance_path<false>(sc, P, r, light, depth, colour, wc);
-      } while (alive && ++segments < P.probe_segments);
-    }
-  }
-  if (probes > 1) alive |= __shfl_xor_sync(kFullMask, alive, 1);
-  if (probes > 2) alive |= __shfl_xor_sync(kFullMask, alive, 2);
-  if (q == 0 && lt < P.local_tiles) {
-    const long long chunk = lt >> 6;
-    const uint32_t pos = (uint32_t)((chunk * P.chunk_stride_inv) % P.n_chunks) << 6 | (uint32_t)(lt & 63);
-    keys[lt] = alive ? pos >> 1 : pos;
-    ids[lt] = (int32_t)lt;
-  }
-}
-
-// The probe of a views launch (ray_b200_render_views_into): tile_probe_kernel with each tile traced by its view's camera,
-// the 12 floats of `cams` (RayQuery::cams) at its view.
-__global__ void __launch_bounds__(256) tile_probe_views_kernel(const __grid_constant__ RenderParams P, uint32_t *__restrict__ keys,
-                                                               int32_t *__restrict__ ids, const float *__restrict__ cams) {
-  const int probes = P.probes_per_tile;
-  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long lt = t / probes;
-  const int q = (int)(t - lt * probes);
-  bool alive = false;
-  if (lt < P.local_tiles) {
-    const int sub = q == 0 ? 11 : (q == 1 ? 22 : (q == 2 ? 17 : 5));
+    constexpr bool kViews = kKind == Query::kViews;
     int v, i, j;
-    if (item_view_pixel(P, (int)(lt << 5) | sub, v, i, j)) {
+    if (kViews ? item_view_pixel(P, (int)(lt << 5) | sub, v, i, j) : item_pixel(P, (int)(lt << 5) | sub, i, j)) {
       const GlobalScene sc{P.nodes, P.geom};
-      Ray r = primary_ray<false, true>(P, i, j, 0, cams + 12 * (size_t)v);
+      Ray r = kViews ? primary_ray<kKind>(P, i, j, 0, cams + 12 * (size_t)v) : primary_ray(P, i, j, 0);
       V3 light = v3(1.0f, 1.0f, 1.0f), colour;
       int depth = 0, segments = 0;
       WorkCounters wc;
@@ -156,9 +127,10 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // finished sample's colour is parked in an L2-resident buffer so that the pixel is summed in SAMPLE
 // ORDER when its last sample lands, which keeps the result bit-identical to the sequential definition.
 //
-// The query kind (kQuery, render_params.h Query) says what is traced.  Query::kPixels: camera rays of a frame, as above;
-// Q is unused.  Every other kind is a ray query (include/ray_b200.h "ray queries"), "ray mode" below: the work items are
-// the caller's rays instead of pixels.  A claim c is ray c (no tile order), a slot is filled from Q.rays, and boxes are
+// The kind (kQuery, render_params.h Query) says what is traced.  The pixel kinds trace camera rays, as above:
+// Query::kPixels a whole frame (Q is unused), Query::kAccumulate and Query::kViews as described at the end.  The other
+// kinds are ray queries (include/ray_b200.h "ray queries"), "ray mode" below: the work items are the caller's rays
+// instead of pixels.  A claim c is ray c (no tile order), a slot is filled from Q.rays, and boxes are
 // tested against the query's (t_min, t_max) instead of the literal (0, 1e9).  Rays of a batch are not coherent: ray mode
 // has no packet walk and no spread samples.
 //
@@ -196,20 +168,20 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // to ray_d.w (the leaf batch loads ray_d).  Ranged variants exist only as a separate template instantiation, so the
 // per-call variants keep their code.
 //
-// kAccum (pixel mode, progressive rendering, include/ray_b200.h ray_b200_render_accumulate): the launch traces samples
-// [Q.s_begin, Q.s_begin + P.spp) of every pixel.  Everything that counts samples is chunk-relative: P.spp is the chunk
-// length (it sizes cbuf and bounds p_ms's 16-bit sample, as spp does for a whole frame), P.offsets starts at the
-// chunk's first sample and is read for every sample (primary_ray<true>), and sample rel of the chunk is sample
-// s_begin + rel of the frame.  Q.accum holds each pixel's f32 sum of samples [0, s_begin): with s_begin > 0 the in-order
-// sum starts from it (p_sum at the pixel-bound refill, the first term of finalize_pixels), with s_begin == 0 from sample
-// 0's colour itself, as in a whole frame.  Where the pixel is written (scaled by P.inv_spp = 1/s_end,
-// write_pixel<true>), its owner stores the new sum back to Q.accum in place.  So a chain of chunks computes the same f32
-// additions in the same order as one frame of s_end samples.
+// Query::kAccumulate, one chunk of a progressive frame (include/ray_b200.h ray_b200_render_accumulate): the launch traces
+// samples [Q.s_begin, Q.s_begin + P.spp) of every pixel.  Everything that counts samples is chunk-relative: P.spp is the
+// chunk length (it sizes cbuf and bounds p_ms's 16-bit sample, as spp does for a whole frame), P.offsets starts at the
+// chunk's first sample and is read for every sample (primary_ray<Query::kAccumulate>), and sample rel of the chunk is
+// sample s_begin + rel of the frame.  Q.accum holds each pixel's f32 sum of samples [0, s_begin): with s_begin > 0 the
+// in-order sum starts from it (p_sum at the pixel-bound refill, the first term of finalize_pixels), with s_begin == 0 from
+// sample 0's colour itself, as in a whole frame.  Where the pixel is written (scaled by P.inv_spp = 1/s_end,
+// write_pixel<Query::kAccumulate>), its owner stores the new sum back to Q.accum in place.  So a chain of chunks computes
+// the same f32 additions in the same order as one frame of s_end samples.
 //
-// kViews (pixel mode, include/ray_b200.h ray_b200_render_views_into): the launch renders Q.n_views frames of one size
-// from one prepared scene.  The work items are the tiles of all views, view after view (P.n_tiles = P.local_tiles =
-// n_views * Q.view_tiles), so the chunk permutation of the claim order mixes the views' sky and ground tiles as it mixes
-// one frame's.  Where a pixel item becomes a pixel (pixel_of: the pixel-bound refill, finish_path's next sample and store,
+// Query::kViews, several views in one launch (include/ray_b200.h ray_b200_render_views_into): the launch renders
+// Q.n_views frames of one size from one prepared scene.  The work items are the tiles of all views, view after view
+// (P.n_tiles = P.local_tiles = n_views * Q.view_tiles), so the chunk permutation of the claim order mixes the views' sky
+// and ground tiles as it mixes one frame's.  Where a pixel item becomes a pixel (pixel_of: the pixel-bound refill, finish_path's next sample and store,
 // the spread dispenser and finalize_pixels) it also gives its view v; the camera ray reads view v's 12 floats of Q.cams
 // instead of P.cam, and the pixel is stored at offset v * H * W.  Nothing else depends on the view, so every view's
 // pixel sees exactly the arithmetic of a one-view frame whose P.cam is that camera.
@@ -223,16 +195,14 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
 
-template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false,
-          bool kAccum = false, bool kViews = false>
+template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
-  constexpr bool kRays = kQuery != Query::kPixels;  // ray mode
+  constexpr bool kRays = is_ray_query(kQuery);  // ray mode
+  constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews;
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
-  static_assert(!kAccum || !kRays, "progressive rendering accumulates the samples of pixels");
-  static_assert(!kViews || (!kRays && !kAccum), "views are whole pixel frames");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
   const float4 *s_nodes, *s_geom;
@@ -333,13 +303,13 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       int pi, pj, pv;
       pixel_of(item, pv, pi, pj);
       if (s < spp) {
-        const Ray nr = primary_ray<kAccum, kViews>(P, pi, pj, s, view_cam(pv));
+        const Ray nr = primary_ray<kQuery>(P, pi, pj, s, view_cam(pv));
         ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
         ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
         p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
         p_sum[slot] = make_float4(sum.x, sum.y, sum.z, __int_as_float(s));
       } else {
-        write_pixel<kAccum, kViews>(P, item, pi, pj, sum, pv);
+        write_pixel<kQuery>(P, item, pi, pj, sum, pv);
         if constexpr (kAccum) {
           float *a = accum_of(pi, pj);
           a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
@@ -446,7 +416,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const int item = ring_item[m];
         int pi, pj, pv;
         if (pixel_of(item, pv, pi, pj)) {
-          write_pixel<kAccum, kViews>(P, item, pi, pj, v3(sum, g, b), pv);
+          write_pixel<kQuery>(P, item, pi, pj, v3(sum, g, b), pv);
           if constexpr (kAccum) {
             float *a = accum_of(pi, pj);
             a[0] = sum; a[1] = g; a[2] = b;
@@ -516,7 +486,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                 p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
               } else if (item < total) {
                 if (pixel_of(item, pv, pi, pj)) {
-                  const Ray r = primary_ray<kAccum, kViews>(P, pi, pj, 0, view_cam(pv));
+                  const Ray r = primary_ray<kQuery>(P, pi, pj, 0, view_cam(pv));
                   p_item[slot] = item;
                   ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                   ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -570,7 +540,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               const int item = ring_item[m];
               int pi, pj, pv;
               if (pixel_of(item, pv, pi, pj)) {
-                const Ray r = primary_ray<kAccum, kViews>(P, pi, pj, s, view_cam(pv));
+                const Ray r = primary_ray<kQuery>(P, pi, pj, s, view_cam(pv));
                 p_item[slot] = item;
                 ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                 ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -663,7 +633,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       // up to 32 (ray, sphere) pairs: closest_hit (ray.fut:78-81) for pixels and closest-hit queries; sphere_hit L[i] r
       // t_min t_max with the query's own t_min (no epsilon) for any-hit and multi-hit queries
       constexpr bool kFull = decltype(full_tag)::value;
-      constexpr bool kEpsilon = kQuery == Query::kPixels || kQuery == Query::kClosest;
+      constexpr bool kEpsilon = !kRays || kQuery == Query::kClosest;
       const int n = kFull ? 32 : n_part;
       bool hit = false;
       uint32_t tb = 0;
@@ -973,7 +943,7 @@ __global__ void detile_kernel(const int32_t *__restrict__ gathered, int32_t *__r
 // opt in to > 48 KB of dynamic shared memory on first use (launch_opted_in), not at context creation:
 // futhark_context_new does not touch the ~50 template instantiations it will never launch.
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
-                          int64_t *launches, const RayQuery *pixq) {
+                          int64_t *launches, Query kind, const RayQuery &q) {
   const long long items = p.local_tiles * kTilePixels;
   if (items <= 0) return cudaSuccess;
   if (lc.kernel == 1) {  // RAY_B200_KERNEL_MEGA
@@ -985,17 +955,15 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
   }
   if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
   if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  return launch_warpqueue(p, Query::kPixels, false, pixq ? *pixq : RayQuery{}, lc, stream, launches);   // RAY_B200_KERNEL_WARPQUEUE
+  return launch_warpqueue(p, kind, false, q, lc, stream, launches);                // RAY_B200_KERNEL_WARPQUEUE
 }
 
-// K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A pixel frame, or a ray query of kind `kind`: the
-// same kernel in ray mode, without spread samples or packets; `ranged`: its rays carry their own intervals.
+// K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A launch of pixel kind `kind`, or a ray query of
+// that kind: the same kernel in ray mode, without spread samples or packets; `ranged`: its rays carry their own intervals.
 cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
                              cudaStream_t stream, int64_t *launches) {
-  const bool rays = kind != Query::kPixels;
+  const bool rays = is_ray_query(kind);
   const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
-  const bool accum = !rays && q.accum != nullptr;   // a chunk of a progressive frame
-  const bool views = !rays && q.cams != nullptr;    // several views of the scene
   // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
   // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
   const long long work = rays ? (long long)q.n : p.local_tiles * kTilePixels * (spread ? (long long)p.spp : 1ll);
@@ -1011,24 +979,18 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
   long long ctas = lc.sm_count;
   const long long useful = (work + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
   if (ctas > useful) ctas = useful;
-  cudaError_t e;
-  if (rays)
-    e = with_query([&](auto query) {
+  const cudaError_t e = with_query([&](auto query) {
+    if constexpr (is_ray_query(query))
       return with_flags([&](auto k2, auto a, auto s, auto rg) {
         return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, query, rg>>(
             lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
       }, k == 2, all_nodes, sph, ranged);
-    }, kind);
-  else if (views)
-    e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, Query::kPixels, false, false, true>>(
-          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
-    }, k == 2, spread, packet, all_nodes, sph);
-  else
-    e = with_flags([&](auto k2, auto sp, auto pk, auto a, auto s, auto ac) {
-      return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, Query::kPixels, false, ac>>(
-          lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
-    }, k == 2, spread, packet, all_nodes, sph, accum);
+    else
+      return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
+        return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(
+            lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
+      }, k == 2, spread, packet, all_nodes, sph);
+  }, kind);
   if (e == cudaSuccess) (*launches)++;
   return e;
 }
@@ -1057,11 +1019,11 @@ size_t tile_order_sort_bytes(int64_t local_tiles) {
   return bytes;
 }
 
-void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches,
-                       const RayQuery *views) {
-  const long long threads = (long long)p.local_tiles * p.probes_per_tile;
-  if (views) tile_probe_views_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(p, b.keys, b.ids, views->cams);
-  else tile_probe_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(p, b.keys, b.ids);
+void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches, Query kind,
+                       const RayQuery &q) {
+  const unsigned blocks = (unsigned)(((long long)p.local_tiles * p.probes_per_tile + 255) / 256);
+  if (kind == Query::kViews) tile_probe_kernel<Query::kViews><<<blocks, 256, 0, stream>>>(p, b.keys, b.ids, q.cams);
+  else tile_probe_kernel<Query::kPixels><<<blocks, 256, 0, stream>>>(p, b.keys, b.ids, nullptr);
   size_t bytes = b.sort_tmp_bytes;
   cub::DeviceRadixSort::SortPairs(b.sort_tmp, bytes, b.keys, b.keys_sorted, b.ids, b.order, (int)p.local_tiles, 0,
                                   tile_order_key_bits(p.n_chunks), stream);

@@ -58,14 +58,21 @@ struct RenderParams {
   unsigned long long *warp_trace;
 };
 
-// What the warp-queue kernel traces (its template parameter kQuery): camera rays of a frame, or the caller's rays of a
-// ray query (include/ray_b200.h "ray queries") to their closest hit or along their path (RayQuery::hits != NULL tells
-// the two apart at run time), to their first accepted sphere (occlusion) or to their k nearest ones (multi-hit).
-enum class Query { kPixels, kClosest, kAnyHit, kMultiHit };
+// What the warp-queue kernel traces (its template parameter kQuery), and which RayQuery fields the launch reads.
+// Pixel kinds, camera rays: kPixels, a whole frame (no field); kAccumulate, one chunk of a progressive frame (accum,
+// s_begin); kViews, several views in one launch (cams, n_views, view_tiles).  Ray kinds, the caller's rays of a ray query
+// (include/ray_b200.h "ray queries"; rays, n, perm, t_min, t_max): kClosest, to their closest hit (hits) or along their
+// path (rgb, segments, max_depth; hits == NULL tells the two apart at run time); kAnyHit, to their first accepted sphere
+// (occluded); kMultiHit, to their k nearest ones (hits, k, counts).  New kinds go at the end: kernel names carry the
+// values, and tools/sass_compare.py reads older builds' names by them.
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews };
+__host__ __device__ constexpr bool is_ray_query(Query q) {
+  return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
+}
 
-// Ray queries: the warp-queue kernel's ray-mode instantiations trace caller-supplied rays instead of camera rays.  A block
-// of its own, passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those
-// parameters, and with them the constant-bank offsets in every pixel instantiation's code.
+// The fields of a launch that RenderParams does not carry (see Query for which kind reads which).  A block of its own,
+// passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those parameters, and
+// with them the constant-bank offsets in every pixel instantiation's code.
 struct RayQuery {
   const float *rays;        // [n][6]: origin.xyz, dir.xyz; ranged query: [n][8] = struct ray_b200_ray
   float *rgb;               // path query: [n][3] colour of ray_colour (ray.fut:126-148)
@@ -79,16 +86,15 @@ struct RayQuery {
   uint8_t *occluded;        // occlusion query: [n] 0 / 1
   int32_t k;                // multi-hit query: records per ray, in [1, 64]
   int32_t *counts;          // multi-hit query, optional: [n] accepted leaves per ray, not capped at k
-  // progressive rendering (pixel mode, kernel template parameter kAccum; include/ray_b200.h ray_b200_render_accumulate):
-  // the frame's samples [s_begin, s_begin + P.spp) are added to accum, row-major [H][W][3], the running f32 sum of each
-  // pixel's samples [0, s_begin) (not read when s_begin == 0)
+  // progressive rendering (Query::kAccumulate; include/ray_b200.h ray_b200_render_accumulate): the frame's samples
+  // [s_begin, s_begin + P.spp) are added to accum, row-major [H][W][3], the running f32 sum of each pixel's samples
+  // [0, s_begin) (not read when s_begin == 0)
   float *accum;
   int32_t s_begin;
-  // several views of one prepared scene (pixel mode, kernel template parameter kViews; include/ray_b200.h
-  // ray_b200_render_views_into): n_views frames of P.W x P.H, one after the other.  Work-item tiles
-  // [v * view_tiles, (v + 1) * view_tiles) are view v's tiles in the row-major tile order of one frame; view v is drawn
-  // with the camera cams[v] (device [n_views][12], 16-byte aligned, laid out as RenderParams::cam) and written at pixel
-  // offset v * H * W of the outputs
+  // several views of one prepared scene (Query::kViews; include/ray_b200.h ray_b200_render_views_into): n_views frames
+  // of P.W x P.H, one after the other.  Work-item tiles [v * view_tiles, (v + 1) * view_tiles) are view v's tiles in the
+  // row-major tile order of one frame; view v is drawn with the camera cams[v] (device [n_views][12], 16-byte aligned,
+  // laid out as RenderParams::cam) and written at pixel offset v * H * W of the outputs
   const float *cams;
   int32_t n_views, view_tiles;
 };
@@ -132,14 +138,12 @@ struct LaunchConfig {
   int max_dynamic_smem;  // the device's opt-in shared-memory limit (kernels opt in on first launch)
 };
 
-// A frame on the kernel lc.kernel names (render_kernels.cu); `pixq` (NULL = a whole frame of one view): a progressive-
-// rendering call's running sums (RayQuery::accum, s_begin) or a views call's camera table (RayQuery::cams, n_views,
-// view_tiles), on the warp-queue kernel only
+// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate and kViews, which read q,
+// on the warp-queue kernel only
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
-                          int64_t *launches, const RayQuery *pixq = nullptr);
-// The warp-queue kernel (render_kernels.cu): a pixel frame (kind = Query::kPixels; q unused unless q.accum is set, which
-// picks the accumulating variants, or q.cams, which picks the views variants), or a ray query of that kind (whatever
-// lc.kernel says); `ranged`: q.rays is [n][8] with an interval per ray (hit, occlusion and multi-hit queries)
+                          int64_t *launches, Query kind, const RayQuery &q);
+// The warp-queue kernel (render_kernels.cu): a launch of kind `kind`, a pixel kind or a ray query (whatever lc.kernel
+// says); `ranged`: q.rays is [n][8] with an interval per ray (hit, occlusion and multi-hit queries)
 cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
                              cudaStream_t stream, int64_t *launches);
 // per translation unit: K5 (render_lanewalk.cu) and the alternatives K1 / K2 / K4 (render_alt_kernels.cu; a product
@@ -161,9 +165,9 @@ inline int tile_order_key_bits(int32_t n_chunks) {  // keys are positions < n_ch
   while (bits < 32 && (1ll << bits) < (long long)n_chunks * 64) bits++;
   return bits;
 }
-// `views` (NULL = one view): the probe traces each tile with its view's camera (RayQuery::cams)
-void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches,
-                       const RayQuery *views = nullptr);
+// of a frame of pixel kind `kind`: Query::kViews probes each tile with its view's camera (q.cams)
+void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches, Query kind,
+                       const RayQuery &q);
 // The same order table from a recorded frame: tiles whose longest path had >= long_path segments first, both groups in
 // the permuted claim sequence (cost = RenderParams::tile_cost of the recorded frame)
 void launch_tile_order_from_cost(const RenderParams &p, const uint32_t *cost, int32_t long_path, const TileOrderBuffers &b,

@@ -3,7 +3,10 @@
 The library is compiled on first use into a fresh temporary directory with oracle/Makefile's flags, so a read-only
 checkout works.  It contains the whole CPU oracle (oracle/oracle.cpp, included unchanged) plus the four ray queries
 (objs_hit, ray_colour, occlusion and multi-hit) for caller-supplied rays; its handles are its own, not liboracle.so's.
-Used by the ray-query tests, __graft_entry__.smoke() and tools/bench_rays.py.
+The ranged forms (methods *_ranged) take rays as float32[n][8] = struct ray_b200_ray (origin, t_min, direction, t_max):
+each answer is that of the per-call query for the ray alone with its (t_min, t_max), and a ray whose interval the
+per-call entry points reject (t_min not finite and >= 0, t_max not finite) gets the empty answer, as the library
+defines it.  Used by the ray-query tests, __graft_entry__.smoke() and tools/bench_rays.py.
 """
 import ctypes as C
 import os
@@ -53,12 +56,22 @@ def lib():
         L.oracle_trace_multi_hits.restype = C.c_int
         L.oracle_trace_multi_hits.argtypes = [vp, vp, i64, f32, f32, i32, vp, vp, i32]
         L.oracle_camera_ray.argtypes = [vp, i64, i64, i32, i64, i64, i32, vp]
+        L.oracle_trace_hits_ranged.restype = C.c_int
+        L.oracle_trace_hits_ranged.argtypes = [vp, vp, i64, vp, i32]
+        L.oracle_trace_occluded_ranged.restype = C.c_int
+        L.oracle_trace_occluded_ranged.argtypes = [vp, vp, i64, vp, i32]
+        L.oracle_trace_multi_hits_ranged.restype = C.c_int
+        L.oracle_trace_multi_hits_ranged.argtypes = [vp, vp, i64, i32, vp, vp, i32]
         _lib = L
     return _lib
 
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _rays8(rays8):
+    return np.ascontiguousarray(rays8, np.float32).reshape(-1, 8)
 
 
 class Prepared:
@@ -109,6 +122,31 @@ class Prepared:
         if lib().oracle_trace_multi_hits(self._h, _p(r), r.shape[0], float(t_min), float(t_max), int(k), _p(out), _p(counts),
                                          int(threads)) != 0:
             raise RuntimeError("oracle_trace_multi_hits failed")
+        return out, counts
+
+    def trace_hits_ranged(self, rays8, threads=0):
+        """objs_hit of every ray with its own interval: float32[n][8] records as struct ray_b200_hit."""
+        r = _rays8(rays8)
+        out = np.empty((r.shape[0], 8), np.float32)
+        if lib().oracle_trace_hits_ranged(self._h, _p(r), r.shape[0], _p(out), int(threads)) != 0:
+            raise RuntimeError("oracle_trace_hits_ranged failed")
+        return out
+
+    def trace_occluded_ranged(self, rays8, threads=0):
+        """Occlusion of every ray with its own interval: bool[n]."""
+        r = _rays8(rays8)
+        out = np.empty(r.shape[0], np.uint8)
+        if lib().oracle_trace_occluded_ranged(self._h, _p(r), r.shape[0], _p(out), int(threads)) != 0:
+            raise RuntimeError("oracle_trace_occluded_ranged failed")
+        return out.view(np.bool_)
+
+    def trace_multi_hits_ranged(self, rays8, k, threads=0):
+        """The multi-hit query of every ray with its own interval: (float32[n][k][8] records, int32[n] counts)."""
+        r = _rays8(rays8)
+        out = np.empty((r.shape[0], int(k), 8), np.float32)
+        counts = np.empty(r.shape[0], np.int32)
+        if lib().oracle_trace_multi_hits_ranged(self._h, _p(r), r.shape[0], int(k), _p(out), _p(counts), int(threads)) != 0:
+            raise RuntimeError("oracle_trace_multi_hits_ranged failed")
         return out, counts
 
     def camera_ray(self, h, w, j, i, s=0, spp=1):

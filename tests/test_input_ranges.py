@@ -13,8 +13,7 @@ import functools
 import numpy as np
 import pytest
 
-import ray_interval_oracle as RQ   # tests/ray_interval_oracle.py: the CPU oracle of the ranged ray queries
-import ray_query_oracle as Q      # tests/ray_query_oracle.py: the CPU oracle of the per-call ray queries
+import ray_query_oracle as Q   # tests/ray_query_oracle.py: the CPU oracle of the per-call and the ranged ray queries
 from oracle import pyoracle as O
 from ray_query_cases import _dev, _np, _torch, bits_differ, hits_differ, quantise, random_rays
 
@@ -455,7 +454,6 @@ def check_queries(ctx, pr, spheres, cam, rays, intervals, ranged_rays, ks=(1, 8)
     """trace_hits, trace_occluded and trace_multi_hits (each k of ks) per call on every interval and ranged on
     `ranged_rays`, against the oracles; records compared NaN-aware.  Returns the number of hits the oracle found."""
     o = Q.prepare_custom(spheres, cam, H, W)
-    ro = RQ.prepare_custom(spheres, cam, H, W)
     d, d8 = _dev(rays), _dev(ranged_rays)
     found = 0
     for t_min, t_max in intervals:
@@ -470,11 +468,11 @@ def check_queries(ctx, pr, spheres, cam, rays, intervals, ranged_rays, ks=(1, 8)
             want_m, want_n = o.trace_multi_hits(rays, k, t_min, t_max)
             assert hits_differ(_hit_records(out).reshape(-1, 8), want_m.reshape(-1, 8)) == 0, f"multi k={k} {what}"
             assert int((_np(out["count"]) != want_n).sum()) == 0, f"multi count k={k} {what}"
-    assert hits_differ(_hit_records(ctx.trace_hits(pr, d8)), ro.trace_hits_ranged(ranged_rays)) == 0, "hits ranged"
-    assert int((_np(ctx.trace_occluded(pr, d8)) != ro.trace_occluded_ranged(ranged_rays)).sum()) == 0, "occluded ranged"
+    assert hits_differ(_hit_records(ctx.trace_hits(pr, d8)), o.trace_hits_ranged(ranged_rays)) == 0, "hits ranged"
+    assert int((_np(ctx.trace_occluded(pr, d8)) != o.trace_occluded_ranged(ranged_rays)).sum()) == 0, "occluded ranged"
     for k in ks:
         out = ctx.trace_multi_hits(pr, d8, k)
-        want_m, want_n = ro.trace_multi_hits_ranged(ranged_rays, k)
+        want_m, want_n = o.trace_multi_hits_ranged(ranged_rays, k)
         assert hits_differ(_hit_records(out).reshape(-1, 8), want_m.reshape(-1, 8)) == 0, f"multi ranged k={k}"
         assert int((_np(out["count"]) != want_n).sum()) == 0, f"multi ranged count k={k}"
     return found
@@ -500,7 +498,6 @@ def test_subnormal_queries(R, e):
     s, c = _tiny_scene(e)
     rays = _tiny_rays(s)
     o = Q.prepare_custom(s, c, H, W)
-    ro = RQ.prepare_custom(s, c, H, W)
     _, hi = _per_ray_intervals(s, len(rays), e)
     rays8 = _ranged(rays, np.zeros(len(rays), np.float32), hi)
     with R.Context() as ctx:
@@ -509,13 +506,13 @@ def test_subnormal_queries(R, e):
         want = o.trace_occluded(rays, 0.0, 1e9)
         assert want.any()
         assert int((_np(ctx.trace_occluded(pr, d, t_min=0.0, t_max=1e9)) != want).sum()) == 0
-        assert int((_np(ctx.trace_occluded(pr, d8)) != ro.trace_occluded_ranged(rays8)).sum()) == 0
+        assert int((_np(ctx.trace_occluded(pr, d8)) != o.trace_occluded_ranged(rays8)).sum()) == 0
         for k in (1, 8):
             out = ctx.trace_multi_hits(pr, d, k, t_min=0.0, t_max=1e9)
             want_m, want_n = o.trace_multi_hits(rays, k, 0.0, 1e9)
             assert hits_differ(_hit_records(out).reshape(-1, 8), want_m.reshape(-1, 8)) == 0, f"multi k={k}"
             assert int((_np(out["count"]) != want_n).sum()) == 0, f"multi count k={k}"
             out = ctx.trace_multi_hits(pr, d8, k)
-            want_m, want_n = ro.trace_multi_hits_ranged(rays8, k)
+            want_m, want_n = o.trace_multi_hits_ranged(rays8, k)
             assert hits_differ(_hit_records(out).reshape(-1, 8), want_m.reshape(-1, 8)) == 0, f"multi ranged k={k}"
             assert int((_np(out["count"]) != want_n).sum()) == 0, f"multi ranged count k={k}"

@@ -8,8 +8,7 @@ import ctypes
 import numpy as np
 import pytest
 
-import ray_interval_oracle as RQ   # tests/ray_interval_oracle.py: the CPU oracle of the ranged ray queries
-import ray_query_oracle as Q      # tests/ray_query_oracle.py: the CPU oracle of the per-call ray queries
+import ray_query_oracle as Q   # tests/ray_query_oracle.py: the CPU oracle of the per-call and the ranged ray queries
 from ray_query_cases import (ALONG_Z, GiB, INTERVALS, PLANS, RANDOM_SCENES, SEGMENT, TWO_CAM, TWO_SPHERES, _dev, _gpu_case,
                              _np, _torch, hits_differ, random_rays)
 
@@ -18,23 +17,12 @@ from ray_query_cases import (ALONG_Z, GiB, INTERVALS, PLANS, RANDOM_SCENES, SEGM
 KINDS = ("hits", "occluded", "multi")
 
 
-class Oracle:
-    """The CPU oracle of one prepared scene: the per-call queries (ray_query_oracle) and the ranged ones
-    (ray_interval_oracle, methods named *_ranged), each library with its own handle of the same scene."""
-
-    def __init__(self, per_call, ranged):
-        self._per_call, self._ranged = per_call, ranged
-
-    def __getattr__(self, name):
-        return getattr(self._ranged if name.endswith("_ranged") else self._per_call, name)
-
-
 def oracle(name, h, w, n=None):
-    return Oracle(Q.prepare(name, h, w, n=n), RQ.prepare(name, h, w, n=n))
+    return Q.prepare(name, h, w, n=n)
 
 
 def oracle_custom(spheres, cam7, h, w):
-    return Oracle(Q.prepare_custom(spheres, cam7, h, w), RQ.prepare_custom(spheres, cam7, h, w))
+    return Q.prepare_custom(spheres, cam7, h, w)
 
 
 def ranged(rays, t_min, t_max):

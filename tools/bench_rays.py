@@ -31,7 +31,7 @@ Random rays come from a fixed seed: origins uniform in the scene's bounding box 
 uniform on the sphere, so every run sees the same inputs.  `ms` = the median of 3 queries (CUDA events of the context,
 after one warm-up query that loads the kernel); Mrays/s = objs_hit calls / kernel time (one per ray for a hit query, the
 segments trace_paths reports for a path query); `parity` = differing values against the CPU oracle
-(tests/ray_query_oracle.py; tests/ray_interval_oracle.py for the ranged queries) on 4096 rays spread over the batch.
+(tests/ray_query_oracle.py) on 4096 rays spread over the batch.
 The card's name and power limit are read in the same run.
 """
 import argparse
@@ -54,10 +54,9 @@ def random_rays(np, spheres, count, seed):
     return np.ascontiguousarray(np.concatenate([o, d / np.linalg.norm(d, axis=1, keepdims=True)], 1), np.float32)
 
 
-def ranged_workload(np, torch, R, Q, RQ, ctx, timed, bits, name, n_spheres, hh, ww, sc, pr, mode, k, args):
+def ranged_workload(np, torch, R, Q, ctx, timed, bits, name, n_spheres, hh, ww, sc, pr, mode, k, args):
     """One workload of rays that carry their own interval (struct ray_b200_ray), with the per-call form beside it."""
-    o = Q.prepare(name, hh, ww, n=n_spheres)            # the per-call queries
-    ro = RQ.prepare(name, hh, ww, n=n_spheres)          # the ranged ones
+    o = Q.prepare(name, hh, ww, n=n_spheres)
     if mode == "lights":
         cam = torch.from_numpy(R.camera_rays(pr.info()["camera"], hh, ww).reshape(-1, 6)).cuda()
         hit = ctx.trace_hits(pr, cam)
@@ -107,17 +106,17 @@ def ranged_workload(np, torch, R, Q, RQ, ctx, timed, bits, name, n_spheres, hh, 
         rec["t_min"], rec["t_max"] = t_min, t_max
     sub = np.linspace(0, cnt - 1, 4096).astype(np.int64)
     if mode == "hits_r":
-        rec["parity"] = int((bits(out8[:, 0].cpu().numpy()[sub]) != bits(ro.trace_hits_ranged(rays8[sub]))).sum())
+        rec["parity"] = int((bits(out8[:, 0].cpu().numpy()[sub]) != bits(o.trace_hits_ranged(rays8[sub]))).sum())
         rec["percall_parity"] = int((bits(out6[:, 0].cpu().numpy()[sub]) != bits(o.trace_hits(rays6[sub], t_min, t_max))).sum())
     elif mode == "multi_r":
-        want, want_c = ro.trace_multi_hits_ranged(rays8[sub], k)
+        want, want_c = o.trace_multi_hits_ranged(rays8[sub], k)
         rec["parity"] = int((bits(out8.cpu().numpy()[sub]) != bits(want)).sum()) + int((c8.cpu().numpy()[sub] != want_c).sum())
         want, want_c = o.trace_multi_hits(rays6[sub], k, t_min, t_max)
         rec["percall_parity"] = int((bits(out6.cpu().numpy()[sub]) != bits(want)).sum()) + int((c6.cpu().numpy()[sub] != want_c).sum())
         rec["k"], rec["mean_count"] = k, round(float(c8.double().mean()), 3)
     else:
         occ8, occ6 = occ8.cpu().numpy(), occ6.cpu().numpy()
-        rec["parity"] = int((occ8[sub] != ro.trace_occluded_ranged(rays8[sub])).sum())
+        rec["parity"] = int((occ8[sub] != o.trace_occluded_ranged(rays8[sub])).sum())
         rec["percall_parity" if mode != "lights" else "segment_parity"] = int((occ6[sub] != o.trace_occluded(rays6[sub], t_min, t_max)).sum())
         rec["occluded_fraction"] = round(float(occ8.mean()), 4)
         if mode == "lights":
@@ -135,7 +134,6 @@ def main():
     import torch
 
     import ray_query_oracle as Q
-    import ray_interval_oracle as RQ
     import raytracers_b200 as R
     from ray_query_cases import quantise
 
@@ -182,7 +180,7 @@ def main():
         pr = ctx.prepare_scene(hh, ww, sc)
         t_min, t_max = (1e-4, 1 - 1e-4) if mode == "shadow" else ((0.0, 1e9) if mode == "depth" else (0.1, 1e9))
         if mode in ("hits_r", "occluded_r", "multi_r", "lights"):
-            out[tag] = ranged_workload(np, torch, R, Q, RQ, ctx, timed, bits, name, n_spheres, hh, ww, sc, pr, mode, k, args)
+            out[tag] = ranged_workload(np, torch, R, Q, ctx, timed, bits, name, n_spheres, hh, ww, sc, pr, mode, k, args)
             pr.free(); sc.free()
             continue
         if mode in ("camera", "shadow", "depth"):

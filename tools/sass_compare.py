@@ -4,11 +4,12 @@
     python tools/sass_compare.py OLD.so NEW.so
 
 cuobjdump -sass of both files, split into functions, names demangled.  A function of OLD must exist in NEW with the
-same instructions and encodings.  The warp-queue kernel's instantiations are matched by one canonical key, (K, spread,
-packet, all-nodes, spheres, query kind, ranged, accum, views), parsed from every form its template has had: five
-parameters (pixel frames only), six (kRays), seven (kAnyHit), eight (kMultiHit), the query-kind enum (Query), the enum
-followed by kRanged (per-ray intervals), by kRanged and kAccum (progressive rendering) and by kRanged, kAccum and kViews
-(several views in one launch); a parameter a form does not have is false.  So OLD and NEW may be builds of any of them.  Functions that exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
+same instructions and encodings.  The warp-queue kernel's instantiations are matched by one key, (K, spread, packet,
+all-nodes, spheres, kind, ranged), parsed from every form its template has had: <K, kSpread, kPacket, kAllNodes, kSpheres>
+followed by nothing (pixels), by kRays[, kAnyHit[, kMultiHit]], or by the Query enum (Query)N[, kRanged[, kAccum[,
+kViews]]]; a parameter a form does not have is false.  The tile probe is matched by its kind: tile_probe_kernel and
+tile_probe_views_kernel, or tile_probe_kernel<(Query)N>.  So OLD and NEW may be builds of any of them.  Functions that
+exist in NEW only are listed.  Exit code 0 = every function of OLD is identical.
 """
 import collections
 import re
@@ -43,28 +44,31 @@ def functions(path):
 
 
 WARPQUEUE = re.compile(r"render_warpqueue_kernel<([^<>]*)>\(")
-KINDS = ("pixels", "closest", "any-hit", "multi-hit")   # the values of the Query enum, in order
+PROBE = re.compile(r"tile_probe(_views)?_kernel(?:<\(.*Query\)(\d+)>)?\(")
+KINDS = ("pixels", "closest", "any-hit", "multi-hit", "accumulate", "views")   # the values of the Query enum, in order
 
 
 def canonical(name):
-    """The key of a warp-queue instantiation, whatever the form of its template; other names as they are."""
+    """The key of a warp-queue instantiation or tile probe, whatever the form of its template; other names as they are."""
+    m = PROBE.search(name)
+    if m:
+        return f"tile_probe_kernel[{'views' if m.group(1) else KINDS[int(m.group(2) or 0)]}]"
     m = WARPQUEUE.search(name)
     if not m:
         return name
     args = [a.strip() for a in m.group(1).split(",")]
     k, (spread, packet, all_nodes, spheres), rest = args[0], args[1:5], args[5:]
     enum = re.fullmatch(r"\(.*Query\)(\d+)", rest[0]) if rest else None
-    ranged = accum = views = False
-    if enum:   # <K, kSpread, kPacket, kAllNodes, kSpheres, (Query)N[, kRanged[, kAccum[, kViews]]]>
-        kind = KINDS[int(enum.group(1))]
-        ranged = len(rest) > 1 and rest[1] == "true"
-        accum = len(rest) > 2 and rest[2] == "true"
-        views = len(rest) > 3 and rest[3] == "true"
-    else:      # <K, kSpread, kPacket, kAllNodes, kSpheres[, kRays[, kAnyHit[, kMultiHit]]]>, false when absent
+    ranged = False
+    if enum:   # (Query)N[, kRanged[, kAccum[, kViews]]]
+        flags = [a == "true" for a in rest[1:]] + [False] * (4 - len(rest))
+        ranged = flags[0]
+        kind = KINDS[5 if flags[2] else 4 if flags[1] else int(enum.group(1))]
+    else:      # [kRays[, kAnyHit[, kMultiHit]]]
         rays, any_hit, multi_hit = [a == "true" for a in rest] + [False] * (3 - len(rest))
         kind = KINDS[0 if not rays else 2 if any_hit else 3 if multi_hit else 1]
     return (f"render_warpqueue_kernel[K={k}, spread={spread}, packet={packet}, all_nodes={all_nodes}, spheres={spheres}, "
-            f"query={kind}{', ranged' if ranged else ''}{', accum' if accum else ''}{', views' if views else ''}]")
+            f"query={kind}{', ranged' if ranged else ''}]")
 
 
 def main():
