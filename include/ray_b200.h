@@ -75,6 +75,39 @@ int64_t ray_b200_context_launch_count(struct futhark_context *ctx);
  * the first CTA started (exit_us may be NULL to query *count = SMs x warps per CTA).  Syncs the stream. */
 int ray_b200_context_trace_warps(struct futhark_context *ctx, int32_t enable);
 int ray_b200_context_warp_trace(struct futhark_context *ctx, float *exit_us, int64_t capacity, int64_t *count);
+/* What a launch traces (struct ray_b200_plan's query): a frame, a chunk of a progressive frame, several views, or the
+ * caller's rays to their closest hit or along their path (trace_hits / trace_paths), to their first hit (occlusion), or
+ * to their k nearest hits (multi-hit). */
+enum ray_b200_query {
+  RAY_B200_QUERY_PIXELS = 0, RAY_B200_QUERY_CLOSEST = 1, RAY_B200_QUERY_ANYHIT = 2, RAY_B200_QUERY_MULTIHIT = 3,
+  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5
+};
+/* The plan of the last render kernel launch on the context: the last frame, progressive chunk, views call or ray query
+ * (for ray_b200_render_batch, its last job), as it was launched.  Calls that launch no render kernel (a query of n = 0
+ * rays or of max_depth 0, ray_b200_count_work, the helper devices of a RAY_GPUS > 1 context) leave it unchanged; before
+ * the first launch it is all zeros (kernel 0).  For a kernel other than the warp-queue kernel only kernel, query and the
+ * staging fields are set.  It shows which of the warp-queue kernel's instantiations ran: the test-suite checks that
+ * every one of them is reached and exact.  Host-only, does not synchronise. */
+struct ray_b200_plan {
+  int32_t kernel;        /* enum ray_b200_kernel of the launched kernel; 0 = nothing launched yet */
+  int32_t query;         /* enum ray_b200_query */
+  int32_t ranged;        /* 1: the rays carried their own intervals (the *_ranged queries) */
+  int32_t k;             /* rays in flight per warp / 32 (1 or 2) */
+  int32_t warps, ctas;   /* warps per CTA, CTAs launched (at most one per SM) */
+  int32_t spread;        /* 1: the samples of a pixel were spread over a warp's slots (a finished-sample buffer was used) */
+  int32_t packet;        /* packet-walk threshold (lanes per node step); 0 = no packet walk */
+  int32_t all_nodes;     /* 1: every BVH node was staged in shared memory */
+  int32_t spheres;       /* 1: every sphere record was staged as well */
+  int32_t ncap, nlow;    /* node-queue allocation (entries); breadth-first node batches below nlow queued items */
+  int32_t smem_nodes;    /* BVH nodes staged in shared memory (a BFS prefix) */
+  int32_t smem_spheres;  /* sphere records staged (0 or n_leaves) */
+  int32_t n_inner, n_leaves;
+  int64_t stage_budget;  /* shared memory (bytes) the kernel's queues left for staging, before the stage_cap tuning cap */
+  int64_t dynamic_smem;  /* dynamic shared memory requested per CTA (bytes) */
+};
+int ray_b200_context_last_plan(struct futhark_context *ctx, struct ray_b200_plan *out);
+/* sizeof(struct ray_b200_plan) as the library was compiled (80). */
+int64_t ray_b200_plan_size(void);
 
 /* ---- scenes ------------------------------------------------------------------------------------ */
 /* spheres: n x 7 floats (pos.xyz, colour.xyz, radius) — the `sphere` record of ray.fut:22-24;

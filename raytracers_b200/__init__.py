@@ -20,7 +20,7 @@ import os
 
 import numpy as np
 
-__all__ = ["Context", "RayError", "Hit", "Ray", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
+__all__ = ["Context", "RayError", "Hit", "Ray", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
            "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -53,6 +53,19 @@ class WorkCounters(C.Structure):
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+class Plan(C.Structure):
+    """struct ray_b200_plan (include/ray_b200.h): the plan of the last render kernel launch on a context, 80 bytes."""
+    _fields_ = [("kernel", C.c_int32), ("query", C.c_int32), ("ranged", C.c_int32), ("k", C.c_int32), ("warps", C.c_int32),
+                ("ctas", C.c_int32), ("spread", C.c_int32), ("packet", C.c_int32), ("all_nodes", C.c_int32),
+                ("spheres", C.c_int32), ("ncap", C.c_int32), ("nlow", C.c_int32), ("smem_nodes", C.c_int32),
+                ("smem_spheres", C.c_int32), ("n_inner", C.c_int32), ("n_leaves", C.c_int32), ("stage_budget", C.c_int64),
+                ("dynamic_smem", C.c_int64)]
+
+
+# enum ray_b200_query: what a launch traces (Plan.query)
+QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views")
 
 
 class RenderJob(C.Structure):
@@ -137,6 +150,8 @@ def load_library(variant=""):
         "ray_b200_context_trace_warps": (C.c_int, [vp, C.c_int32]),
         "ray_b200_context_warp_trace": (C.c_int, [vp, C.POINTER(C.c_float), C.c_int64, C.POINTER(C.c_int64)]),
         "ray_b200_context_launch_count": (i64, [vp]),
+        "ray_b200_context_last_plan": (C.c_int, [vp, C.POINTER(Plan)]),
+        "ray_b200_plan_size": (i64, []),
         "ray_b200_scene_from_arrays": (C.c_int, [vp, pp, vp, i64, vp]),
         "ray_b200_scene_random": (C.c_int, [vp, pp, i64, u64]),
         "ray_b200_scene_num_spheres": (i64, [vp, vp]),
@@ -560,6 +575,15 @@ class Context:
 
     def launch_count(self):
         return int(self.lib.ray_b200_context_launch_count(self.handle))
+
+    def last_plan(self):
+        """The plan of the last render kernel launch on this context (ray_b200_context_last_plan) as a dict of the fields
+        of struct ray_b200_plan, with query as its name in QUERIES.  Host-only: call it after the launch's call returns."""
+        p = Plan()
+        self._check(self.lib.ray_b200_context_last_plan(self.handle, C.byref(p)))
+        out = {k: int(getattr(p, k)) for k, _ in Plan._fields_}
+        out["query"] = QUERIES[out["query"]]
+        return out
 
     def render_into(self, out_pix_dev, h, w, prepared, spp=1, out_rgb_dev=None):
         self._check(self.lib.ray_b200_render_into(self.handle, _ptr(out_pix_dev), _ptr(out_rgb_dev), int(h), int(w), int(spp), prepared.handle))

@@ -63,7 +63,8 @@ struct futhark_context {
   struct OffsetTable { int32_t spp; float *dev; };
   std::vector<OffsetTable> offset_tables;   // per-spp cache (ensure_offsets)
   int64_t launches = 0;
-  WavefrontBuffers wf;                      // ray queues of the wavefront kernel (grown on demand)
+  ray_b200_plan last_plan{};                // plan of the last render kernel launch (ray_b200_context_last_plan)
+  WavefrontBuffers wf;                     // ray queues of the wavefront kernel (grown on demand)
   struct PinnedBlock { unsigned char *ptr; size_t bytes; cudaEvent_t last_use; };
   std::vector<PinnedBlock> pinned_cache;    // page-locked upload buffers of freed prepared scenes, reused by the next prepare_scene
   BvhBuildResult *d_build_result = nullptr, *h_build_result = nullptr;  // device scratch / page-locked host mirror
@@ -192,6 +193,9 @@ struct FrameFlags {
 int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id = 0, bool timed = true,
               const FrameFlags *ff = nullptr, const futhark_opaque_prepared_scene *scene = nullptr,
               Query kind = Query::kPixels, const RayQuery *q = nullptr);
+// Records a launch (P and lc as launched, kind / ranged / q as given to launch_render or launch_warpqueue) as the
+// context's last plan; the warp-queue kernel's fields come from wq_variant, which its launcher uses too.
+void record_plan(futhark_context *ctx, const RenderParams &P, const LaunchConfig &lc, Query kind, bool ranged, const RayQuery &q);
 // api_multigpu.cu: the single-process multi-GPU mode (RAY_GPUS > 1) of futhark_entry_render
 int create_helper_contexts(futhark_context *ctx, const futhark_context_config *cfg, int ndev);
 int render_multi_device(futhark_context *ctx, futhark_i32_2d *img, int64_t h, int64_t w, int32_t spp, const futhark_opaque_prepared_scene *p);

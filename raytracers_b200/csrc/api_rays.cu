@@ -55,6 +55,7 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t 
     CUDA_TRY(ctx, cudaMemsetAsync(L.work_cursor, 0, 2 * sizeof(int32_t), L.stream));
     CUDA_TRY(ctx, launch_warpqueue(P, kind, ranged, Q, lc, L.stream, &ctx->launches));
     CUDA_TRY(ctx, cudaGetLastError());
+    record_plan(ctx, P, lc, kind, ranged, Q);
   }
   // this query reads the scene's device memory until here on lane 0 (release_scene_block waits for it)
   if (!p->last_use[0]) CUDA_TRY(ctx, cudaEventCreateWithFlags(&p->last_use[0], cudaEventDisableTiming));

@@ -66,7 +66,32 @@ static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
   lc.lw_idle_min = ctx->cfg.lw_idle_min;
   lc.lw_passes = ctx->cfg.lw_passes;
   lc.max_dynamic_smem = ctx->max_smem_optin;
+  lc.stage_budget = 0;
   return lc;
+}
+
+static_assert((int)Query::kPixels == RAY_B200_QUERY_PIXELS && (int)Query::kClosest == RAY_B200_QUERY_CLOSEST &&
+                  (int)Query::kAnyHit == RAY_B200_QUERY_ANYHIT && (int)Query::kMultiHit == RAY_B200_QUERY_MULTIHIT &&
+                  (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS,
+              "enum ray_b200_query names the values of Query");
+static_assert(sizeof(struct ray_b200_plan) == 80, "struct ray_b200_plan is 16 int32 and 2 int64");
+
+void record_plan(futhark_context *ctx, const RenderParams &P, const LaunchConfig &lc, Query kind, bool ranged, const RayQuery &q) {
+  ray_b200_plan &r = ctx->last_plan;
+  memset(&r, 0, sizeof r);
+  r.kernel = lc.kernel;
+  r.query = (int32_t)kind;
+  r.ranged = ranged ? 1 : 0;
+  r.smem_nodes = P.smem_nodes; r.smem_spheres = P.smem_spheres;
+  r.n_inner = P.n_inner; r.n_leaves = P.n_leaves;
+  r.stage_budget = lc.stage_budget;
+  if (lc.kernel != RAY_B200_KERNEL_WARPQUEUE) return;
+  const WqVariant v = wq_variant(P, kind, q, lc);
+  r.k = v.k; r.warps = lc.wq_warps; r.ctas = (int32_t)v.ctas;
+  r.spread = v.spread; r.packet = v.packet ? lc.wq_packet : 0;
+  r.all_nodes = v.all_nodes; r.spheres = v.spheres;
+  r.ncap = v.ncap; r.nlow = v.nlow;
+  r.dynamic_smem = (int64_t)v.smem;
 }
 
 // Fills the kernel parameter block for one frame, and the frame's launch plan.  Query::kAccumulate: the launch is one
@@ -177,7 +202,10 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
     budget = (int64_t)ctx->max_smem_optin - w * (int64_t)lw_warp_bytes((int)r, scap) - 512;
     lc.wq_warps = (int32_t)w;
     lc.lw_slots = (int32_t)r;
+    lc.stage_budget = budget;
     budget = cap_staging(ctx, p, budget);
+  } else {
+    lc.stage_budget = budget;
   }
   split_staging(p, budget, P.smem_nodes, P.smem_spheres);
   return 0;
@@ -261,6 +289,7 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
     lc.wq_warps = (int32_t)wq_w;
     lc.wq_k = k;
     lc.wq_ncap = ncap_cfg;
+    lc.stage_budget = budget;
     split_staging(p, cap_staging(ctx, p, budget), P.smem_nodes, P.smem_spheres);
     // belt and braces: the K = 2 plan is only worth anything when the scene is staged whole (a scene that just misses
     // fetches its lower nodes from L2 with half the warps); if anything above left it short, plan again with K = 1
@@ -447,6 +476,7 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
       return 1;
     }
     CUDA_TRY(ctx, le);
+    record_plan(ctx, P, lc, kind, false, pq);
   }
   if (record_order) {  // after the recording frame (outside its timing events' kernel, inside the stream order): cost -> order
     launch_tile_order_from_cost(P, scene->order_cache.cost, ctx->cfg.long_path == 0 ? 4 : ctx->cfg.long_path, L.tile_order_plan, L.stream, &ctx->launches);
@@ -698,6 +728,15 @@ int ray_b200_render_batch(struct futhark_context *ctx, const struct ray_b200_ren
 }
 
 int64_t ray_b200_render_job_size(void) { return (int64_t)sizeof(struct ray_b200_render_job); }
+
+int ray_b200_context_last_plan(struct futhark_context *ctx, struct ray_b200_plan *out) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!out) { set_error(ctx, "context_last_plan: null output"); return 1; }
+  *out = ctx->last_plan;
+  return 0;
+}
+int64_t ray_b200_plan_size(void) { return (int64_t)sizeof(struct ray_b200_plan); }
 
 int ray_b200_context_set_pipeline(struct futhark_context *ctx, int32_t on) {
   if (bad_ctx(ctx)) return 1;

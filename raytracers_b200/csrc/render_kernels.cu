@@ -962,23 +962,15 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
 // that kind: the same kernel in ray mode, without spread samples or packets; `ranged`: its rays carry their own intervals.
 cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, const RayQuery &q, const LaunchConfig &lc,
                              cudaStream_t stream, int64_t *launches) {
-  const bool rays = is_ray_query(kind);
-  const bool spread = !rays && p.sample_buf != nullptr, packet = !rays && lc.wq_packet > 0;
-  // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
-  // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
-  const long long work = rays ? (long long)q.n : p.local_tiles * kTilePixels * (spread ? (long long)p.spp : 1ll);
-  if (work <= 0) return cudaSuccess;
-  const bool all_nodes = p.smem_nodes == p.n_inner, sph = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
-  const int k = lc.wq_k == 1 ? 1 : 2;
+  // the template flags and launch geometry (render_params.h): breadth-first below nlow queued node items (0 = half the
+  // ring, < 0 = never: plain LIFO), no more CTAs than there are rays to start at once
+  const WqVariant v = wq_variant(p, kind, q, lc);
+  if (v.ctas <= 0) return cudaSuccess;
+  const bool spread = v.spread, packet = v.packet, all_nodes = v.all_nodes, sph = v.spheres;
+  const int k = v.k, ncap = v.ncap, nlow = v.nlow;
   const int wthreads = 32 * lc.wq_warps;
-  const int ncap = wq_node_capacity(k, p.max_depth, lc.wq_ncap);
-  // breadth-first below this many queued node items (0 = half the ring, < 0 = never: plain LIFO)
-  const int nring = 1 << (31 - __builtin_clz((unsigned)ncap));
-  const int nlow = lc.wq_low < 0 ? 0 : (lc.wq_low == 0 ? nring / 2 : (lc.wq_low > nring - 96 ? nring - 96 : lc.wq_low));
-  const size_t wsmem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * wq_warp_bytes(k, ncap, packet, spread);
-  long long ctas = lc.sm_count;
-  const long long useful = (work + 32 * k * lc.wq_warps - 1) / (32 * k * lc.wq_warps);
-  if (ctas > useful) ctas = useful;
+  const size_t wsmem = v.smem;
+  const long long ctas = v.ctas;
   const cudaError_t e = with_query([&](auto query) {
     if constexpr (is_ray_query(query))
       return with_flags([&](auto k2, auto a, auto s, auto rg) {

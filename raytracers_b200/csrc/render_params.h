@@ -136,6 +136,7 @@ struct LaunchConfig {
   int lw_idle_min;     // lane-walk kernel: with the ready list empty, shade as soon as this many lanes have nothing to walk
   int lw_passes;       // lane-walk kernel: refill passes per shading phase
   int max_dynamic_smem;  // the device's opt-in shared-memory limit (kernels opt in on first launch)
+  long long stage_budget;  // warp-queue kernel: shared memory its queues leave for staging, before cap_staging (bytes)
 };
 
 // A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate and kViews, which read q,
@@ -213,6 +214,37 @@ __host__ __device__ inline size_t wq_warp_bytes(int k, int ncap, bool packet, bo
   const size_t r = 32 * (size_t)k;
   return ((r * (16 * 4 + (spread ? 4 : 16) + 8 + 4) + 2 * kWqRing * 4 + (packet ? 2 * kWqPacketStack * 4 : 0) + kWqLeafStack * 4 + (size_t)ncap * 4) + 127) & ~(size_t)127;
 }
+// The warp-queue kernel's launch of kind `kind` (`ranged`: per-ray intervals) with parameter block p and plan lc: the
+// template flags it instantiates and its launch geometry.  launch_warpqueue launches exactly this, and the context's
+// launch report (ray_b200_context_last_plan) is made from it.  ctas == 0: there is no work, nothing is launched.
+struct WqVariant {
+  int k;                     // rays in flight per warp / 32
+  bool spread, packet;       // samples spread over a warp's slots (a finished-sample buffer is set); packet walk
+  bool all_nodes, spheres;   // every node staged; every sphere record staged as well
+  int ncap, nlow;            // node-queue allocation; breadth-first below nlow queued items
+  size_t smem;               // dynamic shared memory of a CTA
+  long long ctas;
+};
+inline WqVariant wq_variant(const RenderParams &p, Query kind, const RayQuery &q, const LaunchConfig &lc) {
+  WqVariant v;
+  const bool rays = is_ray_query(kind);
+  v.spread = !rays && p.sample_buf != nullptr;
+  v.packet = !rays && lc.wq_packet > 0;
+  v.all_nodes = p.smem_nodes == p.n_inner;
+  v.spheres = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
+  v.k = lc.wq_k == 1 ? 1 : 2;
+  v.ncap = wq_node_capacity(v.k, p.max_depth, lc.wq_ncap);
+  const int nring = 1 << (31 - __builtin_clz((unsigned)v.ncap));
+  v.nlow = lc.wq_low < 0 ? 0 : (lc.wq_low == 0 ? nring / 2 : (lc.wq_low > nring - 96 ? nring - 96 : lc.wq_low));
+  v.smem = ((staging_bytes(p) + 127) & ~(size_t)127) + (size_t)lc.wq_warps * wq_warp_bytes(v.k, v.ncap, v.packet, v.spread);
+  // no more CTAs than there are rays to start at once: a slot takes one query ray, one SAMPLE when samples are spread, one
+  // pixel otherwise (capping by pixels alone left 26 SMs idle on a 125 K-pixel shard at 64 spp with 32 warps per CTA)
+  const long long work = rays ? (long long)q.n : p.local_tiles * kTilePixels * (v.spread ? (long long)p.spp : 1ll);
+  const long long useful = work <= 0 ? 0 : (work + 32 * v.k * lc.wq_warps - 1) / (32 * v.k * lc.wq_warps);
+  v.ctas = lc.sm_count < useful ? lc.sm_count : useful;
+  return v;
+}
+
 // stream-queue kernel (K4): per-warp bytes (5 float4 + best + item + pending per slot, done/free lists, ring, stacks)
 __host__ __device__ inline size_t sq_warp_bytes(int k, int ncap) {
   const size_t r = 32 * (size_t)k;

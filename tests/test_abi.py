@@ -48,6 +48,16 @@ def test_struct_layouts_match_the_library(R):
     """ctypes mirrors of the C structs have the size the library was compiled with (no GPU needed)."""
     lib = R.load_library()
     assert ctypes.sizeof(R.RenderJob) == lib.ray_b200_render_job_size() == 72
+    assert ctypes.sizeof(R.Plan) == lib.ray_b200_plan_size() == 80
+    assert {"ray_b200_context_last_plan", "ray_b200_plan_size"} <= set(R.declared_symbols())
+
+
+def test_plan_query_names_match_the_header(R):
+    """Context.last_plan() names the query kinds in the order of enum ray_b200_query."""
+    text = open(os.path.join(ROOT, "include", "ray_b200.h")).read()
+    enum = re.search(r"enum ray_b200_query \{(.*?)\}", text, flags=re.S).group(1)
+    values = {name.lower(): int(v) for name, v in re.findall(r"RAY_B200_QUERY_(\w+) = (\d+)", enum)}
+    assert values == {name: i for i, name in enumerate(R.QUERIES)}
 
 
 def test_tuning_parameters_match_the_documented_environment_variables(R):

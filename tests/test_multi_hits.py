@@ -183,7 +183,6 @@ def test_random_rays_on_the_million_sphere_scene(R):
     torch = _torch()
     ctx, sc, pr = _gpu_case(R, "random", 2000, 2000, n=1000000)
     with ctx:
-        assert pr.info()["smem_nodes"] < pr.info()["n_inner"]
         rays = random_rays(sc.arrays()[0], 65536, seed=47)
         d = _dev(rays)
         k = 4
@@ -192,6 +191,8 @@ def test_random_rays_on_the_million_sphere_scene(R):
         torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
         ctx.trace_multi_hits_into(d.data_ptr(), rays.shape[0], pr, k, hits.data_ptr(), counts.data_ptr(), t_min=0.1)
         ctx.sync()
+        plan = ctx.last_plan()
+        assert plan["query"] == "multihit" and plan["smem_nodes"] < plan["n_inner"] and not plan["all_nodes"], plan
         sub = slice(0, None, 16)
         want = Q.prepare("random", 2000, 2000, n=1000000).trace_multi_hits(rays[sub], k, 0.1, 1e9)
         assert_equal((_np(hits)[sub], _np(counts)[sub]), want, "1M")

@@ -118,13 +118,14 @@ def test_random_rays_on_the_million_sphere_scene(R):
     torch = _torch()
     ctx, sc, pr = _gpu_case(R, "random", 2000, 2000, n=1000000)
     with ctx:
-        assert pr.info()["smem_nodes"] < pr.info()["n_inner"]
         rays = random_rays(sc.arrays()[0], 65536, seed=29)
         d = _dev(rays)
         out = torch.empty((rays.shape[0],), dtype=torch.bool, device="cuda")
         torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
         ctx.trace_occluded_into(d.data_ptr(), rays.shape[0], pr, out.data_ptr(), t_min=0.1)
         ctx.sync()
+        plan = ctx.last_plan()
+        assert plan["query"] == "anyhit" and plan["smem_nodes"] < plan["n_inner"] and not plan["all_nodes"], plan
         sub = slice(0, None, 16)
         o = Q.prepare("random", 2000, 2000, n=1000000)
         want = o.trace_occluded(rays[sub], 0.1, 1e9)

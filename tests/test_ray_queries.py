@@ -173,13 +173,15 @@ def test_random_rays_on_the_million_sphere_scene(R):
     torch = _torch()
     ctx, sc, pr = _gpu_case(R, "random", 2000, 2000, n=1000000)
     with ctx:
-        assert pr.info()["smem_nodes"] < pr.info()["n_inner"]
         rays = random_rays(sc.arrays()[0], 65536, seed=11)
         d = _dev(rays)
         hits = torch.empty((rays.shape[0], 8), dtype=torch.float32, device="cuda")
         torch.cuda.synchronize()   # the context's own stream is not ordered after torch's
         ctx.trace_hits_into(d.data_ptr(), rays.shape[0], pr, hits.data_ptr())
+        plan = ctx.last_plan()
+        assert plan["query"] == "closest" and plan["smem_nodes"] < plan["n_inner"] and not plan["all_nodes"], plan
         rgb, seg = ctx.trace_paths(pr, d)
+        assert ctx.last_plan()["smem_nodes"] < plan["n_inner"]
         sub = slice(0, None, 16)
         o = _oracle_for("random", 2000, 2000, n=1000000)
         assert hits_differ(hits.cpu().numpy()[sub], o.trace_hits(rays[sub])) == 0

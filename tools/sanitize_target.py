@@ -52,6 +52,20 @@ def main():
         wnt, _, _ = O.render_scene("random", hh, ww, n=n, seed=3)
         pr = ctx.prepare_scene(hh, ww, ctx.scene_random(n, 3))
         bad += check(ctx.render_host(hh, ww, pr), wnt, "warpqueue deep tree")
+    # every node staged with the spheres read from global memory, and a whole scene of more than 2048 sphere records
+    # (the staging copy's second 32 KB piece of them) behind 3 warps' queues
+    for n, tuning, want_staged in ((600, dict(stage_cap=64 * 599), (599, 0)), (2600, dict(wq_warps=3), (2599, 2600))):
+        hh, ww = 32, 48
+        with R.Context(kernel="warpqueue", **tuning) as ctx:
+            pr = ctx.prepare_scene(hh, ww, ctx.scene_random(n, 5))
+            for s in (1, 3):
+                wnt, _, _ = O.render_scene("random", hh, ww, spp=s, n=n, seed=5)
+                bad += check(ctx.render_host(hh, ww, pr, spp=s), wnt, f"warpqueue {tuning} n={n} spp={s}")
+                plan = ctx.last_plan()
+                staged = (plan["smem_nodes"], plan["smem_spheres"])
+                if staged != want_staged:
+                    print(f"warpqueue {tuning} n={n} spp={s}: staged {staged}, expected {want_staged}", flush=True)
+                    bad += 1
     print("SANITIZE_TARGET", "OK" if bad == 0 else f"FAILED ({bad})", flush=True)
     return 1 if bad else 0
 
