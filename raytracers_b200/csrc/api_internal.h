@@ -89,6 +89,8 @@ struct futhark_context {
     size_t tile_order_bytes = 0;
     TileOrderBuffers tile_order_plan{};
   } lanes[2];
+  // lane `id` for a launch: lane 0 follows the context's stream, which ray_b200_context_set_stream may have changed
+  Lane &lane(int id) { if (id == 0) lanes[0].stream = stream; return lanes[id]; }
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool pipeline = false;                // ray_b200_context_set_pipeline: batches do not join lane 1 back
   uint32_t lane_seq = 0;                // pipelined submission: frames alternate lanes across calls
@@ -115,7 +117,7 @@ struct futhark_opaque_prepared_scene {
   size_t pinned_bytes = 0;
   cudaEvent_t pinned_event = nullptr;  // completion of the last H2D copy that read `pinned`
   bool host_built = false;
-  // last render that read this scene's device memory, per lane (recorded by do_render): the memory is freed / replaced
+  // last render that read this scene's device memory, per lane (record_scene_use): the memory is freed / replaced
   // only after both (release_scene_block)
   mutable cudaEvent_t last_use[2] = {nullptr, nullptr};
   mutable bool used[2] = {false, false};
@@ -167,14 +169,22 @@ inline int64_t tiles_of_rank(int64_t h, int64_t w, int32_t rank, int32_t world) 
 
 // api_render.cu
 int resolve_kernel(const futhark_context *ctx);
-// The parameter block of one frame and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
-// slots, ...), which the caller hands to do_render.  `kind` is a pixel kind; q is read for the other two.
-// Query::kAccumulate (ray_b200_render_accumulate): the frame's samples [q->s_begin, q->s_begin + spp) on the warp-queue
-// kernel, scaled by 1/(s_begin + spp).  Query::kViews (ray_b200_render_views_into; rank 0 of 1): q->n_views frames of
-// h x w, planned as one frame of all their tiles, on the warp-queue kernel; q->view_tiles is set here.
-int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
-                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc,
-                Query kind = Query::kPixels, RayQuery *q = nullptr);
+// One pixel launch as its caller describes it: every entry point that renders fills one Frame, and fill_params and
+// do_render read everything about the launch from it.
+struct Frame {
+  const futhark_opaque_prepared_scene *scene = nullptr;
+  int64_t h = 0, w = 0;
+  int32_t spp = 1;             // the samples of this launch (kAccumulate: of this chunk)
+  int32_t rank = 0, world = 1;
+  int32_t *out_pix = nullptr;
+  float *out_rgb = nullptr;
+  bool tile_major = false;     // out_pix holds this rank's tiles, padded to ray_b200_shard_tiles_padded (do_render zeroes the tail)
+  Query kind = Query::kPixels; // a pixel kind: kAccumulate (ray_b200_render_accumulate), kViews (ray_b200_render_views_into)
+  RayQuery q{};                // kAccumulate: accum, s_begin.  kViews: n_views, and cams once uploaded (view_tiles: fill_params)
+};
+// The parameter block of frame f and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
+// slots, ...), which the caller hands to do_render with f; sets f.q.view_tiles of a kViews frame.
+int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc);
 void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P);  // zeroes P, then its scene half
 // The warp-queue kernel's plan for one launch (pixel frames and ray queries): rays in flight per warp (32 k), warps per
 // CTA, node-queue cap and packet threshold in lc, how much of the scene is staged in shared memory in P.
@@ -190,9 +200,13 @@ struct FrameFlags {
   uint32_t wait_value = 0;
   uint32_t *done_flag = nullptr;
 };
-int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id = 0, bool timed = true,
-              const FrameFlags *ff = nullptr, const futhark_opaque_prepared_scene *scene = nullptr,
-              Query kind = Query::kPixels, const RayQuery *q = nullptr);
+// Enqueues frame f, planned by fill_params into P and lc, on lane `lane` (0 = the context's stream).  `timed`: bracket
+// the launch with the context's timing events.  `ff`: the frame's peer-frame protocol.
+int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const LaunchConfig &lc, int lane = 0, bool timed = true, const FrameFlags *ff = nullptr);
+// fill_params, then do_render: a frame planned and launched with nothing in between
+int render_frame(futhark_context *ctx, Frame &f, int lane = 0, bool timed = true, const FrameFlags *ff = nullptr);
+// The launches enqueued so far on lane `lane` read p's device memory (release_scene_block waits for them)
+int record_scene_use(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int lane);
 // Records a launch (P and lc as launched, kind / ranged / q as given to launch_render or launch_warpqueue) as the
 // context's last plan; the warp-queue kernel's fields come from wq_variant, which its launcher uses too.
 void record_plan(futhark_context *ctx, const RenderParams &P, const LaunchConfig &lc, Query kind, bool ranged, const RayQuery &q);

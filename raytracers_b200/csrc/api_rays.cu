@@ -38,8 +38,7 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t 
   if (!p || !p->dev.nodes || !p->dev.perm) { set_error(ctx, "%s: invalid prepared scene", what); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "%s: BVH depth %d exceeds the traversal stack", what, p->max_depth); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-  futhark_context::Lane &L = ctx->lanes[0];
-  L.stream = ctx->stream;
+  futhark_context::Lane &L = ctx->lane(0);
   CUDA_TRY(ctx, cudaEventRecord(ctx->ev_start, L.stream));
   if (Q.max_depth == 0) {  // a path query whose ray_colour loop does not run: colour 0, no objs_hit call
     CUDA_TRY(ctx, cudaMemsetAsync(Q.rgb, 0, (size_t)n * 3 * sizeof(float), L.stream));
@@ -57,10 +56,7 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t 
     CUDA_TRY(ctx, cudaGetLastError());
     record_plan(ctx, P, lc, kind, ranged, Q);
   }
-  // this query reads the scene's device memory until here on lane 0 (release_scene_block waits for it)
-  if (!p->last_use[0]) CUDA_TRY(ctx, cudaEventCreateWithFlags(&p->last_use[0], cudaEventDisableTiming));
-  CUDA_TRY(ctx, cudaEventRecord(p->last_use[0], L.stream));
-  p->used[0] = true;
+  if (record_scene_use(ctx, p, 0)) return 1;
   CUDA_TRY(ctx, cudaEventRecord(ctx->ev_stop, L.stream));
   ctx->have_timing = true;
   return 0;

@@ -94,31 +94,40 @@ void record_plan(futhark_context *ctx, const RenderParams &P, const LaunchConfig
   r.dynamic_smem = (int64_t)v.smem;
 }
 
-// Fills the kernel parameter block for one frame, and the frame's launch plan.  Query::kAccumulate: the launch is one
-// chunk of a progressive frame: spp samples from q->s_begin on, planned as a frame of spp samples (spread or pixel-bound
+// Bytes of the finished-sample buffer of `spp` spread samples on `warps` warps per CTA (one CTA per SM); 0 when samples
+// are not spread: one sample, more than 65535, spreading switched off, or a buffer over kSpreadBudget.  Planning asks for
+// kWqMaxWarps, which bounds every plan (the warps it picks depend on whether samples are spread); do_render, for lc's.
+static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
+  if (spp <= 1 || spp > 65535 || !ctx->cfg.wq_spread) return 0;
+  const size_t need = (size_t)ctx->sm_count * warps * kWqRing * (size_t)spp * sizeof(float4);
+  return need <= kSpreadBudget ? need : 0;
+}
+
+// Fills the kernel parameter block for frame f, and the frame's launch plan.  Query::kAccumulate: the launch is one
+// chunk of a progressive frame: spp samples from q.s_begin on, planned as a frame of spp samples (spread or pixel-bound
 // by the chunk length), read from the offset table of the whole frame at the chunk's first sample and scaled by
 // 1/s_end; it runs on the warp-queue kernel whatever the context's kernel is.  Query::kViews: the launch renders
-// q->n_views frames of h x w: its work items are the tiles of all of them, so the plan (spread or pixel-bound, K,
+// q.n_views frames of h x w: its work items are the tiles of all of them, so the plan (spread or pixel-bound, K,
 // staging, the sample buffer) is that of one frame of n_views x tiles(h, w) tiles; it runs on the warp-queue kernel too.
-int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t h, int64_t w, int32_t spp,
-                int32_t rank, int32_t world, int32_t *out_pix, float *out_rgb, bool tile_major, RenderParams &P, LaunchConfig &lc,
-                Query kind, RayQuery *q) {
-  const bool views = kind == Query::kViews;
+int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc) {
+  const futhark_opaque_prepared_scene *p = f.scene;
+  const int64_t h = f.h, w = f.w; const int32_t spp = f.spp;
+  const bool views = f.kind == Query::kViews;
   if (!p || !p->dev.nodes) { set_error(ctx, "render: invalid prepared scene"); return 1; }
   if (h <= 0 || w <= 0 || h > 65536 || w > 65536 || ((h + 3) / 4) * ((w + 7) / 8) > ((int64_t)1 << 25)) {
     // work items are 32-bit: at most 2^30 (padded) pixels per frame
     set_error(ctx, "render: bad image size %lldx%lld", (long long)h, (long long)w);
     return 1;
   }
-  if (views && tiles_total(h, w) * q->n_views > ((int64_t)1 << 25)) {
+  if (views && tiles_total(h, w) * f.q.n_views > ((int64_t)1 << 25)) {
     // ... and per launch: at most 2^30 padded pixels over all views
-    set_error(ctx, "render_views: %d views of %lldx%lld exceed 2^30 padded pixels", q->n_views, (long long)h, (long long)w);
+    set_error(ctx, "render_views: %d views of %lldx%lld exceed 2^30 padded pixels", f.q.n_views, (long long)h, (long long)w);
     return 1;
   }
   if (spp < 1) { set_error(ctx, "render: spp must be >= 1"); return 1; }
-  if (world < 1 || rank < 0 || rank >= world) { set_error(ctx, "render: bad shard %d/%d", rank, world); return 1; }
+  if (f.world < 1 || f.rank < 0 || f.rank >= f.world) { set_error(ctx, "render: bad shard %d/%d", f.rank, f.world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
-  const int32_t s_begin = kind == Query::kAccumulate ? q->s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
+  const int32_t s_begin = f.kind == Query::kAccumulate ? f.q.s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
   if (ensure_offsets(ctx, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
@@ -126,14 +135,14 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   memcpy(P.cam, &p->cam, sizeof P.cam);
   P.W = (int32_t)w; P.H = (int32_t)h; P.spp = spp; P.inv_spp = 1.0f / (float)s_end;
   P.offsets = ctx->offsets + 2 * (size_t)s_begin;
-  P.out_pix = out_pix; P.out_rgb = out_rgb; P.tile_major = tile_major ? 1 : 0;
-  P.rank = rank; P.world = world;
+  P.out_pix = f.out_pix; P.out_rgb = f.out_rgb; P.tile_major = f.tile_major ? 1 : 0;
+  P.rank = f.rank; P.world = f.world;
   P.tiles_x = (int32_t)((w + kTileW - 1) / kTileW); P.tiles_y = (int32_t)((h + kTileH - 1) / kTileH);
   P.n_tiles = tiles_total(h, w);
-  P.local_tiles = tiles_of_rank(h, w, rank, world);
+  P.local_tiles = tiles_of_rank(h, w, f.rank, f.world);
   if (views) {  // (the entry point allows no shards)
-    q->view_tiles = (int32_t)P.n_tiles;
-    P.n_tiles = P.local_tiles = P.n_tiles * q->n_views;
+    f.q.view_tiles = (int32_t)P.n_tiles;
+    P.n_tiles = P.local_tiles = P.n_tiles * f.q.n_views;
   }
   P.n_chunks = (int32_t)((P.local_tiles + 63) / 64);
   {  // stride ~ golden ratio * n_chunks, made coprime to n_chunks
@@ -159,13 +168,10 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   // shared-memory staging plan: BFS prefix of the node array, then the sphere records if they all fit.
   // The warp-queue kernel runs one CTA per SM and gives the staging area whatever its queues leave.
   int64_t budget = std::min<int64_t>(ctx->cfg.smem_budget, ctx->max_smem_optin - 1024) - 128;
-  int kern = kind != Query::kPixels ? RAY_B200_KERNEL_WARPQUEUE : resolve_kernel(ctx);
-  if (kern == RAY_B200_KERNEL_LANEWALK && spp > 1) {
-    // K5 traces one sample per slot and needs the finished-sample buffer (0.54 MB per sample on an H100); without it (spreading
-    // switched off, or a sample count whose buffer exceeds the budget) the frame runs on the warp-queue kernel
-    const size_t need = (size_t)ctx->sm_count * kWqMaxWarps * kWqRing * (size_t)spp * sizeof(float4);
-    if (!ctx->cfg.wq_spread || spp > 65535 || need > kSpreadBudget) kern = RAY_B200_KERNEL_WARPQUEUE;
-  }
+  int kern = f.kind != Query::kPixels ? RAY_B200_KERNEL_WARPQUEUE : resolve_kernel(ctx);
+  // K5 traces one sample per slot and needs the finished-sample buffer (0.54 MB per sample on an H100); without it (spreading
+  // switched off, or a sample count whose buffer exceeds the budget) the frame runs on the warp-queue kernel
+  if (kern == RAY_B200_KERNEL_LANEWALK && spp > 1 && !spread_bytes(ctx, kWqMaxWarps, spp)) kern = RAY_B200_KERNEL_WARPQUEUE;
   lc = launch_config(ctx, kern);
   if (kern == RAY_B200_KERNEL_STREAMQUEUE) {
     const int k = 1;
@@ -179,8 +185,7 @@ int fill_params(futhark_context *ctx, const futhark_opaque_prepared_scene *p, in
   if (kern == RAY_B200_KERNEL_WARPQUEUE) {
     // samples will be spread if the finished-sample buffer fits the budget (do_render allocates it; a failed allocation
     // there falls back to pixel-bound samples, whose bigger slots are checked again at launch)
-    const bool will_spread = spp > 1 && spp <= 65535 && ctx->cfg.wq_spread &&
-                             (size_t)ctx->sm_count * kWqMaxWarps * kWqRing * (size_t)spp * sizeof(float4) <= kSpreadBudget;
+    const bool will_spread = spread_bytes(ctx, kWqMaxWarps, spp) != 0;
     // the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame (a warp's tile
     // lies in one view: the density is that of a view, however many there are)
     const bool coherent = spp > 1 || h * w >= ((int64_t)1 << 22);
@@ -375,23 +380,25 @@ static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64
   return 0;
 }
 
-// Enqueues one frame with launch plan `lc` (fill_params) on lane `lane_id` (0 = the context's stream).  `timed`: bracket
-// it with the context's timing events.  `ff`: peer-frame protocol of the frame (api_internal.h).
-// `kind` and `q` as fill_params had them: Query::kAccumulate, a chunk of a progressive frame, is launched without a
-// claim-order pass (see below); Query::kViews, with the camera table q->cams in device memory, without the learned order.
-int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff,
-              const futhark_opaque_prepared_scene *scene, Query kind, const RayQuery *q) {
-  futhark_context::Lane &L = ctx->lanes[lane_id];
-  if (lane_id == 0) L.stream = ctx->stream;
+// One frame on one lane (api_internal.h).  Query::kAccumulate, a chunk of a progressive frame, is launched without a
+// claim-order pass (see below); Query::kViews, with the camera table f.q.cams in device memory, without the learned order.
+int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff) {
+  futhark_context::Lane &L = ctx->lane(lane_id);
+  if (f.tile_major) {  // ranks that own one tile fewer than the padded count leave a zeroed tail (before the timing events)
+    const int64_t padded = ray_b200_shard_tiles_padded(f.h, f.w, f.world);
+    if (P.local_tiles < padded)
+      CUDA_TRY(ctx, cudaMemsetAsync(f.out_pix + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4, L.stream));
+  }
   if (lc.kernel == RAY_B200_KERNEL_WAVEFRONT && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
   P.sample_buf = nullptr;
-  if ((lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_STREAMQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK) && P.spp > 1 && P.spp <= 65535 && ctx->cfg.wq_spread) {
+  const bool slot_kernel = lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_STREAMQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK;
+  const size_t need = slot_kernel ? spread_bytes(ctx, lc.wq_warps, P.spp) : 0;
+  if (need) {
     // samples of a pixel are spread over a warp's slots; finished colours wait here for the in-order sum
     // (0.54 MB per sample on an H100's 132 SMs with 32 warps).  Above a memory budget, or when the allocation fails, the frame falls
     // back to the pixel-bound variant of the same kernel (kSpread = false), which handles any sample count.
-    const size_t need = (size_t)lc.sm_count * lc.wq_warps * kWqRing * (size_t)P.spp * sizeof(float4);
     bool have = need <= L.sample_buf_bytes;
-    if (!have && need <= kSpreadBudget) {
+    if (!have) {
       CUDA_TRY(ctx, cudaStreamSynchronize(L.stream));
       if (L.sample_buf) CUDA_TRY(ctx, cudaFree(L.sample_buf));
       L.sample_buf = nullptr; L.sample_buf_bytes = 0;
@@ -407,7 +414,7 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   // order, and it leaves the scene's learned order as it found it (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = kind != Query::kAccumulate && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = f.kind != Query::kAccumulate && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -422,15 +429,15 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   bool record_order = false;
   // (Frames of more than 2^24 tile-samples do not end on their longest paths any more, and un-mixing cheap and expensive
   // tiles costs them more than the shorter tail saves.)
-  if (!heavy_first && kind == Query::kPixels && scene && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
+  if (!heavy_first && f.kind == Query::kPixels && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
       P.local_tiles < (1ll << 26) && (ctx->cfg.learn_order > 1 || P.local_tiles * (int64_t)P.spp <= ((int64_t)1 << 24))) {
-    auto &oc = scene->order_cache;
+    auto &oc = f.scene->order_cache;
     const bool same = oc.state == 1 && oc.h == P.H && oc.w == P.W && oc.spp == P.spp && oc.rank == P.rank && oc.world == P.world && oc.tiles == P.local_tiles;
     if (same) {
       CUDA_TRY(ctx, cudaStreamWaitEvent(L.stream, oc.ready, 0));   // the sort may have run on the other lane
       P.tile_order = oc.order;
     } else if (oc.state == 1 && ctx->lanes[1].stream &&
-               ((scene->used[0] && cudaEventQuery(scene->last_use[0]) != cudaSuccess) || (scene->used[1] && cudaEventQuery(scene->last_use[1]) != cudaSuccess))) {
+               ((f.scene->used[0] && cudaEventQuery(f.scene->last_use[0]) != cudaSuccess) || (f.scene->used[1] && cudaEventQuery(f.scene->last_use[1]) != cudaSuccess))) {
       // another geometry, and frames in flight on some lane may still be reading the table of the previous one: this frame
       // renders in the plain permuted order (the table is re-recorded by the first frame that finds the scene idle)
       cudaGetLastError();
@@ -466,36 +473,44 @@ int do_render(futhark_context *ctx, RenderParams &P, const LaunchConfig &lc, int
   const bool self_signal = lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK;
   P.frame_flag = (ff && self_signal) ? ff->done_flag : nullptr;
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
-  const RayQuery &pq = q ? *q : RayQuery{};
-  if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, kind, pq);
+  if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, f.kind, f.q);
   {
-    const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches, kind, pq);
+    const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches, f.kind, f.q);
     if (le == cudaErrorNotSupported) {
       set_error(ctx, "render: kernel %d is not part of this build (libray_b200.so carries mega / warpqueue; the alternatives "
                      "persistent / wavefront / streamqueue / lanewalk are in libray_b200_all.so, built with RAYB200_ALL_KERNELS)", lc.kernel);
       return 1;
     }
     CUDA_TRY(ctx, le);
-    record_plan(ctx, P, lc, kind, false, pq);
+    record_plan(ctx, P, lc, f.kind, false, f.q);
   }
   if (record_order) {  // after the recording frame (outside its timing events' kernel, inside the stream order): cost -> order
-    launch_tile_order_from_cost(P, scene->order_cache.cost, ctx->cfg.long_path == 0 ? 4 : ctx->cfg.long_path, L.tile_order_plan, L.stream, &ctx->launches);
-    if (!scene->order_cache.ready) CUDA_TRY(ctx, cudaEventCreateWithFlags(&scene->order_cache.ready, cudaEventDisableTiming));
-    CUDA_TRY(ctx, cudaEventRecord(scene->order_cache.ready, L.stream));
-    scene->order_cache.state = 1;
+    launch_tile_order_from_cost(P, f.scene->order_cache.cost, ctx->cfg.long_path == 0 ? 4 : ctx->cfg.long_path, L.tile_order_plan, L.stream, &ctx->launches);
+    if (!f.scene->order_cache.ready) CUDA_TRY(ctx, cudaEventCreateWithFlags(&f.scene->order_cache.ready, cudaEventDisableTiming));
+    CUDA_TRY(ctx, cudaEventRecord(f.scene->order_cache.ready, L.stream));
+    f.scene->order_cache.state = 1;
   }
   if (ff && ff->done_flag && !self_signal) launch_flag_bump(ff->done_flag, L.stream);
   CUDA_TRY(ctx, cudaGetLastError());
-  if (scene) {  // this frame reads the scene's device memory until here on this lane
-    if (!scene->last_use[lane_id]) CUDA_TRY(ctx, cudaEventCreateWithFlags(&scene->last_use[lane_id], cudaEventDisableTiming));
-    CUDA_TRY(ctx, cudaEventRecord(scene->last_use[lane_id], L.stream));
-    scene->used[lane_id] = true;
-  }
+  if (record_scene_use(ctx, f.scene, lane_id)) return 1;
   if (timed) {
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_stop, L.stream));
     ctx->have_timing = true;
   }
   ctx->renders++;
+  return 0;
+}
+
+int render_frame(futhark_context *ctx, Frame &f, int lane, bool timed, const FrameFlags *ff) {
+  RenderParams P;
+  LaunchConfig lc;
+  return fill_params(ctx, f, P, lc) || do_render(ctx, f, P, lc, lane, timed, ff);
+}
+
+int record_scene_use(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int lane) {
+  if (!p->last_use[lane]) CUDA_TRY(ctx, cudaEventCreateWithFlags(&p->last_use[lane], cudaEventDisableTiming));
+  CUDA_TRY(ctx, cudaEventRecord(p->last_use[lane], ctx->lanes[lane].stream));
+  p->used[lane] = true;
   return 0;
 }
 
@@ -514,8 +529,6 @@ int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d
   const size_t bytes = (size_t)(h > 0 ? h : 0) * (size_t)(w > 0 ? w : 0) * sizeof(int32_t);
   cudaError_t e = cudaMallocAsync(&img->dev, bytes ? bytes : 4, ctx->stream);
   if (e != cudaSuccess) { set_error(ctx, "render: cudaMallocAsync: %s", cudaGetErrorString(e)); delete img; return 1; }
-  RenderParams P;
-  LaunchConfig lc;
   if (!ctx->peers.empty()) {  // single-process multi-GPU (RAY_GPUS > 1): api_multigpu.cu
     if (render_multi_device(ctx, img, h, w, spp, p)) { cudaFreeAsync(img->dev, ctx->stream); delete img; return 1; }
     *out0 = img;
@@ -523,7 +536,8 @@ int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d
   }
   // With a shard configured, the row-major frame only receives this rank's tiles; clear the rest.
   if (ctx->cfg.world > 1) cudaMemsetAsync(img->dev, 0, bytes, ctx->stream);
-  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, img->dev, nullptr, false, P, lc) || do_render(ctx, P, lc, 0, true, nullptr, p)) {
+  Frame f{p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, img->dev};
+  if (render_frame(ctx, f)) {
     cudaFreeAsync(img->dev, ctx->stream);
     delete img;
     return 1;
@@ -545,10 +559,8 @@ int ray_b200_render_into(struct futhark_context *ctx, int32_t *out_pix_dev, floa
   if (!out_pix_dev) { set_error(ctx, "render_into: out_pix_dev is required"); return 1; }
   if (!ctx->peers.empty()) { set_error(ctx, "render_into: not available on a single-process multi-GPU context (RAY_GPUS > 1): only futhark_entry_render / ray_b200_entry_render_spp gather the helper devices' tiles"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-  RenderParams P;
-  LaunchConfig lc;
-  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc)) return 1;
-  return do_render(ctx, P, lc, 0, true, nullptr, p);
+  Frame f{p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev};
+  return render_frame(ctx, f);
 }
 
 int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, int64_t h, int64_t w, int32_t s_begin,
@@ -560,13 +572,11 @@ int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, in
   if (s_begin < 0 || s_end <= s_begin) { set_error(ctx, "render_accumulate: bad sample range [%d, %d)", s_begin, s_end); return 1; }
   if (!accum_dev) { set_error(ctx, "render_accumulate: accum_dev is required"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-  RayQuery acc{};
-  acc.accum = accum_dev;
-  acc.s_begin = s_begin;
-  RenderParams P;
-  LaunchConfig lc;
-  if (fill_params(ctx, p, h, w, s_end - s_begin, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev, false, P, lc, Query::kAccumulate, &acc)) return 1;
-  return do_render(ctx, P, lc, 0, true, nullptr, p, Query::kAccumulate, &acc);
+  Frame f{p, h, w, s_end - s_begin, ctx->cfg.rank, ctx->cfg.world, out_pix_dev, out_rgb_dev};
+  f.kind = Query::kAccumulate;
+  f.q.accum = accum_dev;
+  f.q.s_begin = s_begin;
+  return render_frame(ctx, f);
 }
 
 int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
@@ -580,11 +590,12 @@ int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark
   if (!cams7_host) { set_error(ctx, "render_views_into: cams7_host is required"); return 1; }
   if (!out_pix_dev) { set_error(ctx, "render_views_into: out_pix_dev is required"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-  RayQuery vq{};
-  vq.n_views = n_views;
+  Frame f{p, h, w, spp, 0, 1, out_pix_dev, out_rgb_dev};
+  f.kind = Query::kViews;
+  f.q.n_views = n_views;
   RenderParams P;
   LaunchConfig lc;
-  if (fill_params(ctx, p, h, w, spp, 0, 1, out_pix_dev, out_rgb_dev, false, P, lc, Query::kViews, &vq)) return 1;
+  if (fill_params(ctx, f, P, lc)) return 1;
   // View v's camera is what prepare_scene(h, w) of a scene with camera cams7[v] makes: make_camera with this call's aspect
   // ratio (ray.fut:243-244).  The table goes to stream-ordered device memory, freed behind the launch, so the caller may
   // reuse cams7_host as soon as the call returns.
@@ -600,10 +611,10 @@ int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark
   float *cams_dev = nullptr;
   CUDA_TRY(ctx, cudaMallocAsync(&cams_dev, bytes, ctx->stream));
   const cudaError_t ce = cudaMemcpyAsync(cams_dev, table.data(), bytes, cudaMemcpyHostToDevice, ctx->stream);
-  vq.cams = cams_dev;
+  f.q.cams = cams_dev;
   int rc = 0;
   if (ce != cudaSuccess) { set_error(ctx, "render_views_into: camera table upload failed: %s", cudaGetErrorString(ce)); rc = 1; }
-  if (!rc) rc = do_render(ctx, P, lc, 0, true, nullptr, p, Query::kViews, &vq);
+  if (!rc) rc = do_render(ctx, f, P, lc);
   const cudaError_t fe = cudaFreeAsync(cams_dev, ctx->stream);
   if (!rc && fe != cudaSuccess) { set_error(ctx, "render_views_into: %s", cudaGetErrorString(fe)); rc = 1; }
   return rc;
@@ -620,9 +631,8 @@ int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, flo
   float *d_rgb = nullptr;
   CUDA_TRY(ctx, cudaMallocAsync(&d_pix, px * 4, ctx->stream));
   if (out_rgb_host) CUDA_TRY(ctx, cudaMallocAsync(&d_rgb, px * 12, ctx->stream));
-  RenderParams P;
-  LaunchConfig lc;
-  int rc = fill_params(ctx, p, h, w, spp, 0, 1, d_pix, d_rgb, false, P, lc) || do_render(ctx, P, lc, 0, true, nullptr, p);
+  Frame f{p, h, w, spp, 0, 1, d_pix, d_rgb};
+  int rc = render_frame(ctx, f);
   if (!rc) {
     if (cudaMemcpyAsync(out_pix_host, d_pix, px * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) rc = 1;
     if (!rc && d_rgb && cudaMemcpyAsync(out_rgb_host, d_rgb, px * 12, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) rc = 1;
@@ -649,14 +659,8 @@ int ray_b200_render_shard_into(struct futhark_context *ctx, int32_t *out_tiles_d
   if (!out_tiles_dev) { set_error(ctx, "render_shard_into: null output"); return 1; }
   if (!ctx->peers.empty()) { set_error(ctx, "render_shard_into: not available on a single-process multi-GPU context (RAY_GPUS > 1)"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-  RenderParams P;
-  LaunchConfig lc;
-  if (fill_params(ctx, p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_tiles_dev, nullptr, true, P, lc)) return 1;
-  // ranks that own one tile fewer than the padded count leave a zeroed tail
-  const int64_t padded = ray_b200_shard_tiles_padded(h, w, ctx->cfg.world);
-  if (P.local_tiles < padded)
-    CUDA_TRY(ctx, cudaMemsetAsync(out_tiles_dev + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4, ctx->stream));
-  return do_render(ctx, P, lc, 0, true, nullptr, p);
+  Frame f{p, h, w, spp, ctx->cfg.rank, ctx->cfg.world, out_tiles_dev, nullptr, true};
+  return render_frame(ctx, f);
 }
 // Several frames in one call, up to two of them in flight: job i runs on lane i % 2, lane 1 forks from the context's
 // stream at the start of the call and joins it at the end, so for the caller the batch behaves like one stream-ordered
@@ -693,24 +697,10 @@ int ray_b200_render_batch(struct futhark_context *ctx, const struct ray_b200_ren
   for (int32_t i = 0; i < n && !rc; i++) {
     const ray_b200_render_job &j = jobs[i];
     const int lane = pipe ? (int)(ctx->lane_seq++ & 1u) : (two_lanes ? (i & 1) : 0);
-    const int32_t spp = j.spp > 0 ? j.spp : ctx->cfg.spp;
-    RenderParams P;
-    LaunchConfig lc;
-    if (j.shard_layout) {
-      rc = fill_params(ctx, j.prepared, j.h, j.w, spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, nullptr, true, P, lc);
-      const int64_t padded = rc ? 0 : ray_b200_shard_tiles_padded(j.h, j.w, ctx->cfg.world);
-      if (!rc && P.local_tiles < padded &&
-          cudaMemsetAsync(j.out_dev + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4,
-                          lane ? L1.stream : ctx->stream) != cudaSuccess) {
-        set_error(ctx, "render_batch: memset failed");
-        rc = 1;
-      }
-    } else {
-      rc = fill_params(ctx, j.prepared, j.h, j.w, spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, j.out_rgb_dev, false, P, lc);
-    }
-    FrameFlags ff;
-    ff.wait_flag = j.wait_flag; ff.wait_value = j.wait_value; ff.done_flag = j.done_flag;
-    if (!rc) rc = do_render(ctx, P, lc, lane, false, (ff.wait_flag || ff.done_flag) ? &ff : nullptr, j.prepared);
+    // (a shard-layout job has no float output: checked above)
+    Frame f{j.prepared, j.h, j.w, j.spp > 0 ? j.spp : ctx->cfg.spp, ctx->cfg.rank, ctx->cfg.world, j.out_dev, j.out_rgb_dev, j.shard_layout != 0};
+    FrameFlags ff{j.wait_flag, j.wait_value, j.done_flag};
+    rc = render_frame(ctx, f, lane, false, (ff.wait_flag || ff.done_flag) ? &ff : nullptr);
   }
   // join even after a failure: whatever was enqueued on lane 1 must be ordered before later work on the context's stream
   // (pipelined submission: no join - the caller orders its reads, see ray_b200_context_set_pipeline)
@@ -859,9 +849,10 @@ int ray_b200_count_work(struct futhark_context *ctx, int64_t h, int64_t w, int32
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
   int32_t *scratch = nullptr;
   CUDA_TRY(ctx, cudaMallocAsync(&scratch, (size_t)h * w * 4, ctx->stream));
+  Frame f{p, h, w, spp, 0, 1, scratch};
   RenderParams P;
   LaunchConfig lc;
-  int rc = fill_params(ctx, p, h, w, spp, 0, 1, scratch, nullptr, false, P, lc);
+  int rc = fill_params(ctx, f, P, lc);
   if (!rc) {
     cudaMemsetAsync(ctx->counters, 0, 4 * sizeof(unsigned long long), ctx->stream);
     launch_count_work(P, ctx->stream, &ctx->launches);

@@ -330,10 +330,11 @@ int ray_b200_prepared_info(struct futhark_context *ctx, const struct futhark_opa
   memset(info, 0, sizeof *info);
   info->n_leaves = p->n; info->n_inner = p->n - 1;
   info->max_depth = p->max_depth; info->refit_sweeps = p->refit_sweeps; info->stale_nodes = p->stale_nodes;
+  Frame f{p, 8, 8, 1};
   RenderParams P;
   LaunchConfig lc;
   std::lock_guard<std::mutex> g(ctx->mu);
-  if (fill_params(ctx, p, 8, 8, 1, 0, 1, nullptr, nullptr, false, P, lc) == 0) info->smem_nodes = P.smem_nodes;
+  if (fill_params(ctx, f, P, lc) == 0) info->smem_nodes = P.smem_nodes;
   memcpy(info->root_box, p->root_box, sizeof info->root_box);
   memcpy(info->camera, &p->cam, sizeof info->camera);
   return 0;
