@@ -75,12 +75,12 @@ int64_t ray_b200_context_launch_count(struct futhark_context *ctx);
  * the first CTA started (exit_us may be NULL to query *count = SMs x warps per CTA).  Syncs the stream. */
 int ray_b200_context_trace_warps(struct futhark_context *ctx, int32_t enable);
 int ray_b200_context_warp_trace(struct futhark_context *ctx, float *exit_us, int64_t capacity, int64_t *count);
-/* What a launch traces (struct ray_b200_plan's query): a frame, a chunk of a progressive frame, several views, or the
- * caller's rays to their closest hit or along their path (trace_hits / trace_paths), to their first hit (occlusion), or
- * to their k nearest hits (multi-hit). */
+/* What a launch traces (struct ray_b200_plan's query): a frame, a chunk of a progressive frame, several views, the
+ * selected pixels of an adaptive progressive frame, or the caller's rays to their closest hit or along their path
+ * (trace_hits / trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit). */
 enum ray_b200_query {
   RAY_B200_QUERY_PIXELS = 0, RAY_B200_QUERY_CLOSEST = 1, RAY_B200_QUERY_ANYHIT = 2, RAY_B200_QUERY_MULTIHIT = 3,
-  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5
+  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6
 };
 /* The plan of the last render kernel launch on the context: the last frame, progressive chunk, views call or ray query
  * (for ray_b200_render_batch, its last job), as it was launched.  Calls that launch no render kernel (a query of n = 0
@@ -182,6 +182,39 @@ int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, flo
 int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, int64_t h, int64_t w,
                                int32_t s_begin, int32_t s_end, int32_t *out_pix_dev, float *out_rgb_dev,
                                const struct futhark_opaque_prepared_scene *p);
+/* Adaptive progressive rendering: n_add more samples for the pixels the caller selects, each pixel continuing from its
+ * own sample count, so that a progressive renderer spends its samples where the image is still noisy (edges,
+ * reflections) and leaves converged pixels alone.
+ * accum_dev: device float[h][w][3], row-major: each pixel's running sum.  counts_dev: device int32[h][w]: how many samples
+ * that sum holds; where counts[p] == 0 the sum is not read (as at s_begin == 0 above).  mask_dev: device uint8[h][w] (a
+ * torch.bool buffer works): a nonzero byte selects the pixel; NULL selects every pixel.
+ *   A selected pixel p with c = counts[p] gets samples [c, c + n_add) added to accum[p] one at a time in sample order in
+ *   f32 (when c == 0 the sum starts as colour_0 itself), counts[p] becomes c + n_add, and out_pix_dev[p] / out_rgb_dev[p]
+ *   (each may be NULL; int32[h][w] / float[h][w][3]) get the pixel at spp = c + n_add: the sum scaled by 1/(c + n_add),
+ *   quantised by the rule above.  Sample s is sample s of the spp semantics above, whatever the chunking.
+ *   Unselected pixels: none of accum, counts, out_pix or out_rgb is read or written there, so the output frame can be the
+ *   caller's persistent display buffer.  A selected pixel whose count is negative, or would pass INT32_MAX (c > INT32_MAX
+ *   - n_add), is treated as unselected and left untouched: the library cannot check counts without a device
+ *   synchronisation (as invalid intervals of the *_ranged queries give the empty answer).
+ *   Exactness: after any sequence of calls on counts that started at 0, accum[p] equals bit for bit what
+ *   ray_b200_render_accumulate(s_begin = 0, s_end = counts[p]) leaves at p, and the pixel and float pixel equal
+ *   ray_b200_render_into(spp = counts[p]) at p (NaN-aware: a NaN is some NaN).  With mask NULL (or all ones) and every
+ *   count equal to s_begin, the call equals ray_b200_render_accumulate(s_begin, s_begin + n_add) in accum and both
+ *   outputs, and raises every count by n_add.
+ *   The call is asynchronous on the context's stream and is two kernel launches, both counted by
+ *   ray_b200_context_launch_count: a selection pass that lists the selected pixels, then the render kernel, which traces
+ *   only those (ray_b200_context_last_render_ms covers both).  Stream order and freeing the prepared scene while the call
+ *   is in flight behave as for ray_b200_render_accumulate.  It runs on the warp-queue kernel whatever RAY_KERNEL or the
+ *   context's kernel says, and uses neither the heavy-first probe nor the learned claim order, nor changes them: renders
+ *   before and after it plan and launch exactly as without it.  The selection list (4 bytes per padded pixel) is
+ *   stream-ordered device memory freed behind the launch.
+ *   Errors (nonzero return, futhark_context_get_error; the context stays usable): every error of
+ *   ray_b200_render_accumulate (image size, an invalid prepared scene, a RAY_GPUS > 1 context), n_add < 1,
+ *   accum_dev == NULL, counts_dev == NULL, and a shard set (world > 1). */
+int ray_b200_render_adaptive(struct futhark_context *ctx, float *accum_dev, int32_t *counts_dev,
+                             const uint8_t *mask_dev, int64_t h, int64_t w, int32_t n_add,
+                             int32_t *out_pix_dev, float *out_rgb_dev,
+                             const struct futhark_opaque_prepared_scene *p);
 /* Several views of one prepared scene in one launch, each with its own camera, sharing the scene's BVH: a camera
  * fly-through over a static scene, a stereo pair, the six faces of a cube map, a batch of poses, or (n_views = 1) the
  * prepared scene seen from another camera without preparing it again.

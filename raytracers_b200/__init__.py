@@ -65,7 +65,7 @@ class Plan(C.Structure):
 
 
 # enum ray_b200_query: what a launch traces (Plan.query)
-QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views")
+QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive")
 
 
 class RenderJob(C.Structure):
@@ -165,6 +165,7 @@ def load_library(variant=""):
         "ray_b200_render_into": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_host": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_accumulate": (C.c_int, [vp, vp, i64, i64, i32, i32, vp, vp, vp]),
+        "ray_b200_render_adaptive": (C.c_int, [vp, vp, vp, vp, i64, i64, i32, vp, vp, vp]),
         "ray_b200_render_views_into": (C.c_int, [vp, vp, vp, i32, i64, i64, i32, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
@@ -616,6 +617,50 @@ class Context:
                                     rgb.data_ptr() if rgb is not None else None)
         self.sync()
         return (pix, rgb) if want_rgb else pix
+
+    def render_adaptive_into(self, accum_dev, counts_dev, h, w, prepared, n_add, mask_dev=None, out_pix_dev=None,
+                             out_rgb_dev=None):
+        """Adaptive progressive rendering (ray_b200_render_adaptive): adds samples [c, c + n_add) to the running sum
+        accum_dev[p] (device float[h][w][3]) of every pixel p that mask_dev (device uint8[h][w]; None = every pixel)
+        selects, where c = counts_dev[p] (device int32[h][w]), raises the count by n_add and writes the pixel at
+        spp = c + n_add to out_pix_dev (int32[h][w]) / out_rgb_dev (float[h][w][3]) where given.  Unselected pixels are
+        neither read nor written.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_render_adaptive(self.handle, _ptr(accum_dev), _ptr(counts_dev), _ptr(mask_dev), int(h),
+                                                      int(w), int(n_add), _ptr(out_pix_dev), _ptr(out_rgb_dev), prepared.handle))
+
+    def render_adaptive(self, prepared, accum, counts, n_add, mask=None, pixels=None, rgb=None):
+        """Adds n_add samples to the pixels `mask` selects, each from its own count: accum is a float32 CUDA tensor
+        [h, w, 3] of running sums, counts an int32 [h, w] tensor of how many samples each sum holds, mask a bool or uint8
+        [h, w] tensor or None (every pixel); all contiguous and on the context's device.  accum and counts are updated in
+        place.  pixels (int32 [h, w]) and rgb (float32 [h, w, 3]), where given, get the selected pixels at their new
+        counts; the other pixels keep what they held.  Returns (pixels, rgb).  Waits for torch's current stream before, and
+        synchronises the context after the call."""
+        import torch
+
+        def check(name, t, dtypes, shape):
+            if not isinstance(t, torch.Tensor) or t.device.type != "cuda" or t.device.index != self.device:
+                raise ValueError(f"{name} must be a CUDA tensor on cuda:{self.device}")
+            if t.dtype not in dtypes or tuple(t.shape) != shape or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous {'/'.join(str(d) for d in dtypes)} tensor of shape {list(shape)}, "
+                                 f"got {t.dtype} {tuple(t.shape)}")
+
+        if not isinstance(accum, torch.Tensor) or accum.dim() != 3:
+            raise ValueError("accum must be a float32 CUDA tensor of shape [h, w, 3]")
+        h, w = int(accum.shape[0]), int(accum.shape[1])
+        check("accum", accum, (torch.float32,), (h, w, 3))
+        check("counts", counts, (torch.int32,), (h, w))
+        if mask is not None:
+            check("mask", mask, (torch.bool, torch.uint8), (h, w))
+        if pixels is not None:
+            check("pixels", pixels, (torch.int32,), (h, w))
+        if rgb is not None:
+            check("rgb", rgb, (torch.float32,), (h, w, 3))
+        # the tensors may still be in flight on torch's stream, which the context's own stream is not ordered after
+        torch.cuda.current_stream(accum.device).synchronize()
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        self.render_adaptive_into(accum.data_ptr(), counts.data_ptr(), h, w, prepared, n_add, ptr(mask), ptr(pixels), ptr(rgb))
+        self.sync()
+        return pixels, rgb
 
     def render_views_into(self, prepared, cams, h, w, spp, out_pix_dev, out_rgb_dev=None):
         """Several views of one prepared scene in one launch (ray_b200_render_views_into): cams = host [V, 7] cameras

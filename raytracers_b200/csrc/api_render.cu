@@ -72,7 +72,8 @@ static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
 
 static_assert((int)Query::kPixels == RAY_B200_QUERY_PIXELS && (int)Query::kClosest == RAY_B200_QUERY_CLOSEST &&
                   (int)Query::kAnyHit == RAY_B200_QUERY_ANYHIT && (int)Query::kMultiHit == RAY_B200_QUERY_MULTIHIT &&
-                  (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS,
+                  (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS &&
+                  (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE,
               "enum ray_b200_query names the values of Query");
 static_assert(sizeof(struct ray_b200_plan) == 80, "struct ray_b200_plan is 16 int32 and 2 int64");
 
@@ -109,6 +110,9 @@ static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
 // 1/s_end; it runs on the warp-queue kernel whatever the context's kernel is.  Query::kViews: the launch renders
 // q.n_views frames of h x w: its work items are the tiles of all of them, so the plan (spread or pixel-bound, K,
 // staging, the sample buffer) is that of one frame of n_views x tiles(h, w) tiles; it runs on the warp-queue kernel too.
+// Query::kAdaptive: the launch adds spp = n_add samples to the selected pixels, planned as a frame of n_add samples over all
+// tiles (an upper bound on its work: the selection is on the device); each pixel's sample offsets are computed by the
+// kernel, so no offset table is made; on the warp-queue kernel too.
 int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc) {
   const futhark_opaque_prepared_scene *p = f.scene;
   const int64_t h = f.h, w = f.w; const int32_t spp = f.spp;
@@ -128,13 +132,14 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   if (f.world < 1 || f.rank < 0 || f.rank >= f.world) { set_error(ctx, "render: bad shard %d/%d", f.rank, f.world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
   const int32_t s_begin = f.kind == Query::kAccumulate ? f.q.s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
-  if (ensure_offsets(ctx, s_end)) return 1;
+  const bool adaptive = f.kind == Query::kAdaptive;
+  if (!adaptive && ensure_offsets(ctx, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
   // h, w only set the pixel grid (ray.fut:246-247) — exactly as in the reference.
   memcpy(P.cam, &p->cam, sizeof P.cam);
   P.W = (int32_t)w; P.H = (int32_t)h; P.spp = spp; P.inv_spp = 1.0f / (float)s_end;
-  P.offsets = ctx->offsets + 2 * (size_t)s_begin;
+  P.offsets = adaptive ? nullptr : ctx->offsets + 2 * (size_t)s_begin;
   P.out_pix = f.out_pix; P.out_rgb = f.out_rgb; P.tile_major = f.tile_major ? 1 : 0;
   P.rank = f.rank; P.world = f.world;
   P.tiles_x = (int32_t)((w + kTileW - 1) / kTileW); P.tiles_y = (int32_t)((h + kTileH - 1) / kTileH);
@@ -381,7 +386,9 @@ static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64
 }
 
 // One frame on one lane (api_internal.h).  Query::kAccumulate, a chunk of a progressive frame, is launched without a
-// claim-order pass (see below); Query::kViews, with the camera table f.q.cams in device memory, without the learned order.
+// claim-order pass (see below); Query::kViews, with the camera table f.q.cams in device memory, without the learned order;
+// Query::kAdaptive, with its selection list f.q.sel / f.q.n_sel in device memory, as two launches: the selection pass, then
+// the render kernel, without a claim-order pass either.
 int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff) {
   futhark_context::Lane &L = ctx->lane(lane_id);
   if (f.tile_major) {  // ranks that own one tile fewer than the padded count leave a zeroed tail (before the timing events)
@@ -414,7 +421,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   // order, and it leaves the scene's learned order as it found it (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = f.kind != Query::kAccumulate && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = f.kind != Query::kAccumulate && f.kind != Query::kAdaptive && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -474,6 +481,10 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   P.frame_flag = (ff && self_signal) ? ff->done_flag : nullptr;
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
   if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, f.kind, f.q);
+  if (f.kind == Query::kAdaptive) {
+    CUDA_TRY(ctx, cudaMemsetAsync(f.q.n_sel, 0, sizeof(int32_t), L.stream));
+    launch_adaptive_select(P, f.q, L.stream, &ctx->launches);
+  }
   {
     const cudaError_t le = launch_render(P, lc, &ctx->wf, L.stream, &ctx->launches, f.kind, f.q);
     if (le == cudaErrorNotSupported) {
@@ -577,6 +588,37 @@ int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, in
   f.q.accum = accum_dev;
   f.q.s_begin = s_begin;
   return render_frame(ctx, f);
+}
+
+int ray_b200_render_adaptive(struct futhark_context *ctx, float *accum_dev, int32_t *counts_dev, const uint8_t *mask_dev,
+                             int64_t h, int64_t w, int32_t n_add, int32_t *out_pix_dev, float *out_rgb_dev,
+                             const struct futhark_opaque_prepared_scene *p) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!ctx->peers.empty()) { set_error(ctx, "render_adaptive: not available on a single-process multi-GPU context (RAY_GPUS > 1)"); return 1; }
+  if (ctx->cfg.world > 1) { set_error(ctx, "render_adaptive: not available with a shard set (rank %d of %d)", ctx->cfg.rank, ctx->cfg.world); return 1; }
+  if (n_add < 1) { set_error(ctx, "render_adaptive: n_add must be >= 1, got %d", n_add); return 1; }
+  if (!accum_dev) { set_error(ctx, "render_adaptive: accum_dev is required"); return 1; }
+  if (!counts_dev) { set_error(ctx, "render_adaptive: counts_dev is required"); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  Frame f{p, h, w, n_add, 0, 1, out_pix_dev, out_rgb_dev};
+  f.kind = Query::kAdaptive;
+  f.q.accum = accum_dev;
+  f.q.sample_counts = counts_dev;
+  f.q.mask = mask_dev;
+  RenderParams P;
+  LaunchConfig lc;
+  if (fill_params(ctx, f, P, lc)) return 1;
+  // The selection list, one item per pixel at most, and its counter in front of it: stream-ordered memory, freed behind the
+  // launch, so nothing is held between calls
+  int32_t *sel = nullptr;
+  CUDA_TRY(ctx, cudaMallocAsync(&sel, ((size_t)P.local_tiles * kTilePixels + 1) * sizeof(int32_t), ctx->stream));
+  f.q.n_sel = sel;
+  f.q.sel = sel + 1;
+  int rc = do_render(ctx, f, P, lc);
+  const cudaError_t fe = cudaFreeAsync(sel, ctx->stream);
+  if (!rc && fe != cudaSuccess) { set_error(ctx, "render_adaptive: %s", cudaGetErrorString(fe)); rc = 1; }
+  return rc;
 }
 
 int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,

@@ -438,6 +438,7 @@ cudaError_t with_query(F &&f, Query q) {
     case Query::kMultiHit: return f(std::integral_constant<Query, Query::kMultiHit>{});
     case Query::kAccumulate: return f(std::integral_constant<Query, Query::kAccumulate>{});
     case Query::kViews: return f(std::integral_constant<Query, Query::kViews>{});
+    case Query::kAdaptive: return f(std::integral_constant<Query, Query::kAdaptive>{});
     default: return cudaErrorInvalidValue;
   }
 }

@@ -97,6 +97,60 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
   ids[lt] = (int32_t)lt;
 }
 
+// ====================================================================================== adaptive progressive rendering
+// Query::kAdaptive: get_ray for sample s of pixel (row j, column i), as primary_ray makes it for a frame of more than one
+// sample, except that the offsets of sample s are computed here, exactly as sample_offsets computes them on the host (the
+// same f32 products, floorf and differences; -fmad=false keeps them apart): each pixel continues from its own count, so
+// there is no one table for the launch.
+__device__ __forceinline__ Ray adaptive_ray(const RenderParams &P, const int i, const int j, const int s) {
+  const float a = (float)s * 0.7548776662f, b = (float)s * 0.5698402909f;
+  const float u = ((float)i + (a - floorf(a))) / (float)P.W;
+  const float v = ((float)(P.H - j) + (b - floorf(b))) / (float)P.H;
+  return camera_ray(P.cam, u, v);
+}
+
+// Query::kAdaptive: the pixel (row j, column i) of sum at spp = n, where inv = 1 / n: written as write_pixel writes a
+// progressive frame's (row-major, each output optional)
+__device__ __forceinline__ void write_adaptive_pixel(const RenderParams &P, const int i, const int j, const V3 sum, const float inv) {
+  const V3 col = vscale(inv, sum);
+  const size_t px = (size_t)j * P.W + i;
+  if (P.out_pix) P.out_pix[px] = pack_pixel(col);
+  if (P.out_rgb) {
+    float *q = P.out_rgb + 3 * px;
+    q[0] = col.x; q[1] = col.y; q[2] = col.z;
+  }
+}
+
+// The selection pass.
+// Query::kAdaptive: the work items of the selected pixels, in claim order.  Thread c walks claim c of the frame's claim
+// sequence (the plain chunk permutation: an adaptive launch has no heavy-first or learned order) and keeps its item when it
+// is a pixel (not tile padding), the mask selects it (mask NULL: every pixel) and its count c_p is valid, 0 <= c_p <=
+// INT32_MAX - n_add.  The count is read only where the mask selects the pixel.  A warp's 32 claims are one tile: one
+// ballot and one atomicAdd per warp append its kept items together, so a tile's selected pixels stay neighbours in the
+// list.  The order of the warps' appends is not fixed; it changes only when a pixel is traced, never its value.
+__global__ void __launch_bounds__(256) select_pixels_kernel(const __grid_constant__ RenderParams P, const __grid_constant__ RayQuery Q) {
+  const long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int lane = threadIdx.x & 31;
+  bool keep = false;
+  int item = 0, i, j;
+  if (c < ((long long)P.n_chunks << 11)) {
+    item = claim_to_item(P, (int)c);
+    if (item < P.local_tiles * kTilePixels && item_pixel(P, item, i, j)) {
+      const size_t px = (size_t)j * P.W + i;
+      if (Q.mask == nullptr || Q.mask[px] != 0) {
+        const int32_t n = Q.sample_counts[px];
+        keep = n >= 0 && n <= 0x7fffffff - P.spp;
+      }
+    }
+  }
+  const unsigned b = __ballot_sync(kFullMask, keep);
+  if (b == 0u) return;
+  int base = 0;
+  if (lane == 0) base = atomicAdd(Q.n_sel, __popc(b));
+  base = __shfl_sync(kFullMask, base, 0);
+  if (keep) Q.sel[base + __popc(b & ((1u << lane) - 1u))] = item;
+}
+
 // ====================================================================================== K3: warp work-queue
 // Dense traversal.  K1/K2 bind a lane to a ray for a whole segment, so a warp's SIMT efficiency is
 // mean/max of its lanes' traversal lengths.  The reference's
@@ -185,6 +239,15 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 // the spread dispenser and finalize_pixels) it also gives its view v; the camera ray reads view v's 12 floats of Q.cams
 // instead of P.cam, and the pixel is stored at offset v * H * W.  Nothing else depends on the view, so every view's
 // pixel sees exactly the arithmetic of a one-view frame whose P.cam is that camera.
+//
+// Query::kAdaptive, the selected pixels of a progressive frame (include/ray_b200.h ray_b200_render_adaptive): every
+// selected pixel p gets the P.spp = n_add samples [c_p, c_p + n_add) that follow its own count c_p =
+// Q.sample_counts[p].  The work items are not the frame's tiles but the list the selection pass (select_pixels_kernel)
+// made in front of the launch: claim c is item Q.sel[c], for c < *Q.n_sel.  Everything else is Query::kAccumulate with
+// c_p in place of Q.s_begin: sample rel of the chunk is sample c_p + rel of the pixel, whose offsets adaptive_ray computes
+// (there is no table of them: the host does not know the counts), the in-order sum starts from Q.accum where c_p > 0, and
+// the owner writes the pixel scaled by 1 / (c_p + n_add), then stores the sum and the count.  c_p is read from
+// Q.sample_counts wherever it is needed; only the pixel's owner writes it, once its last sample has been added.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -200,7 +263,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   constexpr bool kRays = is_ray_query(kQuery);  // ray mode
-  constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews;
+  constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews, kAdapt = kQuery == Query::kAdaptive;
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -250,7 +313,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   uint32_t *nstk = lstk + kWqLeafStack;
 
   const int total = kRays ? Q.n : (int)(P.local_tiles * kTilePixels);
-  const int total_claims = kRays ? Q.n : P.n_chunks << 11;
+  const int total_claims = kRays ? Q.n : (kAdapt ? *Q.n_sel : P.n_chunks << 11);
   // the query's interval (ray mode; kRanged: each slot's own instead) or the literal one of ray_colour (ray.fut:130)
   const float t_lo = kRays ? Q.t_min : 0.0f, t_hi = kRays ? Q.t_max : 1000000000.0f;
   const int spp = P.spp;
@@ -265,6 +328,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   if (kSpread) cbuf = P.sample_buf + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * kWqRing * (size_t)spp;
   // kAccum: the running sum of pixel (row pj, column pi), row-major as the frame (64-bit offsets: 2^30 pixels pass 4 GiB)
   [[maybe_unused]] auto accum_of = [&](const int pi, const int pj) { return Q.accum + 3 * ((size_t)pj * P.W + pi); };
+  // kAdapt: the sample count of pixel (row pj, column pi)
+  [[maybe_unused]] auto count_of = [&](const int pi, const int pj) { return Q.sample_counts + ((size_t)pj * P.W + pi); };
   // pixel item -> (view, column, row), false for a padding pixel; the view is 0 unless kViews
   auto pixel_of = [&](const int item, int &pv, int &pi, int &pj) {
     if constexpr (kViews) return item_view_pixel(P, item, pv, pi, pj);
@@ -293,6 +358,30 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       __stcg(cbuf + (size_t)(ms >> 16) * spp + (ms & 0xffff), make_float4(colour.x, colour.y, colour.z, 0.0f));
       atomicAdd(ring_done + (ms >> 16), 1);
       p_item[slot] = -1;
+    } else if constexpr (kAdapt) {
+      // as kAccum below, from the pixel's own count c: only its sample c + 0 = 0 starts the sum, later ones add to it
+      const int item = p_item[slot];
+      const float4 ps = p_sum[slot];
+      int s = __float_as_int(ps.w);
+      int pi, pj, pv;
+      pixel_of(item, pv, pi, pj);
+      int32_t *cnt = count_of(pi, pj);
+      const int c = *cnt;
+      const V3 sum = (s == 0 && c == 0) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
+      s++;
+      if (s < spp) {
+        const Ray nr = adaptive_ray(P, pi, pj, c + s);
+        ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
+        ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
+        p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
+        p_sum[slot] = make_float4(sum.x, sum.y, sum.z, __int_as_float(s));
+      } else {
+        write_adaptive_pixel(P, pi, pj, sum, 1.0f / (float)(c + spp));
+        float *a = accum_of(pi, pj);
+        a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
+        *cnt = c + spp;
+        p_item[slot] = -1;
+      }
     } else {
       const int item = p_item[slot];
       const float4 ps = p_sum[slot];
@@ -394,7 +483,20 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       float sum = 0.0f;
       if (ready && ch < 3) {
         const float *c = reinterpret_cast<const float *>(cbuf + (size_t)m * spp) + ch;
-        if constexpr (kAccum) {
+        if constexpr (kAdapt) {
+          // the pixel's running sum where its count is above 0, else its first sample of this call (a selected pixel is
+          // never a padding pixel)
+          int s = 1, pi, pj;
+          item_pixel(P, ring_item[m], pi, pj);
+          if (*count_of(pi, pj) > 0) {
+            sum = accum_of(pi, pj)[ch];
+            s = 0;
+          } else {
+            sum = __ldcg(c);
+          }
+#pragma unroll 4
+          for (; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+        } else if constexpr (kAccum) {
           // a later chunk adds its samples to the running sum of the earlier ones, the first chunk starts at its sample 0
           int s = 1, pi, pj;
           if (Q.s_begin > 0 && item_pixel(P, ring_item[m], pi, pj)) {
@@ -416,10 +518,19 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const int item = ring_item[m];
         int pi, pj, pv;
         if (pixel_of(item, pv, pi, pj)) {
-          write_pixel<kQuery>(P, item, pi, pj, v3(sum, g, b), pv);
-          if constexpr (kAccum) {
+          if constexpr (kAdapt) {
+            int32_t *cnt = count_of(pi, pj);
+            const int cp = *cnt;
+            write_adaptive_pixel(P, pi, pj, v3(sum, g, b), 1.0f / (float)(cp + spp));
             float *a = accum_of(pi, pj);
             a[0] = sum; a[1] = g; a[2] = b;
+            *cnt = cp + spp;
+          } else {
+            write_pixel<kQuery>(P, item, pi, pj, v3(sum, g, b), pv);
+            if constexpr (kAccum) {
+              float *a = accum_of(pi, pj);
+              a[0] = sum; a[1] = g; a[2] = b;
+            }
           }
         } else if (P.tile_major) {
           P.out_pix[item] = 0;
@@ -460,7 +571,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             const int slot = lane + 32 * k;
             if (p_item[slot] < 0) {
               const int c = base + rank++;
-              const int item = c < total_claims ? (kRays ? c : claim_to_item(P, c)) : total;
+              const int item = c < total_claims ? (kRays ? c : (kAdapt ? __ldg(Q.sel + c) : claim_to_item(P, c))) : total;
               int pi, pj, pv;
               if (kRanged && item < total) {
                 // struct ray_b200_ray (64-bit offset: n reaches 2^30); a 16-byte aligned buffer takes two 16-byte loads
@@ -486,7 +597,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                 p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
               } else if (item < total) {
                 if (pixel_of(item, pv, pi, pj)) {
-                  const Ray r = primary_ray<kQuery>(P, pi, pj, 0, view_cam(pv));
+                  const int c0 = kAdapt ? *count_of(pi, pj) : 0;  // kAdapt: the pixel's first sample of this call
+                  const Ray r = kAdapt ? adaptive_ray(P, pi, pj, c0) : primary_ray<kQuery>(P, pi, pj, 0, view_cam(pv));
                   p_item[slot] = item;
                   ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                   ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -494,6 +606,13 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                   if constexpr (kAccum) {  // a later chunk's sum starts from the running sum of the earlier ones
                     float4 ps = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
                     if (Q.s_begin > 0) {
+                      const float *a = accum_of(pi, pj);
+                      ps.x = a[0]; ps.y = a[1]; ps.z = a[2];
+                    }
+                    p_sum[slot] = ps;
+                  } else if constexpr (kAdapt) {  // ... and from the pixel's own running sum where its count is above 0
+                    float4 ps = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
+                    if (c0 > 0) {
                       const float *a = accum_of(pi, pj);
                       ps.x = a[0]; ps.y = a[1]; ps.z = a[2];
                     }
@@ -519,7 +638,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
           if (lane == 0) c = atomicAdd(P.work_cursor, 1);
           c = __shfl_sync(kFullMask, c, 0);
           if (c >= total_claims) { exhausted = true; break; }
-          const int item = claim_to_item(P, c);
+          const int item = kAdapt ? __ldg(Q.sel + c) : claim_to_item(P, c);
           if (item >= total) continue;  // tail of the last (partial) chunk
           __syncwarp();                 // every lane has read ring_done[m] before lane 0 overwrites it
           if (lane == 0) { ring_item[m] = item; ring_done[m] = 0; }
@@ -540,7 +659,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               const int item = ring_item[m];
               int pi, pj, pv;
               if (pixel_of(item, pv, pi, pj)) {
-                const Ray r = primary_ray<kQuery>(P, pi, pj, s, view_cam(pv));
+                const Ray r = kAdapt ? adaptive_ray(P, pi, pj, *count_of(pi, pj) + s) : primary_ray<kQuery>(P, pi, pj, s, view_cam(pv));
                 p_item[slot] = item;
                 ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                 ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -979,8 +1098,11 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
       }, k == 2, all_nodes, sph, ranged);
     else
       return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-        return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(
-            lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
+        // (kAdaptive is not built for every sphere staged without every node, which split_staging never plans)
+        if constexpr (query == Query::kAdaptive && s && !a) return cudaErrorInvalidValue;
+        else
+          return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(
+              lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
       }, k == 2, spread, packet, all_nodes, sph);
   }, kind);
   if (e == cudaSuccess) (*launches)++;
@@ -1020,6 +1142,12 @@ void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStr
   cub::DeviceRadixSort::SortPairs(b.sort_tmp, bytes, b.keys, b.keys_sorted, b.ids, b.order, (int)p.local_tiles, 0,
                                   tile_order_key_bits(p.n_chunks), stream);
   if (launches) *launches += 2;  // the cub sort is counted as one
+}
+
+void launch_adaptive_select(const RenderParams &p, const RayQuery &q, cudaStream_t stream, int64_t *launches) {
+  const long long claims = (long long)p.n_chunks << 11;
+  select_pixels_kernel<<<(unsigned)((claims + 255) / 256), 256, 0, stream>>>(p, q);
+  (*launches)++;
 }
 
 void launch_tile_order_from_cost(const RenderParams &p, const uint32_t *cost, int32_t long_path, const TileOrderBuffers &b,

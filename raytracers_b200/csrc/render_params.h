@@ -63,9 +63,10 @@ struct RenderParams {
 // s_begin); kViews, several views in one launch (cams, n_views, view_tiles).  Ray kinds, the caller's rays of a ray query
 // (include/ray_b200.h "ray queries"; rays, n, perm, t_min, t_max): kClosest, to their closest hit (hits) or along their
 // path (rgb, segments, max_depth; hits == NULL tells the two apart at run time); kAnyHit, to their first accepted sphere
-// (occluded); kMultiHit, to their k nearest ones (hits, k, counts).  New kinds go at the end: kernel names carry the
-// values, and tools/sass_compare.py reads older builds' names by them.
-enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews };
+// (occluded); kMultiHit, to their k nearest ones (hits, k, counts).  kAdaptive, a pixel kind: the selected pixels of a
+// progressive frame, each from its own sample count (accum, sample_counts, mask, sel, n_sel).  New kinds go at the end:
+// kernel names carry the values, and tools/sass_compare.py reads older builds' names by them.
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive };
 __host__ __device__ constexpr bool is_ray_query(Query q) {
   return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
 }
@@ -97,6 +98,15 @@ struct RayQuery {
   // laid out as RenderParams::cam) and written at pixel offset v * H * W of the outputs
   const float *cams;
   int32_t n_views, view_tiles;
+  // adaptive progressive rendering (Query::kAdaptive; include/ray_b200.h ray_b200_render_adaptive): P.spp = n_add samples
+  // are added to the selected pixels, each from its own count.  sample_counts, row-major [H][W]: the samples in accum's
+  // sum of each pixel (accum is not read where it is 0); mask, row-major [H][W] (NULL = every pixel): nonzero = selected.
+  // The selection pass writes the work items of the selected pixels with a valid count to sel, in claim order, and their
+  // number to *n_sel, which the render kernel claims instead of the frame's tiles
+  int32_t *sample_counts;
+  const uint8_t *mask;
+  int32_t *sel;
+  int32_t *n_sel;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
@@ -139,8 +149,8 @@ struct LaunchConfig {
   long long stage_budget;  // warp-queue kernel: shared memory its queues leave for staging, before cap_staging (bytes)
 };
 
-// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate and kViews, which read q,
-// on the warp-queue kernel only
+// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate, kViews and kAdaptive, which
+// read q, on the warp-queue kernel only
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches, Query kind, const RayQuery &q);
 // The warp-queue kernel (render_kernels.cu): a launch of kind `kind`, a pixel kind or a ray query (whatever lc.kernel
@@ -166,6 +176,8 @@ inline int tile_order_key_bits(int32_t n_chunks) {  // keys are positions < n_ch
   while (bits < 32 && (1ll << bits) < (long long)n_chunks * 64) bits++;
   return bits;
 }
+// Query::kAdaptive: the selection pass in front of the render kernel (q.sel, q.n_sel; *q.n_sel zeroed by the caller)
+void launch_adaptive_select(const RenderParams &p, const RayQuery &q, cudaStream_t stream, int64_t *launches);
 // of a frame of pixel kind `kind`: Query::kViews probes each tile with its view's camera (q.cams)
 void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches, Query kind,
                        const RayQuery &q);
