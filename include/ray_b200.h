@@ -76,11 +76,11 @@ int64_t ray_b200_context_launch_count(struct futhark_context *ctx);
 int ray_b200_context_trace_warps(struct futhark_context *ctx, int32_t enable);
 int ray_b200_context_warp_trace(struct futhark_context *ctx, float *exit_us, int64_t capacity, int64_t *count);
 /* What a launch traces (struct ray_b200_plan's query): a frame, a chunk of a progressive frame, several views, the
- * selected pixels of an adaptive progressive frame, or the caller's rays to their closest hit or along their path
+ * selected pixels of an adaptive progressive frame (ADAPTIVE_VAR: with their sample variance), or the caller's rays to their closest hit or along their path
  * (trace_hits / trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit). */
 enum ray_b200_query {
   RAY_B200_QUERY_PIXELS = 0, RAY_B200_QUERY_CLOSEST = 1, RAY_B200_QUERY_ANYHIT = 2, RAY_B200_QUERY_MULTIHIT = 3,
-  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6
+  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6, RAY_B200_QUERY_ADAPTIVE_VAR = 7
 };
 /* The plan of the last render kernel launch on the context: the last frame, progressive chunk, views call or ray query
  * (for ray_b200_render_batch, its last job), as it was launched.  Calls that launch no render kernel (a query of n = 0
@@ -215,6 +215,50 @@ int ray_b200_render_adaptive(struct futhark_context *ctx, float *accum_dev, int3
                              const uint8_t *mask_dev, int64_t h, int64_t w, int32_t n_add,
                              int32_t *out_pix_dev, float *out_rgb_dev,
                              const struct futhark_opaque_prepared_scene *p);
+/* Adaptive progressive rendering with a noise estimate: ray_b200_render_adaptive that also keeps, per pixel and channel,
+ * the spread of the pixel's samples, so that a caller can tell where the image is still noisy (ray_b200_adaptive_select).
+ * m2_dev: device float[h][w][3], row-major like accum_dev: M2, Welford's running f32 sum of squared deviations from the
+ * mean.  Everything ray_b200_render_adaptive promises holds unchanged (selection, counts, outputs, untouched unselected
+ * pixels, invalid counts, errors, the two launches); m2 is read and written exactly where accum is.
+ *   The rule, per channel: let x_k be the colour of the pixel's sample k, counted over the pixel's whole life, and S_k
+ *   the f32 sum of samples [0, k) that accum holds (S_1 = x_0, S_{k+1} = S_k + x_k).  After sample 0, M2 = +0.0 (where
+ *   the count is 0, m2 is not read, as accum is not).  Sample k >= 1 updates
+ *       M2 = M2 + (x_k - S_k / f32(k)) * (x_k - S_{k+1} / f32(k + 1))
+ *   in f32 with IEEE division and no contraction, one sample at a time in sample order, whatever the chunking of calls.
+ *   Then M2 / (n - 1) is the sample variance of the pixel's n samples.  Welford's form, not a sum of squares: M2 / n -
+ *   mean^2 cancels catastrophically in f32 once counts reach the hundreds.
+ *   Exactness: after any sequence of calls on counts that started at 0, accum, counts and both outputs equal what the
+ *   same sequence of ray_b200_render_adaptive calls leaves, bit for bit, and m2[p] equals the rule applied to samples
+ *   [0, counts[p]) of p (NaN-aware).  Where the caller mixes in other calls, m2 is whatever the caller left there.
+ *   Errors: those of ray_b200_render_adaptive, and m2_dev == NULL. */
+int ray_b200_render_adaptive_var(struct futhark_context *ctx, float *accum_dev, float *m2_dev, int32_t *counts_dev,
+                                 const uint8_t *mask_dev, int64_t h, int64_t w, int32_t n_add,
+                                 int32_t *out_pix_dev, float *out_rgb_dev,
+                                 const struct futhark_opaque_prepared_scene *p);
+/* The pixels of an adaptive progressive frame that still need samples, by the noise estimate of
+ * ray_b200_render_adaptive_var: writes mask_dev[p] (device uint8[h][w]; a torch.bool buffer works) = 0 or 1 for every
+ * pixel.  With n = counts_dev[p], S = accum_dev[p] and M = m2_dev[p] (device buffers laid out as for
+ * ray_b200_render_adaptive_var), mask[p] = 1 iff 0 <= n < max_count and either n < min_count or E > T, where, in f32 and
+ * in this order:
+ *       v = (M.r + M.g) + M.b
+ *       E = v / (f32(n) * f32(n - 1))                  (the three channels' variances of the mean, summed)
+ *       m = ((S.r + S.g) + S.b) / f32(n) + mean_floor
+ *       T = (rel_err * m) * (rel_err * m)
+ *   So a pixel is done when the standard error of its channel sum is at most rel_err times its mean (plus mean_floor,
+ *   which keeps dark pixels from asking for a relative error of 0).  NaN compares false: a NaN pixel at or above
+ *   min_count is not selected.  accum and m2 are read only where min_count <= n < max_count.  n_selected_dev (device
+ *   int32, may be NULL) receives the number of ones.
+ *   The call is one kernel launch on the context's stream, asynchronous, counted by ray_b200_context_launch_count; it
+ *   leaves ray_b200_context_last_plan and ray_b200_context_last_render_ms unchanged.  The mask feeds the next
+ *   ray_b200_render_adaptive_var, so a caller renders "to 1 % noise, at most 512 spp" reading nothing but n_selected:
+ *       render_adaptive_var(mask = NULL, n_add = min_spp)
+ *       repeat: adaptive_select(..., max_count = max_spp - step + 1, ...); render_adaptive_var(mask, step)
+ *   Errors (nonzero return, futhark_context_get_error; the context stays usable): an image size ray_b200_render_into
+ *   rejects, a NULL accum_dev, m2_dev, counts_dev or mask_dev, rel_err or mean_floor not finite or below 0,
+ *   min_count < 2 (E needs two samples), and max_count < min_count. */
+int ray_b200_adaptive_select(struct futhark_context *ctx, const float *accum_dev, const float *m2_dev,
+                             const int32_t *counts_dev, int64_t h, int64_t w, float rel_err, float mean_floor,
+                             int32_t min_count, int32_t max_count, uint8_t *mask_dev, int32_t *n_selected_dev);
 /* Several views of one prepared scene in one launch, each with its own camera, sharing the scene's BVH: a camera
  * fly-through over a static scene, a stereo pair, the six faces of a cube map, a batch of poses, or (n_views = 1) the
  * prepared scene seen from another camera without preparing it again.

@@ -65,7 +65,7 @@ class Plan(C.Structure):
 
 
 # enum ray_b200_query: what a launch traces (Plan.query)
-QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive")
+QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var")
 
 
 class RenderJob(C.Structure):
@@ -166,6 +166,8 @@ def load_library(variant=""):
         "ray_b200_render_host": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_accumulate": (C.c_int, [vp, vp, i64, i64, i32, i32, vp, vp, vp]),
         "ray_b200_render_adaptive": (C.c_int, [vp, vp, vp, vp, i64, i64, i32, vp, vp, vp]),
+        "ray_b200_render_adaptive_var": (C.c_int, [vp, vp, vp, vp, vp, i64, i64, i32, vp, vp, vp]),
+        "ray_b200_adaptive_select": (C.c_int, [vp, vp, vp, vp, i64, i64, C.c_float, C.c_float, i32, i32, vp, vp]),
         "ray_b200_render_views_into": (C.c_int, [vp, vp, vp, i32, i64, i64, i32, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
@@ -289,6 +291,16 @@ def camera_table(cams):
     if a.dtype.kind != "f":
         raise ValueError(f"cams must be floating-point, got {a.dtype}")
     return np.ascontiguousarray(a, np.float32)
+
+
+def _check_tensor(device, name, t, dtypes, shape):
+    """ValueError unless t is a contiguous CUDA tensor on cuda:device of one of dtypes and of this shape"""
+    import torch
+    if not isinstance(t, torch.Tensor) or t.device.type != "cuda" or t.device.index != device:
+        raise ValueError(f"{name} must be a CUDA tensor on cuda:{device}")
+    if t.dtype not in dtypes or tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous {'/'.join(str(d) for d in dtypes)} tensor of shape {list(shape)}, "
+                         f"got {t.dtype} {tuple(t.shape)}")
 
 
 def camera_rays(camera, h, w, spp=1):
@@ -628,26 +640,41 @@ class Context:
         self._check(self.lib.ray_b200_render_adaptive(self.handle, _ptr(accum_dev), _ptr(counts_dev), _ptr(mask_dev), int(h),
                                                       int(w), int(n_add), _ptr(out_pix_dev), _ptr(out_rgb_dev), prepared.handle))
 
-    def render_adaptive(self, prepared, accum, counts, n_add, mask=None, pixels=None, rgb=None):
+    def render_adaptive_var_into(self, accum_dev, m2_dev, counts_dev, h, w, prepared, n_add, mask_dev=None, out_pix_dev=None,
+                                 out_rgb_dev=None):
+        """render_adaptive_into that also keeps each pixel's M2 (ray_b200_render_adaptive_var): m2_dev (device
+        float[h][w][3]) is Welford's running sum of squared deviations of the pixel's samples, per channel, so that
+        m2 / (count - 1) is their variance.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_render_adaptive_var(self.handle, _ptr(accum_dev), _ptr(m2_dev), _ptr(counts_dev),
+                                                          _ptr(mask_dev), int(h), int(w), int(n_add), _ptr(out_pix_dev),
+                                                          _ptr(out_rgb_dev), prepared.handle))
+
+    def adaptive_select_into(self, accum_dev, m2_dev, counts_dev, h, w, rel_err, mean_floor, min_count, max_count, mask_dev,
+                             n_selected_dev=None):
+        """The pixels that still need samples (ray_b200_adaptive_select): mask_dev[p] (device uint8[h][w]) = 1 where
+        0 <= count < max_count and either count < min_count or the pixel's variance of the mean, summed over the
+        channels, is above (rel_err * (mean channel sum + mean_floor))^2; n_selected_dev (device int32, or None) gets
+        the number of ones.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_adaptive_select(self.handle, _ptr(accum_dev), _ptr(m2_dev), _ptr(counts_dev), int(h),
+                                                      int(w), float(rel_err), float(mean_floor), int(min_count),
+                                                      int(max_count), _ptr(mask_dev), _ptr(n_selected_dev)))
+
+    def render_adaptive(self, prepared, accum, counts, n_add, mask=None, pixels=None, rgb=None, m2=None):
         """Adds n_add samples to the pixels `mask` selects, each from its own count: accum is a float32 CUDA tensor
         [h, w, 3] of running sums, counts an int32 [h, w] tensor of how many samples each sum holds, mask a bool or uint8
         [h, w] tensor or None (every pixel); all contiguous and on the context's device.  accum and counts are updated in
         place.  pixels (int32 [h, w]) and rgb (float32 [h, w, 3]), where given, get the selected pixels at their new
-        counts; the other pixels keep what they held.  Returns (pixels, rgb).  Waits for torch's current stream before, and
-        synchronises the context after the call."""
+        counts; the other pixels keep what they held.  m2 (float32 [h, w, 3]), where given, is each pixel's M2 and is
+        updated too (ray_b200_render_adaptive_var; see adaptive_select).  Returns (pixels, rgb).  Waits for torch's
+        current stream before, and synchronises the context after the call."""
         import torch
-
-        def check(name, t, dtypes, shape):
-            if not isinstance(t, torch.Tensor) or t.device.type != "cuda" or t.device.index != self.device:
-                raise ValueError(f"{name} must be a CUDA tensor on cuda:{self.device}")
-            if t.dtype not in dtypes or tuple(t.shape) != shape or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous {'/'.join(str(d) for d in dtypes)} tensor of shape {list(shape)}, "
-                                 f"got {t.dtype} {tuple(t.shape)}")
-
+        check = lambda *a: _check_tensor(self.device, *a)
         if not isinstance(accum, torch.Tensor) or accum.dim() != 3:
             raise ValueError("accum must be a float32 CUDA tensor of shape [h, w, 3]")
         h, w = int(accum.shape[0]), int(accum.shape[1])
         check("accum", accum, (torch.float32,), (h, w, 3))
+        if m2 is not None:
+            check("m2", m2, (torch.float32,), (h, w, 3))
         check("counts", counts, (torch.int32,), (h, w))
         if mask is not None:
             check("mask", mask, (torch.bool, torch.uint8), (h, w))
@@ -658,9 +685,80 @@ class Context:
         # the tensors may still be in flight on torch's stream, which the context's own stream is not ordered after
         torch.cuda.current_stream(accum.device).synchronize()
         ptr = lambda t: t.data_ptr() if t is not None else None
-        self.render_adaptive_into(accum.data_ptr(), counts.data_ptr(), h, w, prepared, n_add, ptr(mask), ptr(pixels), ptr(rgb))
+        if m2 is None:
+            self.render_adaptive_into(accum.data_ptr(), counts.data_ptr(), h, w, prepared, n_add, ptr(mask), ptr(pixels), ptr(rgb))
+        else:
+            self.render_adaptive_var_into(accum.data_ptr(), m2.data_ptr(), counts.data_ptr(), h, w, prepared, n_add, ptr(mask),
+                                          ptr(pixels), ptr(rgb))
         self.sync()
         return pixels, rgb
+
+    def adaptive_select(self, accum, m2, counts, rel_err, mean_floor, min_count, max_count, out=None):
+        """The pixels of an adaptive frame that still need samples, by the noise estimate of render_adaptive(m2=...)
+        (ray_b200_adaptive_select): accum and m2 are float32 CUDA tensors [h, w, 3], counts int32 [h, w], out a bool or
+        uint8 [h, w] tensor or None (a new bool tensor); all contiguous and on the context's device.  A pixel with count n
+        is selected when 0 <= n < max_count and either n < min_count or the variance of its mean, summed over the three
+        channels, is above (rel_err * (mean channel sum + mean_floor))^2.  Returns (mask, n_selected), n_selected an int32
+        CUDA tensor of shape [1].  Waits for torch's current stream before, and synchronises the context after the call."""
+        import torch
+        check = lambda *a: _check_tensor(self.device, *a)
+        if not isinstance(accum, torch.Tensor) or accum.dim() != 3:
+            raise ValueError("accum must be a float32 CUDA tensor of shape [h, w, 3]")
+        h, w = int(accum.shape[0]), int(accum.shape[1])
+        check("accum", accum, (torch.float32,), (h, w, 3))
+        check("m2", m2, (torch.float32,), (h, w, 3))
+        check("counts", counts, (torch.int32,), (h, w))
+        if out is None:
+            out = torch.empty((h, w), dtype=torch.bool, device=accum.device)
+        check("out", out, (torch.bool, torch.uint8), (h, w))
+        n_sel = torch.empty(1, dtype=torch.int32, device=accum.device)
+        torch.cuda.current_stream(accum.device).synchronize()
+        self.adaptive_select_into(accum.data_ptr(), m2.data_ptr(), counts.data_ptr(), h, w, rel_err, mean_floor, min_count,
+                                  max_count, out.data_ptr(), n_sel.data_ptr())
+        self.sync()
+        return out, n_sel
+
+    def render_converged(self, prepared, h, w, rel_err, mean_floor=0.1, min_spp=8, step=8, max_spp=512, want_rgb=False):
+        """Renders the prepared scene at h x w until every pixel's noise estimate is within rel_err, at most max_spp
+        samples per pixel: min_spp samples everywhere, then rounds of `step` more samples for the pixels adaptive_select
+        still selects (min_count = min_spp, max_count = max_spp - step + 1, so no pixel passes max_spp), until a round
+        selects none.  A pixel's target is rel_err times (its mean channel sum + mean_floor).  The floor keeps dark
+        pixels from asking for a relative error of a mean near 0, which no sample count reaches; the default 0.1 is a
+        channel sum of about 8 / 255 per channel, the darkest level the quantised pixel shows apart from black.
+        Every pixel equals render_into(spp = counts[p]) at its own count.  Reads the selected count once per round.
+        Returns (pixels int32 [h, w], rgb float32 [h, w, 3] if want_rgb, counts int32 [h, w],
+        {"rounds": calls of the render kernel, "samples": samples traced}).  Waits for torch's current stream before,
+        and synchronises the context after the call."""
+        import torch
+        if min_spp < 2 or step < 1 or max_spp < min_spp:
+            raise ValueError(f"render_converged: need min_spp >= 2, step >= 1 and max_spp >= min_spp, got {min_spp}, {step}, {max_spp}")
+        dev = torch.device("cuda", self.device)
+        accum = torch.empty((h, w, 3), dtype=torch.float32, device=dev)
+        m2 = torch.empty((h, w, 3), dtype=torch.float32, device=dev)
+        counts = torch.zeros((h, w), dtype=torch.int32, device=dev)
+        pix = torch.zeros((h, w), dtype=torch.int32, device=dev)
+        rgb = torch.zeros((h, w, 3), dtype=torch.float32, device=dev) if want_rgb else None
+        mask = torch.empty((h, w), dtype=torch.bool, device=dev)
+        n_sel = torch.empty(1, dtype=torch.int32, device=dev)
+        torch.cuda.current_stream(dev).synchronize()
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        self.render_adaptive_var_into(accum.data_ptr(), m2.data_ptr(), counts.data_ptr(), h, w, prepared, min_spp, None,
+                                      pix.data_ptr(), ptr(rgb))
+        rounds, samples = 1, h * w * min_spp
+        while min_spp + step <= max_spp:
+            self.adaptive_select_into(accum.data_ptr(), m2.data_ptr(), counts.data_ptr(), h, w, rel_err, mean_floor, min_spp,
+                                      max_spp - step + 1, mask.data_ptr(), n_sel.data_ptr())
+            self.render_adaptive_var_into(accum.data_ptr(), m2.data_ptr(), counts.data_ptr(), h, w, prepared, step,
+                                          mask.data_ptr(), pix.data_ptr(), ptr(rgb))
+            self.sync()
+            n = int(n_sel.item())
+            if n == 0:
+                break
+            rounds += 1
+            samples += n * step
+        self.sync()
+        stats = {"rounds": rounds, "samples": samples}
+        return (pix, rgb, counts, stats) if want_rgb else (pix, counts, stats)
 
     def render_views_into(self, prepared, cams, h, w, spp, out_pix_dev, out_rgb_dev=None):
         """Several views of one prepared scene in one launch (ray_b200_render_views_into): cams = host [V, 7] cameras

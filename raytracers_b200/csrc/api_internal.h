@@ -180,9 +180,9 @@ struct Frame {
   float *out_rgb = nullptr;
   bool tile_major = false;     // out_pix holds this rank's tiles, padded to ray_b200_shard_tiles_padded (do_render zeroes the tail)
   Query kind = Query::kPixels; // a pixel kind: kAccumulate (ray_b200_render_accumulate), kViews (ray_b200_render_views_into),
-                               // kAdaptive (ray_b200_render_adaptive)
+                               // kAdaptive (ray_b200_render_adaptive), kAdaptiveVar (ray_b200_render_adaptive_var)
   RayQuery q{};                // kAccumulate: accum, s_begin.  kViews: n_views, and cams once uploaded (view_tiles: fill_params).
-                               // kAdaptive: accum, sample_counts, mask, and sel / n_sel once allocated
+                               // kAdaptive: accum, sample_counts, mask, and sel / n_sel once allocated.  kAdaptiveVar: those and m2
 };
 // The parameter block of frame f and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
 // slots, ...), which the caller hands to do_render with f; sets f.q.view_tiles of a kViews frame.

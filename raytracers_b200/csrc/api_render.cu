@@ -73,7 +73,7 @@ static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
 static_assert((int)Query::kPixels == RAY_B200_QUERY_PIXELS && (int)Query::kClosest == RAY_B200_QUERY_CLOSEST &&
                   (int)Query::kAnyHit == RAY_B200_QUERY_ANYHIT && (int)Query::kMultiHit == RAY_B200_QUERY_MULTIHIT &&
                   (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS &&
-                  (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE,
+                  (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE && (int)Query::kAdaptiveVar == RAY_B200_QUERY_ADAPTIVE_VAR,
               "enum ray_b200_query names the values of Query");
 static_assert(sizeof(struct ray_b200_plan) == 80, "struct ray_b200_plan is 16 int32 and 2 int64");
 
@@ -95,6 +95,11 @@ void record_plan(futhark_context *ctx, const RenderParams &P, const LaunchConfig
   r.dynamic_smem = (int64_t)v.smem;
 }
 
+// A frame size every pixel launch accepts: work items are 32-bit, so at most 2^30 (padded) pixels per frame
+static bool image_size_ok(int64_t h, int64_t w) {
+  return h > 0 && w > 0 && h <= 65536 && w <= 65536 && ((h + 3) / 4) * ((w + 7) / 8) <= ((int64_t)1 << 25);
+}
+
 // Bytes of the finished-sample buffer of `spp` spread samples on `warps` warps per CTA (one CTA per SM); 0 when samples
 // are not spread: one sample, more than 65535, spreading switched off, or a buffer over kSpreadBudget.  Planning asks for
 // kWqMaxWarps, which bounds every plan (the warps it picks depend on whether samples are spread); do_render, for lc's.
@@ -112,14 +117,13 @@ static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
 // staging, the sample buffer) is that of one frame of n_views x tiles(h, w) tiles; it runs on the warp-queue kernel too.
 // Query::kAdaptive: the launch adds spp = n_add samples to the selected pixels, planned as a frame of n_add samples over all
 // tiles (an upper bound on its work: the selection is on the device); each pixel's sample offsets are computed by the
-// kernel, so no offset table is made; on the warp-queue kernel too.
+// kernel, so no offset table is made; on the warp-queue kernel too.  Query::kAdaptiveVar is planned as kAdaptive.
 int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc) {
   const futhark_opaque_prepared_scene *p = f.scene;
   const int64_t h = f.h, w = f.w; const int32_t spp = f.spp;
   const bool views = f.kind == Query::kViews;
   if (!p || !p->dev.nodes) { set_error(ctx, "render: invalid prepared scene"); return 1; }
-  if (h <= 0 || w <= 0 || h > 65536 || w > 65536 || ((h + 3) / 4) * ((w + 7) / 8) > ((int64_t)1 << 25)) {
-    // work items are 32-bit: at most 2^30 (padded) pixels per frame
+  if (!image_size_ok(h, w)) {
     set_error(ctx, "render: bad image size %lldx%lld", (long long)h, (long long)w);
     return 1;
   }
@@ -132,7 +136,7 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   if (f.world < 1 || f.rank < 0 || f.rank >= f.world) { set_error(ctx, "render: bad shard %d/%d", f.rank, f.world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
   const int32_t s_begin = f.kind == Query::kAccumulate ? f.q.s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
-  const bool adaptive = f.kind == Query::kAdaptive;
+  const bool adaptive = f.kind == Query::kAdaptive || f.kind == Query::kAdaptiveVar;
   if (!adaptive && ensure_offsets(ctx, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
@@ -388,7 +392,7 @@ static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64
 // One frame on one lane (api_internal.h).  Query::kAccumulate, a chunk of a progressive frame, is launched without a
 // claim-order pass (see below); Query::kViews, with the camera table f.q.cams in device memory, without the learned order;
 // Query::kAdaptive, with its selection list f.q.sel / f.q.n_sel in device memory, as two launches: the selection pass, then
-// the render kernel, without a claim-order pass either.
+// the render kernel, without a claim-order pass either; Query::kAdaptiveVar as kAdaptive.
 int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff) {
   futhark_context::Lane &L = ctx->lane(lane_id);
   if (f.tile_major) {  // ranks that own one tile fewer than the padded count leave a zeroed tail (before the timing events)
@@ -421,7 +425,8 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   // order, and it leaves the scene's learned order as it found it (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = f.kind != Query::kAccumulate && f.kind != Query::kAdaptive && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool adaptive = f.kind == Query::kAdaptive || f.kind == Query::kAdaptiveVar;
+  const bool heavy_first = f.kind != Query::kAccumulate && !adaptive && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -481,7 +486,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   P.frame_flag = (ff && self_signal) ? ff->done_flag : nullptr;
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
   if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, f.kind, f.q);
-  if (f.kind == Query::kAdaptive) {
+  if (adaptive) {
     CUDA_TRY(ctx, cudaMemsetAsync(f.q.n_sel, 0, sizeof(int32_t), L.stream));
     launch_adaptive_select(P, f.q, L.stream, &ctx->launches);
   }
@@ -590,20 +595,26 @@ int ray_b200_render_accumulate(struct futhark_context *ctx, float *accum_dev, in
   return render_frame(ctx, f);
 }
 
-int ray_b200_render_adaptive(struct futhark_context *ctx, float *accum_dev, int32_t *counts_dev, const uint8_t *mask_dev,
-                             int64_t h, int64_t w, int32_t n_add, int32_t *out_pix_dev, float *out_rgb_dev,
-                             const struct futhark_opaque_prepared_scene *p) {
+}  // extern "C"
+
+// ray_b200_render_adaptive (m2_dev == NULL, Query::kAdaptive) and ray_b200_render_adaptive_var (Query::kAdaptiveVar),
+// whose errors carry the name `what`
+static int render_adaptive(struct futhark_context *ctx, float *accum_dev, float *m2_dev, int32_t *counts_dev,
+                           const uint8_t *mask_dev, int64_t h, int64_t w, int32_t n_add, int32_t *out_pix_dev,
+                           float *out_rgb_dev, const struct futhark_opaque_prepared_scene *p, bool var, const char *what) {
   if (bad_ctx(ctx)) return 1;
   std::lock_guard<std::mutex> g(ctx->mu);
-  if (!ctx->peers.empty()) { set_error(ctx, "render_adaptive: not available on a single-process multi-GPU context (RAY_GPUS > 1)"); return 1; }
-  if (ctx->cfg.world > 1) { set_error(ctx, "render_adaptive: not available with a shard set (rank %d of %d)", ctx->cfg.rank, ctx->cfg.world); return 1; }
-  if (n_add < 1) { set_error(ctx, "render_adaptive: n_add must be >= 1, got %d", n_add); return 1; }
-  if (!accum_dev) { set_error(ctx, "render_adaptive: accum_dev is required"); return 1; }
-  if (!counts_dev) { set_error(ctx, "render_adaptive: counts_dev is required"); return 1; }
+  if (!ctx->peers.empty()) { set_error(ctx, "%s: not available on a single-process multi-GPU context (RAY_GPUS > 1)", what); return 1; }
+  if (ctx->cfg.world > 1) { set_error(ctx, "%s: not available with a shard set (rank %d of %d)", what, ctx->cfg.rank, ctx->cfg.world); return 1; }
+  if (n_add < 1) { set_error(ctx, "%s: n_add must be >= 1, got %d", what, n_add); return 1; }
+  if (!accum_dev) { set_error(ctx, "%s: accum_dev is required", what); return 1; }
+  if (var && !m2_dev) { set_error(ctx, "%s: m2_dev is required", what); return 1; }
+  if (!counts_dev) { set_error(ctx, "%s: counts_dev is required", what); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
   Frame f{p, h, w, n_add, 0, 1, out_pix_dev, out_rgb_dev};
-  f.kind = Query::kAdaptive;
+  f.kind = var ? Query::kAdaptiveVar : Query::kAdaptive;
   f.q.accum = accum_dev;
+  f.q.m2 = m2_dev;
   f.q.sample_counts = counts_dev;
   f.q.mask = mask_dev;
   RenderParams P;
@@ -617,8 +628,49 @@ int ray_b200_render_adaptive(struct futhark_context *ctx, float *accum_dev, int3
   f.q.sel = sel + 1;
   int rc = do_render(ctx, f, P, lc);
   const cudaError_t fe = cudaFreeAsync(sel, ctx->stream);
-  if (!rc && fe != cudaSuccess) { set_error(ctx, "render_adaptive: %s", cudaGetErrorString(fe)); rc = 1; }
+  if (!rc && fe != cudaSuccess) { set_error(ctx, "%s: %s", what, cudaGetErrorString(fe)); rc = 1; }
   return rc;
+}
+
+extern "C" {
+
+int ray_b200_render_adaptive(struct futhark_context *ctx, float *accum_dev, int32_t *counts_dev, const uint8_t *mask_dev,
+                             int64_t h, int64_t w, int32_t n_add, int32_t *out_pix_dev, float *out_rgb_dev,
+                             const struct futhark_opaque_prepared_scene *p) {
+  return render_adaptive(ctx, accum_dev, nullptr, counts_dev, mask_dev, h, w, n_add, out_pix_dev, out_rgb_dev, p, false,
+                         "render_adaptive");
+}
+
+int ray_b200_render_adaptive_var(struct futhark_context *ctx, float *accum_dev, float *m2_dev, int32_t *counts_dev,
+                                 const uint8_t *mask_dev, int64_t h, int64_t w, int32_t n_add, int32_t *out_pix_dev,
+                                 float *out_rgb_dev, const struct futhark_opaque_prepared_scene *p) {
+  return render_adaptive(ctx, accum_dev, m2_dev, counts_dev, mask_dev, h, w, n_add, out_pix_dev, out_rgb_dev, p, true,
+                         "render_adaptive_var");
+}
+
+int ray_b200_adaptive_select(struct futhark_context *ctx, const float *accum_dev, const float *m2_dev, const int32_t *counts_dev,
+                             int64_t h, int64_t w, float rel_err, float mean_floor, int32_t min_count, int32_t max_count,
+                             uint8_t *mask_dev, int32_t *n_selected_dev) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!image_size_ok(h, w)) { set_error(ctx, "adaptive_select: bad image size %lldx%lld", (long long)h, (long long)w); return 1; }
+  if (!accum_dev || !m2_dev || !counts_dev || !mask_dev) {
+    set_error(ctx, "adaptive_select: accum_dev, m2_dev, counts_dev and mask_dev are required");
+    return 1;
+  }
+  if (!(std::isfinite(rel_err) && rel_err >= 0.0f)) { set_error(ctx, "adaptive_select: rel_err must be finite and >= 0, got %g", (double)rel_err); return 1; }
+  if (!(std::isfinite(mean_floor) && mean_floor >= 0.0f)) {
+    set_error(ctx, "adaptive_select: mean_floor must be finite and >= 0, got %g", (double)mean_floor);
+    return 1;
+  }
+  if (min_count < 2) { set_error(ctx, "adaptive_select: min_count must be >= 2 (the variance needs two samples), got %d", min_count); return 1; }
+  if (max_count < min_count) { set_error(ctx, "adaptive_select: max_count %d is below min_count %d", max_count, min_count); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (n_selected_dev) CUDA_TRY(ctx, cudaMemsetAsync(n_selected_dev, 0, sizeof(int32_t), ctx->stream));
+  launch_adaptive_error_select(accum_dev, m2_dev, counts_dev, h * w, rel_err, mean_floor, min_count, max_count, mask_dev,
+                               n_selected_dev, ctx->stream, &ctx->launches);
+  CUDA_TRY(ctx, cudaGetLastError());
+  return 0;
 }
 
 int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,

@@ -439,6 +439,7 @@ cudaError_t with_query(F &&f, Query q) {
     case Query::kAccumulate: return f(std::integral_constant<Query, Query::kAccumulate>{});
     case Query::kViews: return f(std::integral_constant<Query, Query::kViews>{});
     case Query::kAdaptive: return f(std::integral_constant<Query, Query::kAdaptive>{});
+    case Query::kAdaptiveVar: return f(std::integral_constant<Query, Query::kAdaptiveVar>{});
     default: return cudaErrorInvalidValue;
   }
 }

@@ -121,6 +121,13 @@ __device__ __forceinline__ void write_adaptive_pixel(const RenderParams &P, cons
   }
 }
 
+// Query::kAdaptiveVar: Welford's update of a channel's M2 by sample k >= 1 of the pixel, x, where s_old is the f32 sum of
+// samples [0, k) and s_new = s_old + x (include/ray_b200.h ray_b200_render_adaptive_var).  IEEE divisions; -fmad=false
+// keeps the product and the sum apart.
+__device__ __forceinline__ float welford_m2(const float m2, const float x, const float s_old, const float s_new, const int k) {
+  return m2 + (x - s_old / (float)k) * (x - s_new / (float)(k + 1));
+}
+
 // The selection pass.
 // Query::kAdaptive: the work items of the selected pixels, in claim order.  Thread c walks claim c of the frame's claim
 // sequence (the plain chunk permutation: an adaptive launch has no heavy-first or learned order) and keeps its item when it
@@ -149,6 +156,37 @@ __global__ void __launch_bounds__(256) select_pixels_kernel(const __grid_constan
   if (lane == 0) base = atomicAdd(Q.n_sel, __popc(b));
   base = __shfl_sync(kFullMask, base, 0);
   if (keep) Q.sel[base + __popc(b & ((1u << lane) - 1u))] = item;
+}
+
+// ray_b200_adaptive_select: pixel p is selected when 0 <= n < max_count for its count n, and n < min_count or its error
+// estimate E (the three channels' variances of the mean, summed) is above the target T; the arithmetic and its order are
+// include/ray_b200.h's.  accum and m2 are read only where min_count <= n < max_count.  One ballot and one atomicAdd per
+// warp count the ones into *n_selected.  64-bit offsets: 3 * n_px floats pass 2^32 bytes at 2^30 pixels.
+__global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__restrict__ accum, const float *__restrict__ m2,
+                                                              const int32_t *__restrict__ counts, const long long n_px,
+                                                              const float rel_err, const float mean_floor, const int min_count,
+                                                              const int max_count, uint8_t *__restrict__ mask,
+                                                              int32_t *__restrict__ n_selected) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  bool sel = false;
+  if (p < n_px) {
+    const int n = counts[p];
+    if (n >= 0 && n < max_count) {
+      if (n < min_count) {
+        sel = true;
+      } else {
+        const float *S = accum + 3 * (size_t)p, *M = m2 + 3 * (size_t)p;
+        const float v = (M[0] + M[1]) + M[2];
+        const float e = v / ((float)n * (float)(n - 1));
+        const float m = ((S[0] + S[1]) + S[2]) / (float)n + mean_floor;
+        const float t = (rel_err * m) * (rel_err * m);
+        sel = e > t;  // (NaN: not selected)
+      }
+    }
+    mask[p] = sel ? 1 : 0;
+  }
+  const unsigned b = __ballot_sync(kFullMask, sel);
+  if (n_selected && b && (threadIdx.x & 31) == 0) atomicAdd(n_selected, __popc(b));
 }
 
 // ====================================================================================== K3: warp work-queue
@@ -248,6 +286,13 @@ __global__ void __launch_bounds__(256) select_pixels_kernel(const __grid_constan
 // (there is no table of them: the host does not know the counts), the in-order sum starts from Q.accum where c_p > 0, and
 // the owner writes the pixel scaled by 1 / (c_p + n_add), then stores the sum and the count.  c_p is read from
 // Q.sample_counts wherever it is needed; only the pixel's owner writes it, once its last sample has been added.
+//
+// Query::kAdaptiveVar is Query::kAdaptive (kAdapt is true for both) that also carries each pixel's M2 in Q.m2, one
+// welford_m2 step per sample in sample order, next to the in-order sum that already has the old and new sums in hand.
+// Pixel-bound samples: the slot owns the pixel for all its samples, so finish_path reads, updates and writes Q.m2 at the
+// pixel once per finished sample (+0 after the pixel's sample 0).  Spread samples: the lane of a ring entry that sums one
+// channel over cbuf runs that channel's M2 chain in the same loop, from Q.m2 where the count is above 0, and stores it.
+// No shared memory is added, so the plan, the staging and wq_warp_bytes are those of Query::kAdaptive.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -263,7 +308,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   constexpr bool kRays = is_ray_query(kQuery);  // ray mode
-  constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews, kAdapt = kQuery == Query::kAdaptive;
+  constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews;
+  constexpr bool kVar = kQuery == Query::kAdaptiveVar, kAdapt = kQuery == Query::kAdaptive || kVar;
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -330,6 +376,8 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   [[maybe_unused]] auto accum_of = [&](const int pi, const int pj) { return Q.accum + 3 * ((size_t)pj * P.W + pi); };
   // kAdapt: the sample count of pixel (row pj, column pi)
   [[maybe_unused]] auto count_of = [&](const int pi, const int pj) { return Q.sample_counts + ((size_t)pj * P.W + pi); };
+  // kVar: the M2 of pixel (row pj, column pi), laid out as its sum
+  [[maybe_unused]] auto m2_of = [&](const int pi, const int pj) { return Q.m2 + 3 * ((size_t)pj * P.W + pi); };
   // pixel item -> (view, column, row), false for a padding pixel; the view is 0 unless kViews
   auto pixel_of = [&](const int item, int &pv, int &pi, int &pj) {
     if constexpr (kViews) return item_view_pixel(P, item, pv, pi, pj);
@@ -368,6 +416,17 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       int32_t *cnt = count_of(pi, pj);
       const int c = *cnt;
       const V3 sum = (s == 0 && c == 0) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
+      if constexpr (kVar) {  // sample c + s of the pixel: +0 after sample 0, then one Welford step per sample
+        float *m = m2_of(pi, pj);
+        const int k = c + s;
+        if (k == 0) {
+          m[0] = 0.0f; m[1] = 0.0f; m[2] = 0.0f;
+        } else {
+          m[0] = welford_m2(m[0], colour.x, ps.x, sum.x, k);
+          m[1] = welford_m2(m[1], colour.y, ps.y, sum.y, k);
+          m[2] = welford_m2(m[2], colour.z, ps.z, sum.z, k);
+        }
+      }
       s++;
       if (s < spp) {
         const Ray nr = adaptive_ray(P, pi, pj, c + s);
@@ -488,14 +547,27 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
           // never a padding pixel)
           int s = 1, pi, pj;
           item_pixel(P, ring_item[m], pi, pj);
-          if (*count_of(pi, pj) > 0) {
+          const int cp = *count_of(pi, pj);
+          float m2 = 0.0f;  // kVar: this channel's M2, +0 after the pixel's sample 0
+          if (cp > 0) {
             sum = accum_of(pi, pj)[ch];
+            if constexpr (kVar) m2 = m2_of(pi, pj)[ch];
             s = 0;
           } else {
             sum = __ldcg(c);
           }
+          if constexpr (kVar) {
 #pragma unroll 4
-          for (; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+            for (; s < spp; s++) {
+              const float x = __ldcg(c + 4 * s), next = sum + x;
+              m2 = welford_m2(m2, x, sum, next, cp + s);
+              sum = next;
+            }
+            m2_of(pi, pj)[ch] = m2;
+          } else {
+#pragma unroll 4
+            for (; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+          }
         } else if constexpr (kAccum) {
           // a later chunk adds its samples to the running sum of the earlier ones, the first chunk starts at its sample 0
           int s = 1, pi, pj;
@@ -1098,8 +1170,8 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
       }, k == 2, all_nodes, sph, ranged);
     else
       return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-        // (kAdaptive is not built for every sphere staged without every node, which split_staging never plans)
-        if constexpr (query == Query::kAdaptive && s && !a) return cudaErrorInvalidValue;
+        // (kAdaptive and kAdaptiveVar are not built for every sphere staged without every node, which split_staging never plans)
+        if constexpr ((query == Query::kAdaptive || query == Query::kAdaptiveVar) && s && !a) return cudaErrorInvalidValue;
         else
           return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(
               lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);
@@ -1147,6 +1219,14 @@ void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStr
 void launch_adaptive_select(const RenderParams &p, const RayQuery &q, cudaStream_t stream, int64_t *launches) {
   const long long claims = (long long)p.n_chunks << 11;
   select_pixels_kernel<<<(unsigned)((claims + 255) / 256), 256, 0, stream>>>(p, q);
+  (*launches)++;
+}
+
+void launch_adaptive_error_select(const float *accum, const float *m2, const int32_t *counts, int64_t n_px, float rel_err,
+                                  float mean_floor, int32_t min_count, int32_t max_count, uint8_t *mask, int32_t *n_selected,
+                                  cudaStream_t stream, int64_t *launches) {
+  adaptive_select_kernel<<<(unsigned)((n_px + 255) / 256), 256, 0, stream>>>(accum, m2, counts, n_px, rel_err, mean_floor,
+                                                                          min_count, max_count, mask, n_selected);
   (*launches)++;
 }
 

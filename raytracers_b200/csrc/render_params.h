@@ -64,9 +64,10 @@ struct RenderParams {
 // (include/ray_b200.h "ray queries"; rays, n, perm, t_min, t_max): kClosest, to their closest hit (hits) or along their
 // path (rgb, segments, max_depth; hits == NULL tells the two apart at run time); kAnyHit, to their first accepted sphere
 // (occluded); kMultiHit, to their k nearest ones (hits, k, counts).  kAdaptive, a pixel kind: the selected pixels of a
-// progressive frame, each from its own sample count (accum, sample_counts, mask, sel, n_sel).  New kinds go at the end:
-// kernel names carry the values, and tools/sass_compare.py reads older builds' names by them.
-enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive };
+// progressive frame, each from its own sample count (accum, sample_counts, mask, sel, n_sel).  kAdaptiveVar: kAdaptive
+// that also keeps each pixel's running sum of squared deviations (m2).  New kinds go at the end: kernel names carry the
+// values, and tools/sass_compare.py reads older builds' names by them.
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar };
 __host__ __device__ constexpr bool is_ray_query(Query q) {
   return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
 }
@@ -107,6 +108,9 @@ struct RayQuery {
   const uint8_t *mask;
   int32_t *sel;
   int32_t *n_sel;
+  // Query::kAdaptiveVar (include/ray_b200.h ray_b200_render_adaptive_var): row-major [H][W][3], each pixel's M2, Welford's
+  // running f32 sum of squared deviations from the mean of its samples (not read where its count is 0)
+  float *m2;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
@@ -149,8 +153,8 @@ struct LaunchConfig {
   long long stage_budget;  // warp-queue kernel: shared memory its queues leave for staging, before cap_staging (bytes)
 };
 
-// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate, kViews and kAdaptive, which
-// read q, on the warp-queue kernel only
+// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate, kViews, kAdaptive and
+// kAdaptiveVar, which read q, on the warp-queue kernel only
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches, Query kind, const RayQuery &q);
 // The warp-queue kernel (render_kernels.cu): a launch of kind `kind`, a pixel kind or a ray query (whatever lc.kernel
@@ -178,6 +182,11 @@ inline int tile_order_key_bits(int32_t n_chunks) {  // keys are positions < n_ch
 }
 // Query::kAdaptive: the selection pass in front of the render kernel (q.sel, q.n_sel; *q.n_sel zeroed by the caller)
 void launch_adaptive_select(const RenderParams &p, const RayQuery &q, cudaStream_t stream, int64_t *launches);
+// ray_b200_adaptive_select (include/ray_b200.h): the noise rule over n_px pixels, mask[p] = 0 / 1, and the number of ones
+// added to *n_selected where it is not NULL (zeroed by the caller)
+void launch_adaptive_error_select(const float *accum, const float *m2, const int32_t *counts, int64_t n_px, float rel_err,
+                                  float mean_floor, int32_t min_count, int32_t max_count, uint8_t *mask, int32_t *n_selected,
+                                  cudaStream_t stream, int64_t *launches);
 // of a frame of pixel kind `kind`: Query::kViews probes each tile with its view's camera (q.cams)
 void launch_tile_order(const RenderParams &p, const TileOrderBuffers &b, cudaStream_t stream, int64_t *launches, Query kind,
                        const RayQuery &q);
