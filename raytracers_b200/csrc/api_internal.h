@@ -174,15 +174,14 @@ int resolve_kernel(const futhark_context *ctx);
 struct Frame {
   const futhark_opaque_prepared_scene *scene = nullptr;
   int64_t h = 0, w = 0;
-  int32_t spp = 1;             // the samples of this launch (kAccumulate: of this chunk)
+  int32_t spp = 1;             // the samples of this launch (progressive kinds: added to each pixel)
   int32_t rank = 0, world = 1;
   int32_t *out_pix = nullptr;
   float *out_rgb = nullptr;
   bool tile_major = false;     // out_pix holds this rank's tiles, padded to ray_b200_shard_tiles_padded (do_render zeroes the tail)
-  Query kind = Query::kPixels; // a pixel kind: kAccumulate (ray_b200_render_accumulate), kViews (ray_b200_render_views_into),
-                               // kAdaptive (ray_b200_render_adaptive), kAdaptiveVar (ray_b200_render_adaptive_var)
-  RayQuery q{};                // kAccumulate: accum, s_begin.  kViews: n_views, and cams once uploaded (view_tiles: fill_params).
-                               // kAdaptive: accum, sample_counts, mask, and sel / n_sel once allocated.  kAdaptiveVar: those and m2
+  Query kind = Query::kPixels; // a pixel kind (render_params.h Query)
+  RayQuery q{};                // the fields of q that kind reads (render_params.h RayQuery); fill_params sets view_tiles,
+                               // the adaptive entry point sel / n_sel once allocated
 };
 // The parameter block of frame f and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
 // slots, ...), which the caller hands to do_render with f; sets f.q.view_tiles of a kViews frame.

@@ -109,15 +109,12 @@ static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
   return need <= kSpreadBudget ? need : 0;
 }
 
-// Fills the kernel parameter block for frame f, and the frame's launch plan.  Query::kAccumulate: the launch is one
-// chunk of a progressive frame: spp samples from q.s_begin on, planned as a frame of spp samples (spread or pixel-bound
-// by the chunk length), read from the offset table of the whole frame at the chunk's first sample and scaled by
-// 1/s_end; it runs on the warp-queue kernel whatever the context's kernel is.  Query::kViews: the launch renders
-// q.n_views frames of h x w: its work items are the tiles of all of them, so the plan (spread or pixel-bound, K,
-// staging, the sample buffer) is that of one frame of n_views x tiles(h, w) tiles; it runs on the warp-queue kernel too.
-// Query::kAdaptive: the launch adds spp = n_add samples to the selected pixels, planned as a frame of n_add samples over all
-// tiles (an upper bound on its work: the selection is on the device); each pixel's sample offsets are computed by the
-// kernel, so no offset table is made; on the warp-queue kernel too.  Query::kAdaptiveVar is planned as kAdaptive.
+// Fills the kernel parameter block for frame f, and the frame's launch plan.  Every kind but kPixels runs on the warp-queue
+// kernel whatever the context's kernel is, planned as a frame of f.spp samples (spread or pixel-bound by that count).
+// Query::kAccumulate reads the offset table of the whole frame from the chunk's first sample on and scales by 1/s_end.
+// Query::kViews: the work items are the tiles of all q.n_views frames, so the plan (K, staging, the sample buffer) is
+// that of one frame of n_views x tiles(h, w) tiles.  The adaptive kinds are planned over all tiles, an upper bound on
+// their work (the selection is on the device).
 int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc) {
   const futhark_opaque_prepared_scene *p = f.scene;
   const int64_t h = f.h, w = f.w; const int32_t spp = f.spp;
@@ -136,7 +133,7 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   if (f.world < 1 || f.rank < 0 || f.rank >= f.world) { set_error(ctx, "render: bad shard %d/%d", f.rank, f.world); return 1; }
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
   const int32_t s_begin = f.kind == Query::kAccumulate ? f.q.s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
-  const bool adaptive = f.kind == Query::kAdaptive || f.kind == Query::kAdaptiveVar;
+  const bool adaptive = is_adaptive(f.kind);
   if (!adaptive && ensure_offsets(ctx, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
@@ -389,10 +386,9 @@ static int plan_tile_order(futhark_context *ctx, futhark_context::Lane &L, int64
   return 0;
 }
 
-// One frame on one lane (api_internal.h).  Query::kAccumulate, a chunk of a progressive frame, is launched without a
-// claim-order pass (see below); Query::kViews, with the camera table f.q.cams in device memory, without the learned order;
-// Query::kAdaptive, with its selection list f.q.sel / f.q.n_sel in device memory, as two launches: the selection pass, then
-// the render kernel, without a claim-order pass either; Query::kAdaptiveVar as kAdaptive.
+// One frame on one lane (api_internal.h).  The progressive kinds are launched without a claim-order pass (see below);
+// Query::kViews, with the camera table f.q.cams in device memory, without the learned order; the adaptive kinds, with
+// their selection list f.q.sel / f.q.n_sel in device memory, as two launches: the selection pass, then the render kernel.
 int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const LaunchConfig &lc, int lane_id, bool timed, const FrameFlags *ff) {
   futhark_context::Lane &L = ctx->lane(lane_id);
   if (f.tile_major) {  // ranks that own one tile fewer than the padded count leave a zeroed tail (before the timing events)
@@ -421,12 +417,10 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   }
   // heavy-first claim order (warp-queue kernel): worth its probe pass when a frame is long enough to have a tail to lose
   // — more than one sample per pixel — and pointless when every tile is claimed in the first wave anyway.
-  // A chunk of a progressive frame uses neither this nor the learned order below: it is one launch in the plain permuted
-  // order, and it leaves the scene's learned order as it found it (DESIGN.md, progressive rendering).  A views launch
+  // A progressive launch uses neither this nor the learned order below (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool adaptive = f.kind == Query::kAdaptive || f.kind == Query::kAdaptiveVar;
-  const bool heavy_first = f.kind != Query::kAccumulate && !adaptive && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = !is_progressive(f.kind) && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -486,7 +480,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   P.frame_flag = (ff && self_signal) ? ff->done_flag : nullptr;
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
   if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, f.kind, f.q);
-  if (adaptive) {
+  if (is_adaptive(f.kind)) {
     CUDA_TRY(ctx, cudaMemsetAsync(f.q.n_sel, 0, sizeof(int32_t), L.stream));
     launch_adaptive_select(P, f.q, L.stream, &ctx->launches);
   }

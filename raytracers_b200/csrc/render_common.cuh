@@ -189,13 +189,21 @@ __device__ __forceinline__ Ray camera_ray(const float *c, const float u, const f
 // get_ray for sample s of pixel (row j, column i): ray.fut:150-154 with pixel j i -> trace_ray (height-j) i
 // (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).  Query::kAccumulate (a chunk of a
 // progressive frame): s is relative to the chunk, P.offsets starts at its first sample and is read even when P.spp == 1;
-// at s = 0 of the frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  Query::kViews:
-// the camera is view_cam, the pixel's view's 12 floats of RayQuery::cams, instead of P.cam.
+// at s = 0 of the frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  The adaptive
+// kinds: s is relative to the pixel's own first sample c, and the offsets of its sample c + s are computed here exactly as
+// sample_offsets computes them on the host (the same f32 products, floorf and differences; -fmad=false keeps them apart):
+// each pixel continues from its own count, so there is no one table for the launch.  Query::kViews: the camera is
+// view_cam, the pixel's view's 12 floats of RayQuery::cams, instead of P.cam.
 template <Query kKind = Query::kPixels>
-__device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s, const float *view_cam = nullptr) {
+__device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s, const float *view_cam = nullptr,
+                                           int c = 0) {
   constexpr bool kAccum = kKind == Query::kAccumulate, kViews = kKind == Query::kViews;
   float u, v;
-  if (!kAccum && P.spp == 1) {
+  if constexpr (is_adaptive(kKind)) {
+    const float a = (float)(c + s) * 0.7548776662f, b = (float)(c + s) * 0.5698402909f;
+    u = ((float)i + (a - floorf(a))) / (float)P.W;
+    v = ((float)(P.H - j) + (b - floorf(b))) / (float)P.H;
+  } else if (!kAccum && P.spp == 1) {
     u = (float)i / (float)P.W;
     v = (float)(P.H - j) / (float)P.H;
   } else {
@@ -255,25 +263,25 @@ __device__ __forceinline__ int claim_to_item(const RenderParams &P, int c) {
 }
 
 // Query::kAccumulate: the sum of a progressive frame's samples [0, s_end), always scaled by P.inv_spp = 1/s_end (1 * x = x
-// when s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only).  Query::kViews: pixel (i, j) of
-// view `view`, whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the float frames 12 GiB)
+// when s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only).  The adaptive kinds: as
+// kAccumulate, with s_end = n, the pixel's own sample count after the launch.  Query::kViews: pixel (i, j) of view `view`,
+// whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the float frames 12 GiB)
 template <Query kKind = Query::kPixels>
-__device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum, int view = 0) {
-  constexpr bool kAccum = kKind == Query::kAccumulate, kViews = kKind == Query::kViews;
-  const V3 col = (!kAccum && P.spp == 1) ? sum : vscale(P.inv_spp, sum);
+__device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum, int view = 0, int n = 0) {
+  constexpr bool kProg = is_progressive(kKind), kViews = kKind == Query::kViews;
+  const float inv = is_adaptive(kKind) ? 1.0f / (float)n : P.inv_spp;
+  const V3 col = (!kProg && P.spp == 1) ? sum : vscale(inv, sum);
   const int pix = pack_pixel(col);
-  if constexpr (kViews) {
-    const size_t px = (size_t)view * (size_t)P.H * (size_t)P.W + (size_t)j * P.W + i;
-    P.out_pix[px] = pix;
+  if constexpr (kViews || kProg) {  // row-major frames: one offset for both stores (views always write pixels)
+    const size_t px = (kViews ? (size_t)view * (size_t)P.H * (size_t)P.W : 0) + (size_t)j * P.W + i;
+    if (kViews || P.out_pix) P.out_pix[px] = pix;
     if (P.out_rgb) {
       float *q = P.out_rgb + 3 * px;
       q[0] = col.x; q[1] = col.y; q[2] = col.z;
     }
     return;
   }
-  if constexpr (kAccum) {
-    if (P.out_pix) P.out_pix[(size_t)j * P.W + i] = pix;
-  } else if (P.tile_major) {
+  if (P.tile_major) {
     P.out_pix[k] = pix;
   } else {
     P.out_pix[(size_t)j * P.W + i] = pix;

@@ -98,29 +98,6 @@ __global__ void __launch_bounds__(256) tile_cost_keys_kernel(const __grid_consta
 }
 
 // ====================================================================================== adaptive progressive rendering
-// Query::kAdaptive: get_ray for sample s of pixel (row j, column i), as primary_ray makes it for a frame of more than one
-// sample, except that the offsets of sample s are computed here, exactly as sample_offsets computes them on the host (the
-// same f32 products, floorf and differences; -fmad=false keeps them apart): each pixel continues from its own count, so
-// there is no one table for the launch.
-__device__ __forceinline__ Ray adaptive_ray(const RenderParams &P, const int i, const int j, const int s) {
-  const float a = (float)s * 0.7548776662f, b = (float)s * 0.5698402909f;
-  const float u = ((float)i + (a - floorf(a))) / (float)P.W;
-  const float v = ((float)(P.H - j) + (b - floorf(b))) / (float)P.H;
-  return camera_ray(P.cam, u, v);
-}
-
-// Query::kAdaptive: the pixel (row j, column i) of sum at spp = n, where inv = 1 / n: written as write_pixel writes a
-// progressive frame's (row-major, each output optional)
-__device__ __forceinline__ void write_adaptive_pixel(const RenderParams &P, const int i, const int j, const V3 sum, const float inv) {
-  const V3 col = vscale(inv, sum);
-  const size_t px = (size_t)j * P.W + i;
-  if (P.out_pix) P.out_pix[px] = pack_pixel(col);
-  if (P.out_rgb) {
-    float *q = P.out_rgb + 3 * px;
-    q[0] = col.x; q[1] = col.y; q[2] = col.z;
-  }
-}
-
 // Query::kAdaptiveVar: Welford's update of a channel's M2 by sample k >= 1 of the pixel, x, where s_old is the f32 sum of
 // samples [0, k) and s_new = s_old + x (include/ray_b200.h ray_b200_render_adaptive_var).  IEEE divisions; -fmad=false
 // keeps the product and the sum apart.
@@ -220,7 +197,7 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // ORDER when its last sample lands, which keeps the result bit-identical to the sequential definition.
 //
 // The kind (kQuery, render_params.h Query) says what is traced.  The pixel kinds trace camera rays, as above:
-// Query::kPixels a whole frame (Q is unused), Query::kAccumulate and Query::kViews as described at the end.  The other
+// Query::kPixels a whole frame (Q is unused), the other pixel kinds as described at the end.  The other
 // kinds are ray queries (include/ray_b200.h "ray queries"), "ray mode" below: the work items are the caller's rays
 // instead of pixels.  A claim c is ray c (no tile order), a slot is filled from Q.rays, and boxes are
 // tested against the query's (t_min, t_max) instead of the literal (0, 1e9).  Rays of a batch are not coherent: ray mode
@@ -260,39 +237,25 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // to ray_d.w (the leaf batch loads ray_d).  Ranged variants exist only as a separate template instantiation, so the
 // per-call variants keep their code.
 //
-// Query::kAccumulate, one chunk of a progressive frame (include/ray_b200.h ray_b200_render_accumulate): the launch traces
-// samples [Q.s_begin, Q.s_begin + P.spp) of every pixel.  Everything that counts samples is chunk-relative: P.spp is the
-// chunk length (it sizes cbuf and bounds p_ms's 16-bit sample, as spp does for a whole frame), P.offsets starts at the
-// chunk's first sample and is read for every sample (primary_ray<Query::kAccumulate>), and sample rel of the chunk is
-// sample s_begin + rel of the frame.  Q.accum holds each pixel's f32 sum of samples [0, s_begin): with s_begin > 0 the
-// in-order sum starts from it (p_sum at the pixel-bound refill, the first term of finalize_pixels), with s_begin == 0 from
-// sample 0's colour itself, as in a whole frame.  Where the pixel is written (scaled by P.inv_spp = 1/s_end,
-// write_pixel<Query::kAccumulate>), its owner stores the new sum back to Q.accum in place.  So a chain of chunks computes
-// the same f32 additions in the same order as one frame of s_end samples.
+// The progressive kinds add the P.spp samples [c, c + P.spp) that follow each pixel's first sample c of the launch
+// (first_sample) to its running f32 sum in Q.accum: Query::kAccumulate, one chunk of a progressive frame (include/ray_b200.h
+// ray_b200_render_accumulate), the same c = Q.s_begin for every pixel; Query::kAdaptive (ray_b200_render_adaptive), the
+// selected pixels, each from its own count.  Everything that counts samples in the kernel is launch-relative: P.spp sizes
+// cbuf and bounds p_ms's 16-bit sample as it does for a whole frame.  A chain of launches computes the same f32 additions
+// in the same order as one frame of c + P.spp samples.  The adaptive kinds' work items are not the frame's tiles but the
+// list the selection pass (select_pixels_kernel) made in front of the launch: claim c is item Q.sel[c], for c < *Q.n_sel.
+// Their sample offsets are computed per sample (primary_ray): the host does not know the counts.
 //
-// Query::kViews, several views in one launch (include/ray_b200.h ray_b200_render_views_into): the launch renders
-// Q.n_views frames of one size from one prepared scene.  The work items are the tiles of all views, view after view
-// (P.n_tiles = P.local_tiles = n_views * Q.view_tiles), so the chunk permutation of the claim order mixes the views' sky
-// and ground tiles as it mixes one frame's.  Where a pixel item becomes a pixel (pixel_of: the pixel-bound refill, finish_path's next sample and store,
-// the spread dispenser and finalize_pixels) it also gives its view v; the camera ray reads view v's 12 floats of Q.cams
-// instead of P.cam, and the pixel is stored at offset v * H * W.  Nothing else depends on the view, so every view's
-// pixel sees exactly the arithmetic of a one-view frame whose P.cam is that camera.
+// Query::kViews, several views in one launch (include/ray_b200.h ray_b200_render_views_into): the work items are the tiles
+// of all views, view after view (P.n_tiles = P.local_tiles = n_views * Q.view_tiles), so the chunk permutation of the
+// claim order mixes the views' sky and ground tiles as it mixes one frame's.  pixel_of gives a pixel item's view v too;
+// the camera ray reads view v's 12 floats of Q.cams instead of P.cam, and the pixel is stored at offset v * H * W.
+// Nothing else depends on the view, so every view's pixel sees exactly the arithmetic of a one-view frame.
 //
-// Query::kAdaptive, the selected pixels of a progressive frame (include/ray_b200.h ray_b200_render_adaptive): every
-// selected pixel p gets the P.spp = n_add samples [c_p, c_p + n_add) that follow its own count c_p =
-// Q.sample_counts[p].  The work items are not the frame's tiles but the list the selection pass (select_pixels_kernel)
-// made in front of the launch: claim c is item Q.sel[c], for c < *Q.n_sel.  Everything else is Query::kAccumulate with
-// c_p in place of Q.s_begin: sample rel of the chunk is sample c_p + rel of the pixel, whose offsets adaptive_ray computes
-// (there is no table of them: the host does not know the counts), the in-order sum starts from Q.accum where c_p > 0, and
-// the owner writes the pixel scaled by 1 / (c_p + n_add), then stores the sum and the count.  c_p is read from
-// Q.sample_counts wherever it is needed; only the pixel's owner writes it, once its last sample has been added.
-//
-// Query::kAdaptiveVar is Query::kAdaptive (kAdapt is true for both) that also carries each pixel's M2 in Q.m2, one
-// welford_m2 step per sample in sample order, next to the in-order sum that already has the old and new sums in hand.
-// Pixel-bound samples: the slot owns the pixel for all its samples, so finish_path reads, updates and writes Q.m2 at the
-// pixel once per finished sample (+0 after the pixel's sample 0).  Spread samples: the lane of a ring entry that sums one
-// channel over cbuf runs that channel's M2 chain in the same loop, from Q.m2 where the count is above 0, and stores it.
-// No shared memory is added, so the plan, the staging and wq_warp_bytes are those of Query::kAdaptive.
+// Query::kAdaptiveVar is Query::kAdaptive that also carries each pixel's M2 in Q.m2, one welford_m2 step per sample in
+// sample order, next to the in-order sum that already has the old and new sums in hand: in finish_path once per finished
+// sample for pixel-bound samples, in the channel loop of finalize_pixels for spread ones.  No shared memory is added, so
+// the plan, the staging and wq_warp_bytes are those of Query::kAdaptive.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -309,7 +272,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                                                                    const __grid_constant__ RayQuery Q) {
   constexpr bool kRays = is_ray_query(kQuery);  // ray mode
   constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews;
-  constexpr bool kVar = kQuery == Query::kAdaptiveVar, kAdapt = kQuery == Query::kAdaptive || kVar;
+  constexpr bool kProg = is_progressive(kQuery), kAdapt = is_adaptive(kQuery), kVar = kQuery == Query::kAdaptiveVar;
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -372,7 +335,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   int open_seq = 0, disp_seq = 0, disp_s = 0;  // spread dispenser (warp-uniform): pixels opened / next sample to hand out
   float4 *cbuf = nullptr;                      // spread: [kWqRing][spp] finished-sample colours of this warp
   if (kSpread) cbuf = P.sample_buf + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * kWqRing * (size_t)spp;
-  // kAccum: the running sum of pixel (row pj, column pi), row-major as the frame (64-bit offsets: 2^30 pixels pass 4 GiB)
+  // kProg: the running sum of pixel (row pj, column pi), row-major as the frame (64-bit offsets: 2^30 pixels pass 4 GiB)
   [[maybe_unused]] auto accum_of = [&](const int pi, const int pj) { return Q.accum + 3 * ((size_t)pj * P.W + pi); };
   // kAdapt: the sample count of pixel (row pj, column pi)
   [[maybe_unused]] auto count_of = [&](const int pi, const int pj) { return Q.sample_counts + ((size_t)pj * P.W + pi); };
@@ -386,6 +349,24 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   };
   // kViews: the camera of view pv (its 12 floats of Q.cams)
   [[maybe_unused]] auto view_cam = [&](const int pv) -> const float * { return kViews ? Q.cams + 12 * (size_t)pv : nullptr; };
+  // The first sample c of pixel (row pj, column pi) in this launch: 0 for a whole frame or views, the chunk's first sample
+  // (kAccum), the pixel's own count (kAdapt).  Sample s of the launch is sample c + s of the pixel (primary_ray<kQuery>
+  // makes its ray), and the pixel's in-order sum continues from Q.accum exactly when c > 0; otherwise its sample 0 starts it.
+  auto first_sample = [&](const int pi, const int pj) -> int {
+    if constexpr (kAdapt) return *count_of(pi, pj);
+    return kAccum ? Q.s_begin : 0;
+  };
+  // The sum of a pixel's samples [0, c + spp) is final: the pixel is written, and kProg stores the sum back to Q.accum,
+  // kAdapt the new count too.  Only the pixel's owner writes them, once its last sample has been added.
+  auto store_pixel = [&](const int item, const int pi, const int pj, const int pv, const int c, const V3 sum) {
+    const int n = c + spp;
+    write_pixel<kQuery>(P, item, pi, pj, sum, pv, n);
+    if constexpr (kProg) {
+      float *a = accum_of(pi, pj);
+      a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
+    }
+    if constexpr (kAdapt) *count_of(pi, pj) = n;
+  };
 
   // A path in `slot` has ended with `colour`.
   auto finish_path = [&](const int slot, const V3 colour, const int segs) {
@@ -406,15 +387,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       __stcg(cbuf + (size_t)(ms >> 16) * spp + (ms & 0xffff), make_float4(colour.x, colour.y, colour.z, 0.0f));
       atomicAdd(ring_done + (ms >> 16), 1);
       p_item[slot] = -1;
-    } else if constexpr (kAdapt) {
-      // as kAccum below, from the pixel's own count c: only its sample c + 0 = 0 starts the sum, later ones add to it
+    } else {
       const int item = p_item[slot];
       const float4 ps = p_sum[slot];
       int s = __float_as_int(ps.w);
-      int pi, pj, pv;
-      pixel_of(item, pv, pi, pj);
-      int32_t *cnt = count_of(pi, pj);
-      const int c = *cnt;
+      // the pixel is decoded where its kind first needs it: the adaptive kinds read c at the pixel, the others need the
+      // pixel only for the next ray or the store (decoding it ahead of the sum reschedules their code)
+      int pi = 0, pj = 0, pv;
+      if constexpr (kAdapt) pixel_of(item, pv, pi, pj);
+      const int c = first_sample(pi, pj);
       const V3 sum = (s == 0 && c == 0) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
       if constexpr (kVar) {  // sample c + s of the pixel: +0 after sample 0, then one Welford step per sample
         float *m = m2_of(pi, pj);
@@ -428,40 +409,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         }
       }
       s++;
+      if constexpr (!kAdapt) pixel_of(item, pv, pi, pj);
       if (s < spp) {
-        const Ray nr = adaptive_ray(P, pi, pj, c + s);
+        const Ray nr = primary_ray<kQuery>(P, pi, pj, s, view_cam(pv), c);
         ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
         ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
         p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
         p_sum[slot] = make_float4(sum.x, sum.y, sum.z, __int_as_float(s));
       } else {
-        write_adaptive_pixel(P, pi, pj, sum, 1.0f / (float)(c + spp));
-        float *a = accum_of(pi, pj);
-        a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
-        *cnt = c + spp;
-        p_item[slot] = -1;
-      }
-    } else {
-      const int item = p_item[slot];
-      const float4 ps = p_sum[slot];
-      int s = __float_as_int(ps.w);
-      // (kAccum: s counts the chunk's samples; only sample 0 of the frame starts the sum, later chunks start from accum)
-      const V3 sum = (s == 0 && (!kAccum || Q.s_begin == 0)) ? colour : vadd(v3(ps.x, ps.y, ps.z), colour);
-      s++;
-      int pi, pj, pv;
-      pixel_of(item, pv, pi, pj);
-      if (s < spp) {
-        const Ray nr = primary_ray<kQuery>(P, pi, pj, s, view_cam(pv));
-        ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
-        ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
-        p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
-        p_sum[slot] = make_float4(sum.x, sum.y, sum.z, __int_as_float(s));
-      } else {
-        write_pixel<kQuery>(P, item, pi, pj, sum, pv);
-        if constexpr (kAccum) {
-          float *a = accum_of(pi, pj);
-          a[0] = sum.x; a[1] = sum.y; a[2] = sum.z;
-        }
+        store_pixel(item, pi, pj, pv, c, sum);
         p_item[slot] = -1;
       }
     }
@@ -540,70 +496,36 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     const bool ready = ring_done[m] == spp;
     if (__any_sync(kFullMask, ready)) {
       float sum = 0.0f;
+      int c = 0;  // the pixel's first sample of this launch
       if (ready && ch < 3) {
-        const float *c = reinterpret_cast<const float *>(cbuf + (size_t)m * spp) + ch;
-        if constexpr (kAdapt) {
-          // the pixel's running sum where its count is above 0, else its first sample of this call (a selected pixel is
-          // never a padding pixel)
-          int s = 1, pi, pj;
-          item_pixel(P, ring_item[m], pi, pj);
-          const int cp = *count_of(pi, pj);
-          float m2 = 0.0f;  // kVar: this channel's M2, +0 after the pixel's sample 0
-          if (cp > 0) {
-            sum = accum_of(pi, pj)[ch];
-            if constexpr (kVar) m2 = m2_of(pi, pj)[ch];
-            s = 0;
-          } else {
-            sum = __ldcg(c);
-          }
-          if constexpr (kVar) {
-#pragma unroll 4
-            for (; s < spp; s++) {
-              const float x = __ldcg(c + 4 * s), next = sum + x;
-              m2 = welford_m2(m2, x, sum, next, cp + s);
-              sum = next;
-            }
-            m2_of(pi, pj)[ch] = m2;
-          } else {
-#pragma unroll 4
-            for (; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
-          }
-        } else if constexpr (kAccum) {
-          // a later chunk adds its samples to the running sum of the earlier ones, the first chunk starts at its sample 0
-          int s = 1, pi, pj;
-          if (Q.s_begin > 0 && item_pixel(P, ring_item[m], pi, pj)) {
-            sum = accum_of(pi, pj)[ch];
-            s = 0;
-          } else {
-            sum = __ldcg(c);
-          }
-#pragma unroll 4
-          for (; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+        const float *x = reinterpret_cast<const float *>(cbuf + (size_t)m * spp) + ch;
+        // (tile padding keeps c = 0, so it never reads Q.accum; the list of an adaptive launch holds pixels only)
+        int pi, pj, pv;
+        const bool px = pixel_of(ring_item[m], pv, pi, pj);
+        if (kAdapt || px) c = first_sample(pi, pj);
+        int s = 1;
+        float m2 = 0.0f;  // kVar: this channel's M2, +0 after the pixel's sample 0
+        if (c > 0) {
+          sum = accum_of(pi, pj)[ch];
+          if constexpr (kVar) m2 = m2_of(pi, pj)[ch];
+          s = 0;
         } else {
-          sum = __ldcg(c);
-#pragma unroll 4
-          for (int s = 1; s < spp; s++) sum = sum + __ldcg(c + 4 * s);
+          sum = __ldcg(x);
         }
+#pragma unroll 4
+        for (; s < spp; s++) {
+          const float xs = __ldcg(x + 4 * s), next = sum + xs;
+          if constexpr (kVar) m2 = welford_m2(m2, xs, sum, next, c + s);
+          sum = next;
+        }
+        if constexpr (kVar) m2_of(pi, pj)[ch] = m2;
       }
       const float g = __shfl_down_sync(kFullMask, sum, 1), b = __shfl_down_sync(kFullMask, sum, 2);
       if (ready && ch == 0) {
         const int item = ring_item[m];
         int pi, pj, pv;
         if (pixel_of(item, pv, pi, pj)) {
-          if constexpr (kAdapt) {
-            int32_t *cnt = count_of(pi, pj);
-            const int cp = *cnt;
-            write_adaptive_pixel(P, pi, pj, v3(sum, g, b), 1.0f / (float)(cp + spp));
-            float *a = accum_of(pi, pj);
-            a[0] = sum; a[1] = g; a[2] = b;
-            *cnt = cp + spp;
-          } else {
-            write_pixel<kQuery>(P, item, pi, pj, v3(sum, g, b), pv);
-            if constexpr (kAccum) {
-              float *a = accum_of(pi, pj);
-              a[0] = sum; a[1] = g; a[2] = b;
-            }
-          }
+          store_pixel(item, pi, pj, pv, c, v3(sum, g, b));
         } else if (P.tile_major) {
           P.out_pix[item] = 0;
         }
@@ -669,29 +591,18 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                 p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
               } else if (item < total) {
                 if (pixel_of(item, pv, pi, pj)) {
-                  const int c0 = kAdapt ? *count_of(pi, pj) : 0;  // kAdapt: the pixel's first sample of this call
-                  const Ray r = kAdapt ? adaptive_ray(P, pi, pj, c0) : primary_ray<kQuery>(P, pi, pj, 0, view_cam(pv));
+                  const int c = first_sample(pi, pj);
+                  const Ray r = primary_ray<kQuery>(P, pi, pj, 0, view_cam(pv), c);
                   p_item[slot] = item;
                   ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                   ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
                   p_light[slot] = make_float4(1.0f, 1.0f, 1.0f, __int_as_float(0));
-                  if constexpr (kAccum) {  // a later chunk's sum starts from the running sum of the earlier ones
-                    float4 ps = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
-                    if (Q.s_begin > 0) {
-                      const float *a = accum_of(pi, pj);
-                      ps.x = a[0]; ps.y = a[1]; ps.z = a[2];
-                    }
-                    p_sum[slot] = ps;
-                  } else if constexpr (kAdapt) {  // ... and from the pixel's own running sum where its count is above 0
-                    float4 ps = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
-                    if (c0 > 0) {
-                      const float *a = accum_of(pi, pj);
-                      ps.x = a[0]; ps.y = a[1]; ps.z = a[2];
-                    }
-                    p_sum[slot] = ps;
-                  } else {
-                    p_sum[slot] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
+                  float4 ps = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0));
+                  if (c > 0) {
+                    const float *a = accum_of(pi, pj);
+                    ps.x = a[0]; ps.y = a[1]; ps.z = a[2];
                   }
+                  p_sum[slot] = ps;
                 } else if (P.tile_major) {
                   P.out_pix[item] = 0;
                 }
@@ -731,7 +642,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               const int item = ring_item[m];
               int pi, pj, pv;
               if (pixel_of(item, pv, pi, pj)) {
-                const Ray r = kAdapt ? adaptive_ray(P, pi, pj, *count_of(pi, pj) + s) : primary_ray<kQuery>(P, pi, pj, s, view_cam(pv));
+                const Ray r = primary_ray<kQuery>(P, pi, pj, s, view_cam(pv), first_sample(pi, pj));
                 p_item[slot] = item;
                 ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
                 ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -1170,8 +1081,8 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
       }, k == 2, all_nodes, sph, ranged);
     else
       return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-        // (kAdaptive and kAdaptiveVar are not built for every sphere staged without every node, which split_staging never plans)
-        if constexpr ((query == Query::kAdaptive || query == Query::kAdaptiveVar) && s && !a) return cudaErrorInvalidValue;
+        // (the adaptive kinds are not built for every sphere staged without every node, which split_staging never plans)
+        if constexpr (is_adaptive(query) && s && !a) return cudaErrorInvalidValue;
         else
           return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(
               lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);

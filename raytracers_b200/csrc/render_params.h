@@ -71,6 +71,13 @@ enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, k
 __host__ __device__ constexpr bool is_ray_query(Query q) {
   return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
 }
+// Pixel kinds whose pixels each continue from their own sample count (Q.sample_counts): a selection pass in front of the
+// render kernel lists the pixels, which the kernel claims from Q.sel; each sample's offsets are computed on the device, so
+// no offset table is made
+__host__ __device__ constexpr bool is_adaptive(Query q) { return q == Query::kAdaptive || q == Query::kAdaptiveVar; }
+// Pixel kinds that continue a pixel's running sum in Q.accum and store it back.  Such a launch uses neither the heavy-first
+// probe nor the learned claim order, and leaves the learned order as it found it.
+__host__ __device__ constexpr bool is_progressive(Query q) { return q == Query::kAccumulate || is_adaptive(q); }
 
 // The fields of a launch that RenderParams does not carry (see Query for which kind reads which).  A block of its own,
 // passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those parameters, and
@@ -153,8 +160,8 @@ struct LaunchConfig {
   long long stage_budget;  // warp-queue kernel: shared memory its queues leave for staging, before cap_staging (bytes)
 };
 
-// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); kAccumulate, kViews, kAdaptive and
-// kAdaptiveVar, which read q, on the warp-queue kernel only
+// A frame of pixel kind `kind` on the kernel lc.kernel names (render_kernels.cu); every kind but kPixels reads q and runs
+// on the warp-queue kernel only
 cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const WavefrontBuffers *wf, cudaStream_t stream,
                           int64_t *launches, Query kind, const RayQuery &q);
 // The warp-queue kernel (render_kernels.cu): a launch of kind `kind`, a pixel kind or a ray query (whatever lc.kernel
