@@ -76,11 +76,13 @@ int64_t ray_b200_context_launch_count(struct futhark_context *ctx);
 int ray_b200_context_trace_warps(struct futhark_context *ctx, int32_t enable);
 int ray_b200_context_warp_trace(struct futhark_context *ctx, float *exit_us, int64_t capacity, int64_t *count);
 /* What a launch traces (struct ray_b200_plan's query): a frame, a chunk of a progressive frame, several views, the
- * selected pixels of an adaptive progressive frame (ADAPTIVE_VAR: with their sample variance), or the caller's rays to their closest hit or along their path
+ * selected pixels of an adaptive progressive frame (ADAPTIVE_VAR: with their sample variance), the first hits of a frame's
+ * camera rays (GBUFFER: ray_b200_render_gbuffer), or the caller's rays to their closest hit or along their path
  * (trace_hits / trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit). */
 enum ray_b200_query {
   RAY_B200_QUERY_PIXELS = 0, RAY_B200_QUERY_CLOSEST = 1, RAY_B200_QUERY_ANYHIT = 2, RAY_B200_QUERY_MULTIHIT = 3,
-  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6, RAY_B200_QUERY_ADAPTIVE_VAR = 7
+  RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6, RAY_B200_QUERY_ADAPTIVE_VAR = 7,
+  RAY_B200_QUERY_GBUFFER = 8
 };
 /* The plan of the last render kernel launch on the context: the last frame, progressive chunk, views call or ray query
  * (for ray_b200_render_batch, its last job), as it was launched.  Calls that launch no render kernel (a query of n = 0
@@ -285,6 +287,43 @@ int ray_b200_adaptive_select(struct futhark_context *ctx, const float *accum_dev
 int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
                                const float *cams7_host, int32_t n_views, int64_t h, int64_t w, int32_t spp,
                                int32_t *out_pix_dev, float *out_rgb_dev);
+/* The first-hit buffers of a frame ("G-buffer", "AOVs"): what each pixel's camera rays hit first, for a denoiser's guide
+ * buffers (albedo, normal) and for compositing (depth, sphere id for picking and masks, coverage for alpha at edges).
+ * Every output is optional (NULL = not written) and device memory, row-major: id_dev int32[h][w], depth_dev float[h][w],
+ * normal_dev and albedo_dev float[h][w][3], coverage_dev int32[h][w].  Offsets are 64-bit.
+ *   The rule, for pixel (row j, column i) and sample s in [0, spp): r_s is the camera ray ray_b200_render_into(h, w, spp)
+ *   traces on this prepared scene (the prepared camera with this call's pixel grid and the spp semantics above).  H_s is
+ *   the struct ray_b200_hit that ray_b200_trace_hits(p, r_s, t_min = 0, t_max = 1e9) returns: objs_hit as ray_colour's
+ *   first segment calls it (ray.fut:130), epsilon 0.1 in the search, then re-intersection with (0, t_best + 1), where a
+ *   failed re-intersection is no hit.  hit_s means H_s.sphere >= 0.  Then
+ *       id       = H_0.sphere (-1 on a miss)
+ *       depth    = H_0.t (-1 on a miss), in units of the ray's direction: camera directions are not unit length, and the
+ *                  hit point is o + t * d of sample 0's camera ray (which is why there is no position buffer)
+ *       coverage = the number of samples s with hit_s
+ *       normal   = the mean of x_s = H_s.normal (0 on a miss)
+ *       albedo   = the mean of x_s = the colour of sphere H_s.sphere (as ray_b200_scene_get_arrays returns it) where
+ *                  hit_s, else the sky colour ray_colour returns for r_s (ray.fut:141-148, light 1), which is
+ *                  ray_b200_trace_paths(p, r_s, max_depth = 1)'s colour
+ *   A mean is the f32 sum of x_0, ..., x_{spp-1} per component, one sample at a time in sample order, starting from x_0
+ *   itself (not 0 + x_0), scaled as the float framebuffer scales a colour sum: the sum itself at spp = 1, else
+ *   (1.0f / spp) times the sum.  NaN-aware as elsewhere: a NaN is some NaN.
+ *   Identities: id and depth equal ray_b200_trace_hits on sample 0's camera ray; where coverage == 0, albedo equals
+ *   ray_b200_render_into(h, w, spp)'s float framebuffer bit for bit (every path there ends in the sky at its first
+ *   segment, with light 1); at spp = 1, coverage == (id >= 0).
+ *   The call is one kernel launch on the context's stream, asynchronous, counted by ray_b200_context_launch_count and
+ *   timed by ray_b200_context_last_render_ms; ray_b200_context_last_plan reports query RAY_B200_QUERY_GBUFFER.  The
+ *   prepared scene may be freed or re-uploaded while the call is in flight, as for ray_b200_render_into.  It runs on the
+ *   warp-queue kernel whatever RAY_KERNEL or the context's kernel says, each pixel's samples in one slot (never spread),
+ *   and uses neither the heavy-first probe nor the learned claim order, nor changes them: renders before and after it
+ *   plan and launch exactly as without it.  The buffers converge in a few samples and do not change while a progressive
+ *   or adaptive colour frame refines, so a caller computes them once, apart from the colour frame.
+ *   Errors (nonzero return, futhark_context_get_error; the context stays usable): every error of ray_b200_render_into
+ *   (image size, spp, an invalid prepared scene, a RAY_GPUS > 1 context), all five outputs NULL, and a shard set
+ *   (world > 1). */
+int ray_b200_render_gbuffer(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                            int64_t h, int64_t w, int32_t spp,
+                            int32_t *id_dev, float *depth_dev, float *normal_dev, float *albedo_dev,
+                            int32_t *coverage_dev);
 /* Like futhark_entry_render but with explicit spp (library-owned result). */
 int ray_b200_entry_render_spp(struct futhark_context *ctx, struct futhark_i32_2d **out0, int64_t h, int64_t w,
                               int32_t spp, const struct futhark_opaque_prepared_scene *p);

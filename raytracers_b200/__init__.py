@@ -65,7 +65,7 @@ class Plan(C.Structure):
 
 
 # enum ray_b200_query: what a launch traces (Plan.query)
-QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var")
+QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var", "gbuffer")
 
 
 class RenderJob(C.Structure):
@@ -169,6 +169,7 @@ def load_library(variant=""):
         "ray_b200_render_adaptive_var": (C.c_int, [vp, vp, vp, vp, vp, i64, i64, i32, vp, vp, vp]),
         "ray_b200_adaptive_select": (C.c_int, [vp, vp, vp, vp, i64, i64, C.c_float, C.c_float, i32, i32, vp, vp]),
         "ray_b200_render_views_into": (C.c_int, [vp, vp, vp, i32, i64, i64, i32, vp, vp]),
+        "ray_b200_render_gbuffer": (C.c_int, [vp, vp, i64, i64, i32, vp, vp, vp, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
         "ray_b200_shard_tiles_padded": (i64, [i64, i64, i32]),
@@ -783,6 +784,41 @@ class Context:
         self.render_views_into(prepared, c, h, w, spp, pix.data_ptr(), rgb.data_ptr() if rgb is not None else None)
         self.sync()
         return (pix, rgb) if want_rgb else pix
+
+    GBUFFER_OUTPUTS = ("id", "depth", "normal", "albedo", "coverage")
+
+    def render_gbuffer_into(self, prepared, h, w, spp, id_dev=0, depth_dev=0, normal_dev=0, albedo_dev=0, coverage_dev=0):
+        """The first-hit buffers of an h x w frame at spp samples (ray_b200_render_gbuffer), written to the device buffers
+        given (0 / None = not written): id_dev int32[h][w] (sphere of sample 0's first hit, -1 = none), depth_dev
+        float[h][w] (its t along the camera ray, -1 = none), normal_dev and albedo_dev float[h][w][3] (the mean first-hit
+        normal, and the mean of the hit sphere's colour or the sky's), coverage_dev int32[h][w] (samples that hit).
+        Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_render_gbuffer(self.handle, prepared.handle, int(h), int(w), int(spp), _ptr(id_dev),
+                                                     _ptr(depth_dev), _ptr(normal_dev), _ptr(albedo_dev), _ptr(coverage_dev)))
+
+    def render_gbuffer(self, prepared, h, w, spp=1, outputs=GBUFFER_OUTPUTS):
+        """The first-hit buffers of the prepared scene at h x w and spp samples per pixel, as a dict of new CUDA tensors
+        on the context's device, one per name in `outputs`: "id" int32 [h, w], "depth" float32 [h, w], "normal" and
+        "albedo" float32 [h, w, 3], "coverage" int32 [h, w] (see render_gbuffer_into and ray_b200_render_gbuffer for the
+        rule).  Waits for torch's current stream before, and synchronises the context after the call."""
+        import torch
+        names = tuple(outputs)
+        for n in names:
+            if n not in self.GBUFFER_OUTPUTS:
+                raise ValueError(f"render_gbuffer: unknown output {n!r}; the outputs are {', '.join(self.GBUFFER_OUTPUTS)}")
+        if not names:
+            raise ValueError("render_gbuffer: no output requested")
+        dev = torch.device("cuda", self.device)
+        h, w = int(h), int(w)
+        shape = {"id": ((h, w), torch.int32), "depth": ((h, w), torch.float32), "normal": ((h, w, 3), torch.float32),
+                 "albedo": ((h, w, 3), torch.float32), "coverage": ((h, w), torch.int32)}
+        out = {n: torch.empty(shape[n][0], dtype=shape[n][1], device=dev) for n in self.GBUFFER_OUTPUTS if n in names}
+        # the outputs' memory may still be in use on torch's stream, which the context's own stream is not ordered after
+        torch.cuda.current_stream(dev).synchronize()
+        ptr = lambda n: out[n].data_ptr() if n in out else 0
+        self.render_gbuffer_into(prepared, h, w, spp, ptr("id"), ptr("depth"), ptr("normal"), ptr("albedo"), ptr("coverage"))
+        self.sync()
+        return out
 
     def render_host(self, h, w, prepared, spp=1, want_rgb=False, out=None):
         pix = out if out is not None else np.empty((h, w), np.int32)

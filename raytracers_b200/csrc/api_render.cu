@@ -73,7 +73,8 @@ static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
 static_assert((int)Query::kPixels == RAY_B200_QUERY_PIXELS && (int)Query::kClosest == RAY_B200_QUERY_CLOSEST &&
                   (int)Query::kAnyHit == RAY_B200_QUERY_ANYHIT && (int)Query::kMultiHit == RAY_B200_QUERY_MULTIHIT &&
                   (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS &&
-                  (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE && (int)Query::kAdaptiveVar == RAY_B200_QUERY_ADAPTIVE_VAR,
+                  (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE && (int)Query::kAdaptiveVar == RAY_B200_QUERY_ADAPTIVE_VAR &&
+                  (int)Query::kGBuffer == RAY_B200_QUERY_GBUFFER,
               "enum ray_b200_query names the values of Query");
 static_assert(sizeof(struct ray_b200_plan) == 80, "struct ray_b200_plan is 16 int32 and 2 int64");
 
@@ -114,7 +115,8 @@ static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
 // Query::kAccumulate reads the offset table of the whole frame from the chunk's first sample on and scales by 1/s_end.
 // Query::kViews: the work items are the tiles of all q.n_views frames, so the plan (K, staging, the sample buffer) is
 // that of one frame of n_views x tiles(h, w) tiles.  The adaptive kinds are planned over all tiles, an upper bound on
-// their work (the selection is on the device).
+// their work (the selection is on the device).  A pixel-bound kind (Query::kGBuffer) is planned as a frame whose samples
+// are not spread.
 int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc) {
   const futhark_opaque_prepared_scene *p = f.scene;
   const int64_t h = f.h, w = f.w; const int32_t spp = f.spp;
@@ -191,7 +193,7 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   if (kern == RAY_B200_KERNEL_WARPQUEUE) {
     // samples will be spread if the finished-sample buffer fits the budget (do_render allocates it; a failed allocation
     // there falls back to pixel-bound samples, whose bigger slots are checked again at launch)
-    const bool will_spread = spread_bytes(ctx, kWqMaxWarps, spp) != 0;
+    const bool will_spread = !is_pixel_bound(f.kind) && spread_bytes(ctx, kWqMaxWarps, spp) != 0;
     // the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame (a warp's tile
     // lies in one view: the density is that of a view, however many there are)
     const bool coherent = spp > 1 || h * w >= ((int64_t)1 << 22);
@@ -399,7 +401,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   if (lc.kernel == RAY_B200_KERNEL_WAVEFRONT && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
   P.sample_buf = nullptr;
   const bool slot_kernel = lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_STREAMQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK;
-  const size_t need = slot_kernel ? spread_bytes(ctx, lc.wq_warps, P.spp) : 0;
+  const size_t need = slot_kernel && !is_pixel_bound(f.kind) ? spread_bytes(ctx, lc.wq_warps, P.spp) : 0;
   if (need) {
     // samples of a pixel are spread over a warp's slots; finished colours wait here for the in-order sum
     // (0.54 MB per sample on an H100's 132 SMs with 32 warps).  Above a memory budget, or when the allocation fails, the frame falls
@@ -417,10 +419,10 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   }
   // heavy-first claim order (warp-queue kernel): worth its probe pass when a frame is long enough to have a tail to lose
   // — more than one sample per pixel — and pointless when every tile is claimed in the first wave anyway.
-  // A progressive launch uses neither this nor the learned order below (DESIGN.md, progressive rendering).  A views launch
+  // A progressive or G-buffer launch uses neither this nor the learned order below (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = !is_progressive(f.kind) && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = !is_plain_order(f.kind) && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -706,6 +708,29 @@ int ray_b200_render_views_into(struct futhark_context *ctx, const struct futhark
   const cudaError_t fe = cudaFreeAsync(cams_dev, ctx->stream);
   if (!rc && fe != cudaSuccess) { set_error(ctx, "render_views_into: %s", cudaGetErrorString(fe)); rc = 1; }
   return rc;
+}
+
+int ray_b200_render_gbuffer(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, int64_t h, int64_t w,
+                            int32_t spp, int32_t *id_dev, float *depth_dev, float *normal_dev, float *albedo_dev,
+                            int32_t *coverage_dev) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!ctx->peers.empty()) { set_error(ctx, "render_gbuffer: not available on a single-process multi-GPU context (RAY_GPUS > 1)"); return 1; }
+  if (ctx->cfg.world > 1) { set_error(ctx, "render_gbuffer: not available with a shard set (rank %d of %d)", ctx->cfg.rank, ctx->cfg.world); return 1; }
+  if (!id_dev && !depth_dev && !normal_dev && !albedo_dev && !coverage_dev) {
+    set_error(ctx, "render_gbuffer: every output is NULL");
+    return 1;
+  }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  Frame f{p, h, w, spp, 0, 1};
+  f.kind = Query::kGBuffer;
+  f.q.perm = p ? p->dev.perm : nullptr;
+  f.q.gb_id = id_dev;
+  f.q.gb_depth = depth_dev;
+  f.q.gb_normal = normal_dev;
+  f.q.gb_albedo = albedo_dev;
+  f.q.gb_coverage = coverage_dev;
+  return render_frame(ctx, f);
 }
 
 int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, float *out_rgb_host, int64_t h, int64_t w, int32_t spp,

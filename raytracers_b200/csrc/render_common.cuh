@@ -448,6 +448,7 @@ cudaError_t with_query(F &&f, Query q) {
     case Query::kViews: return f(std::integral_constant<Query, Query::kViews>{});
     case Query::kAdaptive: return f(std::integral_constant<Query, Query::kAdaptive>{});
     case Query::kAdaptiveVar: return f(std::integral_constant<Query, Query::kAdaptiveVar>{});
+    case Query::kGBuffer: return f(std::integral_constant<Query, Query::kGBuffer>{});
     default: return cudaErrorInvalidValue;
   }
 }

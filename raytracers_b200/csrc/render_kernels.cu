@@ -256,6 +256,14 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // sample order, next to the in-order sum that already has the old and new sums in hand: in finish_path once per finished
 // sample for pixel-bound samples, in the channel loop of finalize_pixels for spread ones.  No shared memory is added, so
 // the plan, the staging and wq_warp_bytes are those of Query::kAdaptive.
+//
+// Query::kGBuffer, the guide buffers of a frame (include/ray_b200.h ray_b200_render_gbuffer): the camera rays of the
+// frame's tiles in the chunk permutation, as Query::kPixels traces them, but every path ends after its first segment.  The
+// shade step makes the segment's hit as the hit query's finish makes it (re-intersection with (0, tb + 1), sphere through
+// Q.perm), both sky exits make the miss colour of shade_segment, and nothing is scattered.  finish_gsample folds the
+// sample into the pixel's sums; a slot owns its pixel (pixel-bound only, the launcher never gives this kind a
+// finished-sample buffer), and p_sum / p_light carry the normal and albedo sums, so no shared memory is added and the
+// plan, the staging and wq_warp_bytes are those of a pixel-bound Query::kPixels frame.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -273,7 +281,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   constexpr bool kRays = is_ray_query(kQuery);  // ray mode
   constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews;
   constexpr bool kProg = is_progressive(kQuery), kAdapt = is_adaptive(kQuery), kVar = kQuery == Query::kAdaptiveVar;
+  constexpr bool kGBuf = kQuery == Query::kGBuffer;
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
+  static_assert(!is_pixel_bound(kQuery) || !kSpread, "a pixel-bound kind is launched without a finished-sample buffer");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   if (P.warp_trace && threadIdx.x == 0) atomicMin(P.warp_trace, global_timer_ns());
@@ -420,6 +430,54 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         store_pixel(item, pi, pj, pv, c, sum);
         p_item[slot] = -1;
       }
+    }
+  };
+  // kGBuffer: the colour ray_colour returns when the slot's ray r (a = dot(d, d)) leaves for the sky on its first segment,
+  // light 1 (ray.fut:141-148): shade_segment's miss branch
+  [[maybe_unused]] auto sky_colour = [&](Ray r, const float a) {
+    V3 light = v3(1.0f, 1.0f, 1.0f), colour;
+    int depth = 0;
+    shade_segment(sc, P, r, a, -1, 0.0f, light, depth, colour);
+    return colour;
+  };
+  // kGBuffer: sample s of the slot's pixel has its first hit: the sphere (the caller's index, -1 = no hit), t, the normal
+  // n (0 without a hit) and the albedo x (the sphere's colour, or the sky's).  Sample 0 writes the pixel's id and depth;
+  // the normal and albedo sums run in p_sum.xyz and p_light.xyz one sample at a time in sample order (sample 0's values
+  // start them), the sample in p_sum.w and the coverage in p_light.w.  The last sample stores them scaled as write_pixel
+  // scales a colour sum.
+  [[maybe_unused]] auto finish_gsample = [&](const int slot, const int sphere, const float t, const V3 n, const V3 x) {
+    const int item = p_item[slot];
+    const float4 ps = p_sum[slot], pl = p_light[slot];
+    int s = __float_as_int(ps.w);
+    const int cov = __float_as_int(pl.w) + (sphere >= 0 ? 1 : 0);
+    const V3 ns = s == 0 ? n : vadd(v3(ps.x, ps.y, ps.z), n);
+    const V3 xs = s == 0 ? x : vadd(v3(pl.x, pl.y, pl.z), x);
+    int pi, pj, pv;
+    pixel_of(item, pv, pi, pj);
+    const size_t px = (size_t)pj * P.W + pi;  // 64-bit offsets: [H][W][3] floats pass 4 GiB above 2^32 / 12 pixels
+    if (s == 0) {
+      if (Q.gb_id) Q.gb_id[px] = sphere;
+      if (Q.gb_depth) Q.gb_depth[px] = t;
+    }
+    s++;
+    if (s < spp) {
+      const Ray nr = primary_ray<kQuery>(P, pi, pj, s);
+      ray_o[slot] = make_float4(nr.o.x, nr.o.y, nr.o.z, 0.0f);
+      ray_d[slot] = make_float4(nr.d.x, nr.d.y, nr.d.z, 0.0f);
+      p_sum[slot] = make_float4(ns.x, ns.y, ns.z, __int_as_float(s));
+      p_light[slot] = make_float4(xs.x, xs.y, xs.z, __int_as_float(cov));
+    } else {
+      const V3 nm = spp == 1 ? ns : vscale(P.inv_spp, ns), xm = spp == 1 ? xs : vscale(P.inv_spp, xs);
+      if (Q.gb_normal) {
+        float *o = Q.gb_normal + 3 * px;
+        o[0] = nm.x; o[1] = nm.y; o[2] = nm.z;
+      }
+      if (Q.gb_albedo) {
+        float *o = Q.gb_albedo + 3 * px;
+        o[0] = xm.x; o[1] = xm.y; o[2] = xm.z;
+      }
+      if (Q.gb_coverage) Q.gb_coverage[px] = cov;
+      p_item[slot] = -1;
     }
   };
   // hit query: struct ray_b200_hit of the slot's ray (t = -1, sphere = -1, p = normal = 0 when there is no hit)
@@ -694,6 +752,10 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
               continue;
             } else if (kQuery == Query::kClosest && (kRanged || Q.hits)) {  // no hit (paths have no ranged form)
               finish_hit(slot, -1.0f, -1, v3(0.0f, 0.0f, 0.0f), v3(0.0f, 0.0f, 0.0f));
+              continue;
+            }
+            if constexpr (kGBuf) {  // no hit, albedo = the sky
+              finish_gsample(slot, -1, -1.0f, v3(0.0f, 0.0f, 0.0f), sky_colour(r, q.a));
               continue;
             }
             const float4 pl = p_light[slot];  // miss (ray.fut:141-148)
@@ -989,6 +1051,28 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         else finish_hit(slot, -1.0f, -1, p, n);
         continue;
       }
+      if constexpr (kGBuf) {
+        // the first hit as the hit query's finish makes it (t_min = 0; a failed re-intersection is no hit), and its albedo:
+        // the sphere's colour, or the sky's where the path leaves; the path ends here, nothing is scattered
+        int sphere = -1;
+        float t = -1.0f;
+        V3 n = v3(0.0f, 0.0f, 0.0f), x;
+        if (j >= 0) {
+          const float4 g = sc.sphere(j);
+          const float th = sphere_t(g.x, g.y, g.z, g.w, r, ro.w, 0.0f, tb + 1.0f);
+          if (th >= 0.0f) {
+            const V3 p = vadd(r.o, vscale(th, r.d));                  // point_at_param, ray.fut:14-15
+            n = vscale(1.0f / g.w, vsub(p, v3(g.x, g.y, g.z)));       // ray.fut:42-43
+            t = th;
+            sphere = __ldg(Q.perm + j);
+            const float4 col = __ldg(P.colour + j);
+            x = v3(col.x, col.y, col.z);
+          }
+        }
+        if (sphere < 0) x = sky_colour(r, ro.w);
+        finish_gsample(slot, sphere, t, n, x);
+        continue;
+      }
       if (shade_segment(sc, P, r, ro.w, j, tb, light, depth, colour, kRays ? Q.max_depth : kMaxDepth)) {
         ray_o[slot] = make_float4(r.o.x, r.o.y, r.o.z, 0.0f);
         ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
@@ -1081,8 +1165,10 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
       }, k == 2, all_nodes, sph, ranged);
     else
       return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-        // (the adaptive kinds are not built for every sphere staged without every node, which split_staging never plans)
-        if constexpr (is_adaptive(query) && s && !a) return cudaErrorInvalidValue;
+        // (the adaptive and pixel-bound kinds are not built for every sphere staged without every node, which
+        // split_staging never plans; the pixel-bound kinds have no spread variants)
+        if constexpr ((is_adaptive(query) || is_pixel_bound(query)) && s && !a) return cudaErrorInvalidValue;
+        else if constexpr (is_pixel_bound(query) && sp) return cudaErrorInvalidValue;
         else
           return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(
               lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, lc.wq_packet, lc.wq_refill, nlow, q);

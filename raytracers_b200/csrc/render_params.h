@@ -65,9 +65,11 @@ struct RenderParams {
 // path (rgb, segments, max_depth; hits == NULL tells the two apart at run time); kAnyHit, to their first accepted sphere
 // (occluded); kMultiHit, to their k nearest ones (hits, k, counts).  kAdaptive, a pixel kind: the selected pixels of a
 // progressive frame, each from its own sample count (accum, sample_counts, mask, sel, n_sel).  kAdaptiveVar: kAdaptive
-// that also keeps each pixel's running sum of squared deviations (m2).  New kinds go at the end: kernel names carry the
-// values, and tools/sass_compare.py reads older builds' names by them.
-enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar };
+// that also keeps each pixel's running sum of squared deviations (m2).  kGBuffer, a pixel kind: the first hit of every
+// camera ray of a frame (its sphere, t, normal and albedo), reduced per pixel into the guide buffers (gb_id, gb_depth,
+// gb_normal, gb_albedo, gb_coverage).  New kinds go at the end: kernel names carry the values, and tools/sass_compare.py
+// reads older builds' names by them.
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar, kGBuffer };
 __host__ __device__ constexpr bool is_ray_query(Query q) {
   return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
 }
@@ -78,6 +80,12 @@ __host__ __device__ constexpr bool is_adaptive(Query q) { return q == Query::kAd
 // Pixel kinds that continue a pixel's running sum in Q.accum and store it back.  Such a launch uses neither the heavy-first
 // probe nor the learned claim order, and leaves the learned order as it found it.
 __host__ __device__ constexpr bool is_progressive(Query q) { return q == Query::kAccumulate || is_adaptive(q); }
+// Pixel kinds whose slots always own their pixel, whatever the sample count: the launch gets no finished-sample buffer,
+// so it is planned and launched as a pixel-bound frame
+__host__ __device__ constexpr bool is_pixel_bound(Query q) { return q == Query::kGBuffer; }
+// Pixel kinds that claim the frame's tiles in the plain chunk permutation: a launch uses neither the heavy-first probe
+// nor the learned claim order, and leaves the learned order as it found it
+__host__ __device__ constexpr bool is_plain_order(Query q) { return is_progressive(q) || q == Query::kGBuffer; }
 
 // The fields of a launch that RenderParams does not carry (see Query for which kind reads which).  A block of its own,
 // passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those parameters, and
@@ -118,6 +126,14 @@ struct RayQuery {
   // Query::kAdaptiveVar (include/ray_b200.h ray_b200_render_adaptive_var): row-major [H][W][3], each pixel's M2, Welford's
   // running f32 sum of squared deviations from the mean of its samples (not read where its count is 0)
   float *m2;
+  // Query::kGBuffer (include/ray_b200.h ray_b200_render_gbuffer): the guide buffers of the frame, row-major, each optional
+  // (NULL = not written): [H][W] sphere id and t of sample 0's first hit, [H][W][3] mean normal and albedo of the first
+  // hits, [H][W] samples whose camera ray hit a sphere
+  int32_t *gb_id;
+  float *gb_depth;
+  float *gb_normal;
+  float *gb_albedo;
+  int32_t *gb_coverage;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
