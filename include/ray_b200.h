@@ -142,13 +142,63 @@ int ray_b200_prepared_dump(struct futhark_context *ctx, const struct futhark_opa
 int ray_b200_prepared_packed(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, float *nodes,
                              float *nodes_soa, float *geom, float *colour);
 /* Bytes prepare_scene copies host -> device: the sphere records (LBVH build and packing run on the device);
- * with tuning "host_build" / RAY_HOST_BUILD=1 the host-built arrays instead. */
+ * with tuning "host_build" / RAY_HOST_BUILD=1 the host-built arrays instead.  0 for a scene last built by
+ * ray_b200_prepare_scene_device or ray_b200_prepared_update (and re-uploaded since), except on a host_build context. */
 int64_t ray_b200_prepared_upload_bytes(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p);
 /* Bytes of the prepared scene resident in HBM (packed BVH2C + the Karras-order LBVH kept for introspection). */
 int64_t ray_b200_prepared_device_bytes(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p);
 /* Runs prepare_scene's device work again for an existing handle: H2D of the sphere records from page-locked
- * memory + LBVH build on the device (the H2D leg of bench.py's end-to-end step). */
+ * memory + LBVH build on the device (the H2D leg of bench.py's end-to-end step).  For a scene last built from device
+ * memory (below) the records are recovered on the device from the scene's own arrays instead, with no H2D copy. */
 int ray_b200_prepared_reupload(struct futhark_context *ctx, struct futhark_opaque_prepared_scene *p);
+
+/* ---- prepared scenes from device memory: dynamic scenes without a host round trip -------------------------------
+ * A caller whose spheres live in device memory (a simulation, a learned model, an animation computed on the GPU) builds
+ * and rebuilds a prepared scene from them directly.  spheres_dev: device float[n][7] in the layout of
+ * ray_b200_scene_from_arrays (pos.xyz, colour.xyz, radius), 4-byte aligned, readable by the context's device;
+ * cam7_host: host float[7] as there.
+ *   Exactness.  After ray_b200_prepare_scene_device(h, w, S, n, cam7) or ray_b200_prepared_update(p, S, n, cam7) the
+ *   prepared scene is bit for bit the one futhark_entry_prepare_scene(h, w, scene_from_arrays(S, n, cam7)) makes from
+ *   the same 7n floats (on update with cam7_host == NULL, cam7 is the scene's own camera): prepared_info (refit_sweeps,
+ *   stale_nodes, max_depth and the root box included), prepared_dump, prepared_packed, every frame and every ray query.
+ *   The build is prepare_scene's LBVH build, only fed from device memory.  There is no refit-only update: a refit that
+ *   kept the old topology would give a tree other than the reference's, whose stale boxes decide which hits are culled,
+ *   so its frames would not be the reference's.
+ *   No host copy.  The calls copy no records host -> device (ray_b200_prepared_upload_bytes is 0), and the library
+ *   keeps no host copy of them.  Where it needs them it recovers them on the device from the packed arrays,
+ *   sphere[perm[k]] = (geom[k].xyz, colour[k].xyz, geom[k].w), which is exact: ray_b200_prepared_spheres (one gather
+ *   launch), futhark_store_opaque_prepared_scene (which then reads them back and synchronises) and
+ *   ray_b200_prepared_reupload (which rebuilds from the recovered records on the device).
+ *   Stream order and blocking.  spheres_dev is read on the context's stream, after the work enqueued there before the
+ *   call; a producer on another stream must be ordered before it (ray_b200_context_set_stream, or an event).  Like
+ *   prepare_scene, both calls return after the build's 32-byte read-back, because render planning needs the tree
+ *   depth; spheres_dev may then be reused or freed.  (A non-blocking update would need planning without the depth; it
+ *   is not offered.)
+ *   Frames in flight.  Frames, queries and batches enqueued before an update read the old tree, whose memory is freed
+ *   behind them on either pipeline lane; work enqueued after it reads the new tree.  The new tree is built before the old
+ *   one is released, so an update whose build fails leaves the previous tree in place.
+ *   Learned claim order.  An update drops the scene's learned claim order: the renders after it plan and launch as the
+ *   first renders of a freshly prepared scene do.
+ *   Context state.  ray_b200_context_last_plan and last_render_ms are unchanged; ray_b200_context_launch_count counts
+ *   the build's launches as for prepare_scene.
+ *   host_build contexts (RAY_HOST_BUILD=1): the records are read back and the host builder runs; the result is the
+ *   same, and ray_b200_prepared_upload_bytes is the block's, as for prepare_scene there.
+ *   Errors (nonzero return and a message; the context stays usable, and an argument error leaves an existing prepared
+ *   scene unchanged and usable): n < 2 or n > 2^26, a NULL spheres_dev, out0, p or (for prepare_scene_device)
+ *   cam7_host, spheres_dev not readable by the device (plain host memory), h <= 0 or w <= 0, an invalid prepared scene,
+ *   and a RAY_GPUS > 1 context (its helper devices would need the records). */
+int ray_b200_prepare_scene_device(struct futhark_context *ctx, struct futhark_opaque_prepared_scene **out0, int64_t h,
+                                  int64_t w, const float *spheres_dev, int64_t n, const float *cam7_host);
+/* Replaces the spheres of an existing prepared scene (any n in [2, 2^26]) and rebuilds its tree in place, for its
+ * (h, w); cam7_host == NULL keeps the camera, otherwise the camera is remade from cam7_host for the scene's (h, w). */
+int ray_b200_prepared_update(struct futhark_context *ctx, struct futhark_opaque_prepared_scene *p,
+                             const float *spheres_dev, int64_t n, const float *cam7_host);
+/* The prepared scene's current sphere records, in the caller's order, bit for bit as given (by any of the calls that
+ * make or update a prepared scene): spheres_dev = device float[n][7] (NULL: not written; n = prepared_info's n_leaves),
+ * written by one gather launch, asynchronous on the context's stream; cam7_host = host float[7] (NULL: not written).
+ * Errors: an invalid prepared scene. */
+int ray_b200_prepared_spheres(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                              float *spheres_dev, float *cam7_host);
 
 /* ---- render extensions -------------------------------------------------------------------------- */
 /* render with explicit spp; optional float framebuffer.  out_pix_dev: device int32[h][w] (REQUIRED);

@@ -162,6 +162,9 @@ def load_library(variant=""):
         "ray_b200_prepared_packed": (C.c_int, [vp, vp, vp, vp, vp, vp]),
         "ray_b200_prepared_upload_bytes": (i64, [vp, vp]),
         "ray_b200_prepared_device_bytes": (i64, [vp, vp]),
+        "ray_b200_prepare_scene_device": (C.c_int, [vp, pp, i64, i64, vp, i64, vp]),
+        "ray_b200_prepared_update": (C.c_int, [vp, vp, vp, i64, vp]),
+        "ray_b200_prepared_spheres": (C.c_int, [vp, vp, vp, vp]),
         "ray_b200_render_into": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_host": (C.c_int, [vp, vp, vp, i64, i64, i32, vp]),
         "ray_b200_render_accumulate": (C.c_int, [vp, vp, i64, i64, i32, i32, vp, vp, vp]),
@@ -304,6 +307,29 @@ def _check_tensor(device, name, t, dtypes, shape):
                          f"got {t.dtype} {tuple(t.shape)}")
 
 
+def _sphere_rows(device, spheres):
+    """n of spheres, a contiguous float32 CUDA tensor [n, 7] on cuda:device; ValueError for anything else"""
+    import torch
+    if not isinstance(spheres, torch.Tensor) or spheres.dim() != 2:
+        raise ValueError("spheres must be a float32 CUDA tensor of shape [n, 7]")
+    _check_tensor(device, "spheres", spheres, (torch.float32,), (spheres.shape[0], 7))
+    return int(spheres.shape[0])
+
+
+def _camera7(cam7):
+    """cam7 (look_from.xyz, look_at.xyz, fov) as a contiguous float32 [7] host array, from any host array-like of 7
+    floating-point values; a CUDA tensor raises ValueError (reading it would synchronise the device), as does any other
+    shape or dtype."""
+    if type(cam7).__module__.startswith("torch"):
+        if cam7.device.type != "cpu":
+            raise ValueError(f"cam7 must be a host array of 7 floats, got a tensor on {cam7.device}")
+        cam7 = cam7.numpy()
+    a = np.asarray(cam7)
+    if a.shape != (7,) or a.dtype.kind != "f":
+        raise ValueError(f"cam7 must be a host array of 7 floats, got {a.dtype} {a.shape}")
+    return np.ascontiguousarray(a, np.float32)
+
+
 def camera_rays(camera, h, w, spp=1):
     """Camera rays of an h x w frame as render traces them: float32[h][w][spp][6] (origin, direction) of sample s of
     pixel (row j, column i), with the same float32 operations in the same order as the render kernels (ray.fut:109-114,
@@ -407,8 +433,39 @@ class PreparedScene(_Handle):
         return int(self.ctx.lib.ray_b200_prepared_device_bytes(self.ctx.handle, self.handle))
 
     def reupload(self):
-        """Host->device copy of the packed BVH + spheres again (the H2D leg of bench.py's e2e step)."""
+        """Host->device copy of the packed BVH + spheres again (the H2D leg of bench.py's e2e step).  A scene last built
+        from device memory is rebuilt from its own device arrays, with no copy."""
         self.ctx._check(self.ctx.lib.ray_b200_prepared_reupload(self.ctx.handle, self.handle))
+
+    def update_from_ptr(self, spheres_dev, n, cam7=None):
+        """ray_b200_prepared_update: replaces the scene's spheres by the n records at device address spheres_dev
+        (float[n][7], read on the context's stream) and rebuilds its tree; cam7 (host [7]) replaces the camera, None keeps
+        it.  Returns after the build's 32-byte read-back; spheres_dev may then be reused."""
+        c = None if cam7 is None else _camera7(cam7)
+        self.ctx._check(self.ctx.lib.ray_b200_prepared_update(self.ctx.handle, self.handle, _ptr(spheres_dev), int(n), _ptr(c)))
+
+    def update(self, spheres, cam7=None):
+        """Rebuilds the scene from spheres, a contiguous float32 CUDA tensor [n, 7] on the context's device (2 <= n <= 2^26;
+        the layout of Context.scene_from_arrays), and cam7 (host [7]) or None to keep the camera.  The result is the scene
+        prepare_scene makes from the same records, bit for bit; nothing is copied to or from the host.  Frames enqueued
+        before the call render the old scene.  Waits for torch's current stream before the call."""
+        import torch
+        n = _sphere_rows(self.ctx.device, spheres)
+        c = None if cam7 is None else _camera7(cam7)
+        torch.cuda.current_stream(spheres.device).synchronize()   # spheres may still be in flight on torch's stream
+        self.update_from_ptr(spheres.data_ptr(), n, c)
+
+    def spheres(self):
+        """(spheres, cam7): the scene's current records as a new CUDA float32 tensor [n, 7] in the order they were given,
+        bit for bit, and its camera as a host float32 [7] array.  Synchronises the context."""
+        import torch
+        n = int(self.info()["n_leaves"])
+        out = torch.empty((n, 7), dtype=torch.float32, device=torch.device("cuda", self.ctx.device))
+        cam = np.empty(7, np.float32)
+        torch.cuda.current_stream(out.device).synchronize()
+        self.ctx._check(self.ctx.lib.ray_b200_prepared_spheres(self.ctx.handle, self.handle, _ptr(out.data_ptr()), _ptr(cam)))
+        self.ctx.sync()
+        return out, cam
 
     def store(self):
         p = C.c_void_p(None)
@@ -502,6 +559,24 @@ class Context:
 
     def prepare_scene(self, h, w, scene):
         return self._out(PreparedScene, "futhark_entry_prepare_scene", int(h), int(w), scene.handle)
+
+    def prepare_scene_device_from_ptr(self, h, w, spheres_dev, n, cam7):
+        """ray_b200_prepare_scene_device: a prepared scene built from the n sphere records at device address spheres_dev
+        (float[n][7], read on the context's stream) with the host camera cam7 ([7]).  Returns after the build's 32-byte
+        read-back; spheres_dev may then be reused."""
+        c = _camera7(cam7)
+        return self._out(PreparedScene, "ray_b200_prepare_scene_device", int(h), int(w), _ptr(spheres_dev), int(n), _ptr(c))
+
+    def prepare_scene_device(self, h, w, spheres, cam7):
+        """prepare_scene from sphere records in device memory: spheres is a contiguous float32 CUDA tensor [n, 7] on the
+        context's device (the layout of scene_from_arrays), cam7 a host array-like of 7 floats.  The prepared scene equals
+        prepare_scene(h, w, scene_from_arrays(spheres, cam7)) bit for bit, and no record is copied to the host.  Waits for
+        torch's current stream before the call; see PreparedScene.update for animating it."""
+        import torch
+        n = _sphere_rows(self.device, spheres)
+        c = _camera7(cam7)
+        torch.cuda.current_stream(spheres.device).synchronize()   # spheres may still be in flight on torch's stream
+        return self.prepare_scene_device_from_ptr(h, w, spheres.data_ptr(), n, c)
 
     def render(self, h, w, prepared, spp=None):
         if spp is None:

@@ -105,7 +105,11 @@ struct futhark_opaque_scene {
 };
 
 struct futhark_opaque_prepared_scene {
-  HostScene host;   // kept for store/restore and re-preparation
+  HostScene host;   // kept for store/restore and re-preparation; its camera is always the scene's
+  // host.spheres holds the records of the current tree.  False after a build from device memory
+  // (ray_b200_prepare_scene_device / ray_b200_prepared_update): host.spheres is then empty, and whatever needs the
+  // records recovers them from the device arrays (recover_spheres).
+  bool host_current = true;
   int64_t h = 0, w = 0;
   CameraRec cam;
   float root_box[6];
@@ -219,5 +223,9 @@ void free_prepared_device(futhark_context *ctx, futhark_opaque_prepared_scene *p
 int release_scene_block(futhark_context *ctx, futhark_opaque_prepared_scene *p, bool drop_order);
 int prepare_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p);
 int prepare_any(futhark_context *ctx, futhark_opaque_prepared_scene *p);
+// The device build of p from n records already on the device (d_spheres, read on the context's stream); returns after
+// the 32-byte read-back.  The tree is built into a new block before p's old one is released, so a failed build leaves
+// p as it was.  `drop_order`: the scene changes, so its learned claim order is dropped with the old block.
+int build_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p, const float *d_spheres, int64_t n, bool drop_order);
 
 }  // namespace rayb200_api

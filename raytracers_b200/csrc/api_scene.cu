@@ -58,9 +58,9 @@ int release_scene_block(futhark_context *ctx, futhark_opaque_prepared_scene *p, 
     where = ctx->reclaim;
   }
   CUDA_TRY(ctx, cudaFreeAsync(p->dev.block, where));
-  // The learned claim order stays: a prepared scene's spheres and camera never change (ray_b200_prepared_reupload builds
-  // the same tree again), so what the recording frame measured remains true.  When the object itself goes
-  // (`drop_order`), its table is freed behind the same frames as the scene.
+  // The learned claim order stays while the tree is rebuilt from the same records (ray_b200_prepared_reupload builds
+  // the same tree again), so what the recording frame measured remains true.  When the object goes or its records
+  // change (`drop_order`), its table is freed behind the same frames as the scene.
   if (drop_order) {
     if (p->order_cache.cost) CUDA_TRY(ctx, cudaFreeAsync(p->order_cache.cost, where));
     if (p->order_cache.ready) cudaEventDestroy(p->order_cache.ready);
@@ -86,8 +86,32 @@ void free_prepared_device(futhark_context *ctx, futhark_opaque_prepared_scene *p
   p->pinned_event = nullptr;
 }
 
-// A page-locked staging buffer of at least `bytes`, reusing a cached one when possible (main.c frees and
+int build_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p, const float *d_spheres, int64_t n, bool drop_order) {
+  const int32_t sweeps = (int32_t)log2f((float)n) + 2;  // bvh.fut:47, host libm as in the reference's C backend
+  DeviceBvh fresh;
+  cudaError_t e = build_bvh_device(d_spheres, n, sweeps, fresh, ctx->d_build_result, ctx->stream, &ctx->launches);
+  // the host needs the tree depth (stack sizing) and the root box (kernel parameter) before the first render
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(ctx->h_build_result, ctx->d_build_result, sizeof(BvhBuildResult), cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) {
+    if (fresh.block) cudaFreeAsync(fresh.block, ctx->stream);
+    set_error(ctx, "prepare_scene: device LBVH build failed: %s", cudaGetErrorString(e));
+    return 1;
+  }
+  if (release_scene_block(ctx, p, drop_order)) { cudaFreeAsync(fresh.block, ctx->stream); return 1; }
+  p->dev = fresh;
+  memcpy(p->root_box, ctx->h_build_result->root_box, sizeof p->root_box);
+  p->max_depth = ctx->h_build_result->max_depth;
+  p->stale_nodes = ctx->h_build_result->stale_nodes;
+  p->refit_sweeps = sweeps;
+  p->n = n;
+  p->host_built = false;
+  return 0;
+}
 
+// prepare_scene, device path (default): the host records are staged (page-locked copy, H2D), then built from that
+// device copy by build_on_device.
 int prepare_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p) {
   const bool timing = ctx->cfg.debugging != 0;
   const double t0 = timing ? now_us() : 0.0;
@@ -100,28 +124,19 @@ int prepare_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p) {
   CUDA_TRY(ctx, cudaMemcpyAsync(d_spheres, p->pinned, sph_bytes, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(ctx, cudaEventRecord(p->pinned_event, ctx->stream));
   const double t1 = timing ? now_us() : 0.0;
-  p->refit_sweeps = (int32_t)log2f((float)(int64_t)n) + 2;  // bvh.fut:47, host libm as in the reference's C backend
-  if (release_scene_block(ctx, p, false)) return 1;
-  CUDA_TRY(ctx, build_bvh_device(d_spheres, (int64_t)n, p->refit_sweeps, p->dev, ctx->d_build_result, ctx->stream, &ctx->launches));
-  CUDA_TRY(ctx, cudaFreeAsync(d_spheres, ctx->stream));
-  // the host needs the tree depth (stack sizing) and the root box (kernel parameter) before the first render
-  const double t2 = timing ? now_us() : 0.0;
-  CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_build_result, ctx->d_build_result, sizeof(BvhBuildResult), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  const int rc = build_on_device(ctx, p, d_spheres, (int64_t)n, false);
+  cudaFreeAsync(d_spheres, ctx->stream);
+  if (rc) return 1;
   if (timing)
-    fprintf(ctx->log ? ctx->log : stderr, "[ray_b200] prepare_scene n=%zu: stage+H2D enqueue %.0f us, build enqueue %.0f us, wait %.0f us\n", n,
-            t1 - t0, t2 - t1, now_us() - t2);
-  memcpy(p->root_box, ctx->h_build_result->root_box, sizeof p->root_box);
-  p->max_depth = ctx->h_build_result->max_depth;
-  p->stale_nodes = ctx->h_build_result->stale_nodes;
-  p->n = (int64_t)n;
-  p->host_built = false;
+    fprintf(ctx->log ? ctx->log : stderr, "[ray_b200] prepare_scene n=%zu: stage+H2D enqueue %.0f us, build + wait %.0f us\n", n,
+            t1 - t0, now_us() - t1);
+  p->host_current = true;
   return 0;
 }
 
 // prepare_scene, host path (RAY_HOST_BUILD=1 / tuning "host_build"): scene_host.cpp builds and packs, one H2D copy.
 // Kept as an independent implementation the device path is tested against.
-int prepare_on_host(futhark_context *ctx, futhark_opaque_prepared_scene *p) {
+int prepare_on_host(futhark_context *ctx, futhark_opaque_prepared_scene *p, bool drop_order = false) {
   Lbvh tree;
   std::string err;
   if (!build_lbvh(p->host, tree, &err)) { set_error(ctx, "%s", err.c_str()); return 1; }
@@ -143,7 +158,7 @@ int prepare_on_host(futhark_context *ctx, futhark_opaque_prepared_scene *p) {
   memcpy(hostside.right, tree.right.data(), ni * 4);
   memcpy(hostside.parent, tree.parent.data(), ni * 4);
   memcpy(hostside.boxes, tree.boxes.data(), ni * 24);
-  if (release_scene_block(ctx, p, false)) return 1;
+  if (release_scene_block(ctx, p, drop_order)) return 1;
   unsigned char *blk = nullptr;
   CUDA_TRY(ctx, cudaMallocAsync(&blk, total, ctx->stream));
   carve_device_bvh(blk, n, p->dev);
@@ -153,15 +168,86 @@ int prepare_on_host(futhark_context *ctx, futhark_opaque_prepared_scene *p) {
   p->max_depth = tree.max_depth; p->stale_nodes = tree.stale_nodes; p->refit_sweeps = tree.refit_sweeps;
   p->n = n;
   p->host_built = true;
+  p->host_current = true;
+  return 0;
+}
+
+int check_sphere_count(futhark_context *ctx, int64_t n) {
+  if (n < 2) { set_error(ctx, "prepare_scene: a scene needs at least 2 spheres (the reference indexes I[0], bvh.fut:65)"); return 1; }
+  if (n > (int64_t)1 << 26) { set_error(ctx, "prepare_scene: too many spheres (this build packs leaf indices into 26 bits)"); return 1; }
   return 0;
 }
 
 int prepare_any(futhark_context *ctx, futhark_opaque_prepared_scene *p) {
-  const int64_t n = (int64_t)p->host.spheres.size();
-  if (n < 2) { set_error(ctx, "prepare_scene: a scene needs at least 2 spheres (the reference indexes I[0], bvh.fut:65)"); return 1; }
-  if (n > (int64_t)1 << 26) { set_error(ctx, "prepare_scene: too many spheres (this build packs leaf indices into 26 bits)"); return 1; }
+  if (check_sphere_count(ctx, (int64_t)p->host.spheres.size())) return 1;
   return ctx->cfg.host_build ? prepare_on_host(ctx, p) : prepare_on_device(ctx, p);
 }
+
+namespace {
+
+// The records of p in the caller's order, gathered from its device arrays into host memory (synchronises).
+int recover_spheres_host(futhark_context *ctx, const futhark_opaque_prepared_scene *p, std::vector<SphereRec> &out) {
+  const size_t bytes = (size_t)p->n * sizeof(SphereRec);
+  float *d = nullptr;
+  CUDA_TRY(ctx, cudaMallocAsync(&d, bytes, ctx->stream));
+  out.resize((size_t)p->n);
+  const cudaError_t e = gather_spheres_device(p->dev, p->n, d, ctx->stream, &ctx->launches);
+  if (e == cudaSuccess) CUDA_TRY(ctx, cudaMemcpyAsync(out.data(), d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(ctx, cudaFreeAsync(d, ctx->stream));
+  CUDA_TRY(ctx, e);
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
+void set_camera(futhark_opaque_prepared_scene *p, const float *cam7) {
+  memcpy(p->host.look_from, cam7, 12); memcpy(p->host.look_at, cam7 + 3, 12); p->host.fov = cam7[6];
+  p->cam = make_camera(p->host, p->h, p->w);
+}
+
+// The argument checks of prepare_scene_device and prepared_update: an error here changes nothing.
+int check_device_records(futhark_context *ctx, const char *what, const float *spheres_dev, int64_t n) {
+  if (!spheres_dev) { set_error(ctx, "%s: null argument", what); return 1; }
+  if (check_sphere_count(ctx, n)) return 1;
+  if (!ctx->peers.empty()) {
+    set_error(ctx, "%s: not available on a single-process multi-GPU context (RAY_GPUS > 1): its helper devices would need the records", what);
+    return 1;
+  }
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, spheres_dev) != cudaSuccess || a.type == cudaMemoryTypeUnregistered) {
+    cudaGetLastError();
+    set_error(ctx, "%s: spheres_dev is not memory the device can read", what);
+    return 1;
+  }
+  return 0;
+}
+
+// prepare_scene_device / prepared_update after their checks: p's tree built from the n records at spheres_dev, with the
+// camera cam7 (NULL: p's own) made for p's (h, w).  The learned claim order is dropped with the old tree.  The device
+// path keeps no host copy of the records; a host_build context reads them back and runs the host builder.  A failed
+// build leaves p's tree and camera as they were.
+int build_from_device_records(futhark_context *ctx, futhark_opaque_prepared_scene *p, const float *spheres_dev, int64_t n,
+                              const float *cam7) {
+  if (ctx->cfg.host_build) {
+    std::vector<SphereRec> recs((size_t)n);
+    CUDA_TRY(ctx, cudaMemcpyAsync(recs.data(), spheres_dev, (size_t)n * sizeof(SphereRec), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    std::vector<SphereRec> old;
+    old.swap(p->host.spheres);
+    p->host.spheres.swap(recs);
+    if (prepare_on_host(ctx, p, true)) {
+      p->host.spheres.swap(old);
+      return 1;
+    }
+  } else {
+    if (build_on_device(ctx, p, spheres_dev, n, true)) return 1;
+    p->host.spheres = std::vector<SphereRec>();
+    p->host_current = false;
+  }
+  if (cam7) set_camera(p, cam7);
+  return 0;
+}
+
+}  // namespace
 
 }  // namespace rayb200_api
 
@@ -224,15 +310,30 @@ int futhark_free_opaque_prepared_scene(struct futhark_context *ctx, struct futha
   delete obj;
   return 0;
 }
-// A stored prepared scene is the scene plus the (h, w) it was prepared for; restoring re-runs prepare_scene.
+// A stored prepared scene is the scene plus the (h, w) it was prepared for; restoring re-runs prepare_scene.  The records
+// of a scene built from device memory are recovered from its device arrays first (this synchronises).
 int futhark_store_opaque_prepared_scene(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *obj, void **p, size_t *n) {
   if (!ctx || !obj || !n) return 1;
-  const size_t sz = scene_blob_size(obj->host) + 16;
+  HostScene recovered;
+  const HostScene *s = &obj->host;
+  if (!obj->host_current) {
+    if (bad_ctx(ctx) || !obj->dev.block) return 1;
+    memcpy(recovered.look_from, obj->host.look_from, 12); memcpy(recovered.look_at, obj->host.look_at, 12);
+    recovered.fov = obj->host.fov;
+    recovered.spheres.resize((size_t)obj->n);  // the blob's size
+    if (p) {
+      std::lock_guard<std::mutex> g(ctx->mu);
+      CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+      if (recover_spheres_host(ctx, obj, recovered.spheres)) return 1;
+    }
+    s = &recovered;
+  }
+  const size_t sz = scene_blob_size(*s) + 16;
   *n = sz;
   if (p) {
     if (!*p) *p = malloc(sz);
     if (!*p) { set_error(ctx, "store_opaque_prepared_scene: out of memory"); return 1; }
-    scene_to_blob(obj->host, (unsigned char *)*p, kPreparedMagic);
+    scene_to_blob(*s, (unsigned char *)*p, kPreparedMagic);
     memcpy((unsigned char *)*p + sz - 16, &obj->h, 8);
     memcpy((unsigned char *)*p + sz - 8, &obj->w, 8);
   }
@@ -378,17 +479,72 @@ int ray_b200_prepared_reupload(struct futhark_context *ctx, struct futhark_opaqu
   std::lock_guard<std::mutex> g(ctx->mu);
   if (!p || !p->dev.block) { set_error(ctx, "prepared_reupload: invalid prepared scene"); return 1; }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-  return prepare_any(ctx, p);  // H2D of the sphere records again + the device LBVH build (or the host path)
+  if (p->host_current) return prepare_any(ctx, p);  // H2D of the sphere records again + the device LBVH build (or the host path)
+  // Records given in device memory: recovered from the scene's own arrays, on the device (or read back for the host builder)
+  if (ctx->cfg.host_build) {
+    if (recover_spheres_host(ctx, p, p->host.spheres)) return 1;
+    return prepare_on_host(ctx, p);
+  }
+  float *d = nullptr;
+  CUDA_TRY(ctx, cudaMallocAsync(&d, (size_t)p->n * sizeof(SphereRec), ctx->stream));
+  int rc = gather_spheres_device(p->dev, p->n, d, ctx->stream, &ctx->launches) != cudaSuccess;
+  if (rc) set_error(ctx, "prepared_reupload: gather of the sphere records failed");
+  else rc = build_on_device(ctx, p, d, p->n, false);
+  cudaFreeAsync(d, ctx->stream);
+  return rc;
+}
+
+int ray_b200_prepare_scene_device(struct futhark_context *ctx, struct futhark_opaque_prepared_scene **out0, int64_t h, int64_t w,
+                                  const float *spheres_dev, int64_t n, const float *cam7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!out0 || !cam7_host) { set_error(ctx, "prepare_scene_device: null argument"); return 1; }
+  if (h <= 0 || w <= 0) { set_error(ctx, "prepare_scene_device: bad image size"); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (check_device_records(ctx, "prepare_scene_device", spheres_dev, n)) return 1;
+  futhark_opaque_prepared_scene *p = new futhark_opaque_prepared_scene;
+  p->h = h; p->w = w;
+  set_camera(p, cam7_host);
+  if (build_from_device_records(ctx, p, spheres_dev, n, nullptr)) { free_prepared_device(ctx, p); delete p; return 1; }
+  *out0 = p;
+  return 0;
+}
+
+int ray_b200_prepared_update(struct futhark_context *ctx, struct futhark_opaque_prepared_scene *p, const float *spheres_dev, int64_t n,
+                             const float *cam7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!p || !p->dev.block) { set_error(ctx, "prepared_update: invalid prepared scene"); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (check_device_records(ctx, "prepared_update", spheres_dev, n)) return 1;
+  return build_from_device_records(ctx, p, spheres_dev, n, cam7_host);
+}
+
+int ray_b200_prepared_spheres(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p, float *spheres_dev,
+                              float *cam7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  if (!p || !p->dev.block) { set_error(ctx, "prepared_spheres: invalid prepared scene"); return 1; }
+  if (spheres_dev) {
+    CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+    CUDA_TRY(ctx, gather_spheres_device(p->dev, p->n, spheres_dev, ctx->stream, &ctx->launches));
+    ctx->lane(0);
+    if (record_scene_use(ctx, p, 0)) return 1;  // an update or free of p waits for the gather
+  }
+  if (cam7_host) { memcpy(cam7_host, p->host.look_from, 12); memcpy(cam7_host + 3, p->host.look_at, 12); cam7_host[6] = p->host.fov; }
+  return 0;
 }
 int64_t ray_b200_prepared_device_bytes(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p) {
   (void)ctx;
   return p ? (int64_t)p->dev.block_bytes : -1;
 }
-// Bytes prepare_scene / prepared_reupload copy host -> device (the sphere records on the device-build path).
+// Bytes prepare_scene / prepared_reupload copy host -> device (the sphere records on the device-build path; none for
+// records given in device memory).
 int64_t ray_b200_prepared_upload_bytes(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p) {
   (void)ctx;
   if (!p) return -1;
-  return p->host_built ? (int64_t)p->dev.block_bytes : (int64_t)(p->host.spheres.size() * sizeof(SphereRec));
+  if (p->host_built) return (int64_t)p->dev.block_bytes;
+  return p->host_current ? (int64_t)(p->host.spheres.size() * sizeof(SphereRec)) : 0;
 }
 
 // ---- host-only entry points (no context, no device): the setup-path logic, testable without a GPU ----

@@ -223,6 +223,18 @@ __global__ void pack_spheres_kernel(const float *__restrict__ spheres, const int
   colour[k] = make_float4(s[3], s[4], s[5], 0.0f);
 }
 
+// pack_spheres_kernel backwards: every record back at its caller-order index (gather_spheres_device)
+__global__ void gather_spheres_kernel(const float4 *__restrict__ geom, const float4 *__restrict__ colour,
+                                      const int32_t *__restrict__ perm, int64_t n, float *__restrict__ out) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const float4 g = geom[k], c = colour[k];
+  float *s = out + 7 * (int64_t)perm[k];
+  s[0] = g.x; s[1] = g.y; s[2] = g.z;
+  s[3] = c.x; s[4] = c.y; s[5] = c.z;
+  s[6] = g.w;
+}
+
 __global__ void finish_kernel(const float *__restrict__ boxes, const int *__restrict__ result, BvhBuildResult *__restrict__ out) {
   for (int c = 0; c < 6; c++) out->root_box[c] = boxes[c];
   out->max_depth = result[0];
@@ -332,6 +344,12 @@ cudaError_t build_bvh_device(const float *d_spheres, int64_t n64, int32_t refit_
   if (launches) *launches += 9 + refit_sweeps + 2 /* cub passes are counted as one each */;
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   return cudaFreeAsync(scratch, stream);
+}
+
+cudaError_t gather_spheres_device(const DeviceBvh &bvh, int64_t n, float *d_out, cudaStream_t stream, int64_t *launches) {
+  gather_spheres_kernel<<<blocks_for(n), kThreads, 0, stream>>>(bvh.geom, bvh.colour, bvh.perm, n, d_out);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
 }
 
 }  // namespace rayb200

@@ -33,5 +33,8 @@ void carve_device_bvh(unsigned char *block, int64_t n, DeviceBvh &out);
 // libm exactly as the reference does (bvh.fut:47).  *d_result is written on the device.
 cudaError_t build_bvh_device(const float *d_spheres, int64_t n, int32_t refit_sweeps, DeviceBvh &out, BvhBuildResult *d_result,
                              cudaStream_t stream, int64_t *launches);
+// The inverse of the build's sphere packing: writes the n sphere records of `bvh` to d_out (n x 7 floats) in the order
+// they were given, sphere[perm[k]] = (geom[k].xyz, colour[k].xyz, geom[k].w), bit for bit.  One launch on `stream`.
+cudaError_t gather_spheres_device(const DeviceBvh &bvh, int64_t n, float *d_out, cudaStream_t stream, int64_t *launches);
 
 }  // namespace rayb200
