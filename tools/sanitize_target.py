@@ -1,9 +1,13 @@
 #!/usr/bin/env python
 """Small renders that exercise every path of the default kernels (K3 warp-queue: item queues, packet walk, sample
 spreading, pixel-bound samples, two frames in flight, compact shard layout, peer-frame flags; K5 lane-walk) for
-compute-sanitizer (tools/sanitize.sh).  No torch: ctypes binding + numpy only; frames are checked against the oracle."""
+compute-sanitizer (tools/sanitize.sh), then every entry point that writes device memory at the small sizes of
+tests/test_memory_contract.py: frames and shards, batches, detile, accumulate, adaptive chains with adaptive_select,
+views, every G-buffer subset, every ray query per-call and ranged, device-prepared scenes with update and read-back,
+the learned claim order and the heavy-first probe.  Every result is checked against the oracle."""
 import os
 import sys
+import traceback
 
 import numpy as np
 
@@ -66,8 +70,37 @@ def main():
                 if staged != want_staged:
                     print(f"warpqueue {tuning} n={n} spp={s}: staged {staged}, expected {want_staged}", flush=True)
                     bad += 1
+    bad += memory_contract_cases()
     print("SANITIZE_TARGET", "OK" if bad == 0 else f"FAILED ({bad})", flush=True)
     return 1 if bad else 0
+
+
+def memory_contract_cases():
+    """The cases of tests/test_memory_contract.py (guarded outputs, sentinel 0xFF), one small size each."""
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import test_memory_contract as M
+    bad = 0
+
+    def run(what, fn, *args):
+        nonlocal bad
+        try:
+            fn(*args)
+            print(f"{what}: ok", flush=True)
+        except Exception:   # a failed check or an error of the call: counted, and the other cases still run
+            bad += 1
+            print(f"{what}: FAILED\n{traceback.format_exc()}", flush=True)
+    e = M.Env(heavy_first=-1)
+    try:
+        for name, (h, w), spp in (("rgbbox", (9, 5), 3), ("irreg", (33, 65), 3), ("comb", (1, 37), 1), ("irreg", (37, 1), 16)):
+            for case in M.FRAME_CASES:
+                run(f"{case.__name__} {name} {h}x{w} spp={spp}", case, e, name, h, w, spp, 0xFF)
+        for name in M.SCENE_NAMES:
+            run(f"queries {name}", M.case_queries, e, name, 33, 0xFF, M.KS, 4)
+            run(f"device scene {name}", M.case_scene_device, e, name, 0xFF)
+        run("learned order and heavy-first frames", M._learned_order_frames, e, 0xFF)
+    finally:
+        e.close()
+    return bad
 
 
 if __name__ == "__main__":
