@@ -77,12 +77,13 @@ int ray_b200_context_trace_warps(struct futhark_context *ctx, int32_t enable);
 int ray_b200_context_warp_trace(struct futhark_context *ctx, float *exit_us, int64_t capacity, int64_t *count);
 /* What a launch traces (struct ray_b200_plan's query): a frame, a chunk of a progressive frame, several views, the
  * selected pixels of an adaptive progressive frame (ADAPTIVE_VAR: with their sample variance), the first hits of a frame's
- * camera rays (GBUFFER: ray_b200_render_gbuffer), or the caller's rays to their closest hit or along their path
- * (trace_hits / trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit). */
+ * camera rays (GBUFFER: ray_b200_render_gbuffer), one frame of each scene of a scene batch (SCENE_BATCH:
+ * ray_b200_render_scene_batch_into), or the caller's rays to their closest hit or along their path (trace_hits /
+ * trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit). */
 enum ray_b200_query {
   RAY_B200_QUERY_PIXELS = 0, RAY_B200_QUERY_CLOSEST = 1, RAY_B200_QUERY_ANYHIT = 2, RAY_B200_QUERY_MULTIHIT = 3,
   RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6, RAY_B200_QUERY_ADAPTIVE_VAR = 7,
-  RAY_B200_QUERY_GBUFFER = 8
+  RAY_B200_QUERY_GBUFFER = 8, RAY_B200_QUERY_SCENE_BATCH = 9
 };
 /* The plan of the last render kernel launch on the context: the last frame, progressive chunk, views call or ray query
  * (for ray_b200_render_batch, its last job), as it was launched.  Calls that launch no render kernel (a query of n = 0
@@ -199,6 +200,55 @@ int ray_b200_prepared_update(struct futhark_context *ctx, struct futhark_opaque_
  * Errors: an invalid prepared scene. */
 int ray_b200_prepared_spheres(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
                               float *spheres_dev, float *cam7_host);
+
+/* ---- scene batches: many small scenes of equal size, built and rendered together ------------------------------------
+ * A caller with B scenes of n spheres each in device memory (vectorised environments, a dataset generator, a sweep over
+ * a model's outputs) builds all B trees in one pass and renders one frame of every scene in one launch, instead of one
+ * prepare and one render call per scene.  spheres_dev: device float[B][n][7], scene b's records at b n 7, each scene in
+ * the layout of ray_b200_scene_from_arrays, 4-byte aligned, readable by the context's device; cams7_host: host
+ * float[B][7], scene b's camera as there.  B = n_scenes >= 1, 2 <= n, B n <= 2^26; every scene has the same n.
+ *   Exactness.  Member b of ray_b200_scene_batch_new_device(h, w, S, B, n, cams7) is bit for bit the prepared scene
+ *   ray_b200_prepare_scene_device(h, w, S + 7 n b, n, cams7 + 7 b) makes: ray_b200_scene_batch_member returns it, and its
+ *   prepared_info (every field), prepared_dump, prepared_packed, prepared_spheres, frames and ray queries are that
+ *   scene's.  Frame b of ray_b200_render_scene_batch_into(h, w, spp) is ray_b200_render_into(h, w, spp) of member b, bit
+ *   for bit (pixels, and the float framebuffer including its NaNs).
+ *   One build, one read-back.  The build runs the kernels of prepare_scene's device build once over all B scenes (a
+ *   stable sort of (scene, Morton key) is each scene's own sort) and ends in one read-back of B x 32 bytes, the members'
+ *   depths, stale counts and root boxes: one synchronisation per batch.  The cameras are made on the host for the
+ *   build's (h, w) as prepare_scene makes them (the aspect ratio w / h), and kept on the device with the root boxes.
+ *   One launch.  ray_b200_render_scene_batch_into renders frame b of scene b for every b in one launch of the warp-queue
+ *   kernel (the h, w of the call set the pixel grid; the cameras are those of the build's h, w, as for a prepared
+ *   scene), planned over all B trees together.  ray_b200_context_last_plan reports RAY_B200_QUERY_SCENE_BATCH;
+ *   last_render_ms and launch_count count it as a render.  The tiles are claimed in the plain chunk permutation (no
+ *   heavy-first probe, no learned claim order), and no prepared scene's learned order is touched.
+ *   Outputs.  out_pix_dev: device int32[B][h][w] (required), frame b at b h w; out_rgb_dev: device float[B][h][w][3] or
+ *   NULL.  Asynchronous on the context's stream.
+ *   Update.  ray_b200_scene_batch_update rebuilds every member from new records of the same B and n (and new cameras,
+ *   or cams7_host == NULL to keep them), as new_device would.  The new trees are built into a new block before the old
+ *   block is released, behind the renders still reading it on either pipeline lane, as a prepared scene's update does:
+ *   frames enqueued before the update read the old trees, and an update that fails leaves the batch as it was.
+ *   Freeing.  ray_b200_scene_batch_free releases the block behind the renders in flight; it is safe to free a batch
+ *   whose frames have not finished.
+ *   Members.  ray_b200_scene_batch_member(b, s) returns member s as a new, independent prepared scene (its own device
+ *   copy of the arrays, indices made local to it; ray_b200_prepared_upload_bytes 0, as for a scene built from device
+ *   memory); it is ordered after the batch's build on the context's stream and outlives updates and the batch itself.
+ *   Errors (nonzero return and a message; the context stays usable, and a failed call leaves an existing batch unchanged
+ *   and usable): the errors of ray_b200_prepare_scene_device and ray_b200_render_into, and n_scenes < 1, B n > 2^26,
+ *   B x tiles(h, w) > 2^25 (tiles(h, w) = ceil(h / 4) ceil(w / 8)), a member index outside [0, B), a NULL batch, a shard
+ *   set (world > 1), a RAY_GPUS > 1 context, and a host_build context (RAY_HOST_BUILD=1: a batch has no host build). */
+struct ray_b200_scene_batch;
+int ray_b200_scene_batch_new_device(struct futhark_context *ctx, struct ray_b200_scene_batch **out, int64_t h, int64_t w,
+                                    const float *spheres_dev, int32_t n_scenes, int64_t n, const float *cams7_host);
+int ray_b200_scene_batch_update(struct futhark_context *ctx, struct ray_b200_scene_batch *b, const float *spheres_dev,
+                                const float *cams7_host);
+int ray_b200_scene_batch_free(struct futhark_context *ctx, struct ray_b200_scene_batch *b);
+/* the batch's B and n */
+int ray_b200_scene_batch_shape(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t *n_scenes,
+                               int64_t *n);
+int ray_b200_scene_batch_member(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t s,
+                                struct futhark_opaque_prepared_scene **out);
+int ray_b200_render_scene_batch_into(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int64_t h,
+                                     int64_t w, int32_t spp, int32_t *out_pix_dev, float *out_rgb_dev);
 
 /* ---- render extensions -------------------------------------------------------------------------- */
 /* render with explicit spp; optional float framebuffer.  out_pix_dev: device int32[h][w] (REQUIRED);

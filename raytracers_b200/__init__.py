@@ -21,7 +21,8 @@ import os
 import numpy as np
 
 __all__ = ["Context", "RayError", "Hit", "Ray", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
-           "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays"]
+           "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays", "SceneBatch", "scene_batch_rows",
+           "scene_batch_cameras", "scene_batch_frames_ok"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 KERNELS = {"auto": 0, "mega": 1, "persistent": 2, "wavefront": 3, "warpqueue": 4, "streamqueue": 5, "lanewalk": 6}
@@ -65,7 +66,7 @@ class Plan(C.Structure):
 
 
 # enum ray_b200_query: what a launch traces (Plan.query)
-QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var", "gbuffer")
+QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var", "gbuffer", "scene_batch")
 
 
 class RenderJob(C.Structure):
@@ -174,6 +175,12 @@ def load_library(variant=""):
         "ray_b200_render_views_into": (C.c_int, [vp, vp, vp, i32, i64, i64, i32, vp, vp]),
         "ray_b200_render_gbuffer": (C.c_int, [vp, vp, i64, i64, i32, vp, vp, vp, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
+        "ray_b200_scene_batch_new_device": (C.c_int, [vp, pp, i64, i64, vp, i32, i64, vp]),
+        "ray_b200_scene_batch_update": (C.c_int, [vp, vp, vp, vp]),
+        "ray_b200_scene_batch_free": (C.c_int, [vp, vp]),
+        "ray_b200_scene_batch_shape": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i64)]),
+        "ray_b200_scene_batch_member": (C.c_int, [vp, vp, i32, pp]),
+        "ray_b200_render_scene_batch_into": (C.c_int, [vp, vp, i64, i64, i32, vp, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
         "ray_b200_shard_tiles_padded": (i64, [i64, i64, i32]),
         "ray_b200_render_shard_into": (C.c_int, [vp, vp, i64, i64, i32, vp]),
@@ -314,6 +321,37 @@ def _sphere_rows(device, spheres):
         raise ValueError("spheres must be a float32 CUDA tensor of shape [n, 7]")
     _check_tensor(device, "spheres", spheres, (torch.float32,), (spheres.shape[0], 7))
     return int(spheres.shape[0])
+
+
+def scene_batch_rows(device, spheres):
+    """(B, n) of spheres, a contiguous float32 CUDA tensor [B, n, 7] on cuda:device with B >= 1, 2 <= n and B n <= 2^26;
+    ValueError for anything else"""
+    import torch
+    if not isinstance(spheres, torch.Tensor) or spheres.dim() != 3:
+        raise ValueError("spheres must be a float32 CUDA tensor of shape [B, n, 7]")
+    B, n = int(spheres.shape[0]), int(spheres.shape[1])
+    _check_tensor(device, "spheres", spheres, (torch.float32,), (B, n, 7))
+    if B < 1 or n < 2:
+        raise ValueError(f"a scene batch needs B >= 1 scenes of n >= 2 spheres, got B = {B}, n = {n}")
+    if B * n > 1 << 26:
+        raise ValueError(f"a scene batch holds at most 2^26 spheres, got {B} x {n}")
+    return B, n
+
+
+def scene_batch_cameras(cams, B):
+    """cams as the contiguous float32 host [B, 7] array the batch calls read, from a host array-like or a tensor of shape
+    [B, 7] with a floating-point dtype (a CUDA tensor is copied to the host, which synchronises); ValueError otherwise."""
+    if type(cams).__module__.startswith("torch"):
+        cams = cams.detach().cpu().numpy()
+    a = np.asarray(cams)
+    if a.shape != (B, 7) or a.dtype.kind != "f":
+        raise ValueError(f"cams must have shape [{B}, 7] and a floating-point dtype, got {a.dtype} {a.shape}")
+    return np.ascontiguousarray(a, np.float32)
+
+
+def scene_batch_frames_ok(B, h, w):
+    """Whether B frames of h x w fit one launch: h, w in [1, 65536] and B x ceil(h / 4) x ceil(w / 8) <= 2^25 tiles"""
+    return 0 < h <= 65536 and 0 < w <= 65536 and B * ((h + 3) // 4) * ((w + 7) // 8) <= 1 << 25
 
 
 def _camera7(cam7):
@@ -476,6 +514,43 @@ class PreparedScene(_Handle):
         return blob
 
 
+class SceneBatch(_Handle):
+    """B scenes of n spheres each, built together from device memory and rendered in one launch
+    (include/ray_b200.h "scene batches")."""
+    _free_fn = "ray_b200_scene_batch_free"
+
+    @property
+    def shape(self):
+        """(B, n)"""
+        b, n = C.c_int32(0), C.c_int64(0)
+        self.ctx._check(self.ctx.lib.ray_b200_scene_batch_shape(self.ctx.handle, self.handle, C.byref(b), C.byref(n)))
+        return int(b.value), int(n.value)
+
+    def update_from_ptr(self, spheres_dev, cams=None):
+        """ray_b200_scene_batch_update: every member rebuilt from the records at device address spheres_dev (float[B][n][7],
+        read on the context's stream) and the host cameras cams ([B, 7], None keeps them)."""
+        c = None if cams is None else scene_batch_cameras(cams, self.shape[0])
+        self.ctx._check(self.ctx.lib.ray_b200_scene_batch_update(self.ctx.handle, self.handle, _ptr(spheres_dev), _ptr(c)))
+
+    def update(self, spheres, cams=None):
+        """Rebuilds every member from spheres, a contiguous float32 CUDA tensor of the batch's shape [B, n, 7], and cams
+        ([B, 7], see scene_batch_cameras) or None to keep the cameras.  Frames enqueued before the call render the old
+        trees.  Waits for torch's current stream before the call."""
+        import torch
+        B, n = scene_batch_rows(self.ctx.device, spheres)
+        if (B, n) != self.shape:
+            raise ValueError(f"spheres must have the batch's shape {list(self.shape) + [7]}, got {list(spheres.shape)}")
+        c = None if cams is None else scene_batch_cameras(cams, B)
+        torch.cuda.current_stream(spheres.device).synchronize()   # spheres may still be in flight on torch's stream
+        self.update_from_ptr(spheres.data_ptr(), c)
+
+    def member(self, b):
+        """Member b as a new, independent PreparedScene: bit for bit what Context.prepare_scene_device makes of its records."""
+        out = C.c_void_p(None)
+        self.ctx._check(self.ctx.lib.ray_b200_scene_batch_member(self.ctx.handle, self.handle, int(b), C.byref(out)))
+        return PreparedScene(self.ctx, out.value)
+
+
 class Image(_Handle):
     """`[h][w]i32` (ray.fut:164): packed 0x00RRGGBB, row 0 = top; lives on the device."""
     _free_fn = "futhark_free_i32_2d"
@@ -577,6 +652,46 @@ class Context:
         c = _camera7(cam7)
         torch.cuda.current_stream(spheres.device).synchronize()   # spheres may still be in flight on torch's stream
         return self.prepare_scene_device_from_ptr(h, w, spheres.data_ptr(), n, c)
+
+    def prepare_scene_batch_from_ptr(self, h, w, spheres_dev, B, n, cams):
+        """ray_b200_scene_batch_new_device: B scenes of n spheres from device address spheres_dev (float[B][n][7], read on
+        the context's stream) with the host cameras cams ([B, 7]).  Returns after the build's one read-back."""
+        c = scene_batch_cameras(cams, int(B))
+        return self._out(SceneBatch, "ray_b200_scene_batch_new_device", int(h), int(w), _ptr(spheres_dev), int(B), int(n), _ptr(c))
+
+    def prepare_scene_batch(self, h, w, spheres, cams):
+        """A SceneBatch from spheres, a contiguous float32 CUDA tensor [B, n, 7] on the context's device (each scene in the
+        layout of scene_from_arrays), and cams, [B, 7] cameras on the host or in a tensor.  Member b equals
+        prepare_scene_device(h, w, spheres[b], cams[b]) bit for bit.  Waits for torch's current stream before the call."""
+        import torch
+        B, n = scene_batch_rows(self.device, spheres)
+        if not scene_batch_frames_ok(B, int(h), int(w)):
+            raise ValueError(f"{B} frames of {h}x{w} exceed one launch (2^25 tiles of 8x4 pixels, sides <= 65536)")
+        c = scene_batch_cameras(cams, B)
+        torch.cuda.current_stream(spheres.device).synchronize()
+        return self.prepare_scene_batch_from_ptr(h, w, spheres.data_ptr(), B, n, c)
+
+    def render_scene_batch_into(self, batch, h, w, spp, out_pix_dev, out_rgb_dev=None):
+        """One frame of every scene of a SceneBatch in one launch (ray_b200_render_scene_batch_into): out_pix_dev = device
+        int32[B][h][w], out_rgb_dev = device float[B][h][w][3] or None.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_render_scene_batch_into(self.handle, batch.handle, int(h), int(w), int(spp),
+                                                              _ptr(out_pix_dev), _ptr(out_rgb_dev)))
+
+    def render_scene_batch(self, batch, h, w, spp=1, want_rgb=False):
+        """Renders frame b of scene b for every member of a SceneBatch and returns CUDA int32 [B, h, w] pixels, and with
+        want_rgb also the float32 [B, h, w, 3] framebuffers, as (pixels, rgb).  Frame b equals render_into of member b bit
+        for bit.  Waits for torch's current stream before, and synchronises the context after the call."""
+        import torch
+        B = batch.shape[0]
+        if not scene_batch_frames_ok(B, int(h), int(w)):
+            raise ValueError(f"{B} frames of {h}x{w} exceed one launch (2^25 tiles of 8x4 pixels, sides <= 65536)")
+        dev = torch.device("cuda", self.device)
+        pix = torch.empty((B, int(h), int(w)), dtype=torch.int32, device=dev)
+        rgb = torch.empty((B, int(h), int(w), 3), dtype=torch.float32, device=dev) if want_rgb else None
+        torch.cuda.current_stream(dev).synchronize()
+        self.render_scene_batch_into(batch, h, w, spp, pix.data_ptr(), rgb.data_ptr() if rgb is not None else None)
+        self.sync()
+        return (pix, rgb) if want_rgb else pix
 
     def render(self, h, w, prepared, spp=None):
         if spp is None:

@@ -44,7 +44,7 @@ int resolve_kernel(const futhark_context *ctx);
 void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P) {
   memset(&P, 0, sizeof P);
   P.nodes = p->dev.nodes; P.nodes_soa = p->dev.nodes_soa; P.geom = p->dev.geom; P.colour = p->dev.colour;
-  P.n_inner = (int32_t)(p->n - 1); P.n_leaves = (int32_t)p->n;
+  P.n_inner = (int32_t)n_inner_of(p); P.n_leaves = (int32_t)n_leaves_of(p);
   P.max_depth = p->max_depth;
   memcpy(P.root_box, p->root_box, sizeof P.root_box);
 }
@@ -74,7 +74,7 @@ static_assert((int)Query::kPixels == RAY_B200_QUERY_PIXELS && (int)Query::kClose
                   (int)Query::kAnyHit == RAY_B200_QUERY_ANYHIT && (int)Query::kMultiHit == RAY_B200_QUERY_MULTIHIT &&
                   (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS &&
                   (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE && (int)Query::kAdaptiveVar == RAY_B200_QUERY_ADAPTIVE_VAR &&
-                  (int)Query::kGBuffer == RAY_B200_QUERY_GBUFFER,
+                  (int)Query::kGBuffer == RAY_B200_QUERY_GBUFFER && (int)Query::kSceneBatch == RAY_B200_QUERY_SCENE_BATCH,
               "enum ray_b200_query names the values of Query");
 static_assert(sizeof(struct ray_b200_plan) == 80, "struct ray_b200_plan is 16 int32 and 2 int64");
 
@@ -113,14 +113,14 @@ static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
 // Fills the kernel parameter block for frame f, and the frame's launch plan.  Every kind but kPixels runs on the warp-queue
 // kernel whatever the context's kernel is, planned as a frame of f.spp samples (spread or pixel-bound by that count).
 // Query::kAccumulate reads the offset table of the whole frame from the chunk's first sample on and scales by 1/s_end.
-// Query::kViews: the work items are the tiles of all q.n_views frames, so the plan (K, staging, the sample buffer) is
-// that of one frame of n_views x tiles(h, w) tiles.  The adaptive kinds are planned over all tiles, an upper bound on
+// Query::kViews and kSceneBatch: the work items are the tiles of all q.n_views frames, so the plan (K, staging, the sample
+// buffer) is that of one frame of n_views x tiles(h, w) tiles (a scene batch's over all its trees, see n_inner_of).  The adaptive kinds are planned over all tiles, an upper bound on
 // their work (the selection is on the device).  A pixel-bound kind (Query::kGBuffer) is planned as a frame whose samples
 // are not spread.
 int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc) {
   const futhark_opaque_prepared_scene *p = f.scene;
   const int64_t h = f.h, w = f.w; const int32_t spp = f.spp;
-  const bool views = f.kind == Query::kViews;
+  const bool views = is_multi_frame(f.kind);
   if (!p || !p->dev.nodes) { set_error(ctx, "render: invalid prepared scene"); return 1; }
   if (!image_size_ok(h, w)) {
     set_error(ctx, "render: bad image size %lldx%lld", (long long)h, (long long)w);
@@ -128,7 +128,8 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   }
   if (views && tiles_total(h, w) * f.q.n_views > ((int64_t)1 << 25)) {
     // ... and per launch: at most 2^30 padded pixels over all views
-    set_error(ctx, "render_views: %d views of %lldx%lld exceed 2^30 padded pixels", f.q.n_views, (long long)h, (long long)w);
+    set_error(ctx, "%s: %d %s of %lldx%lld exceed 2^30 padded pixels", f.kind == Query::kViews ? "render_views" : "render_scene_batch",
+              f.q.n_views, f.kind == Query::kViews ? "views" : "frames", (long long)h, (long long)w);
     return 1;
   }
   if (spp < 1) { set_error(ctx, "render: spp must be >= 1"); return 1; }
@@ -205,7 +206,7 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
     const int scap = lw_stack_capacity(p->max_depth);
     int64_t w = ctx->cfg.lw_warps < 1 ? 32 : std::min<int64_t>(ctx->cfg.lw_warps, kWqMaxWarps);
     int64_t r = ctx->cfg.lw_slots < 1 ? 48 : (ctx->cfg.lw_slots >= 64 ? 64 : (ctx->cfg.lw_slots >= 48 ? 48 : 32));  // 32 / 48 / 64 are built
-    const int64_t full_stage = 128 + (int64_t)(p->n - 1) * 64 + (int64_t)p->n * 16;
+    const int64_t full_stage = 128 + n_inner_of(p) * 64 + n_leaves_of(p) * 16;
     const int64_t want_stage = std::min<int64_t>(full_stage, 16 * 1024);
     while (w * (int64_t)lw_warp_bytes((int)r, scap) + want_stage + 1024 > (int64_t)ctx->max_smem_optin) {
       if (r > 32) r -= 16;
@@ -227,7 +228,7 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
 // Shared memory not used by the warp-queue / lane-walk kernels stays L1: a tree far larger than the caches gains more from
 // 60-100 KB of L1 for its hot middle levels than from a few hundred more staged top nodes.  Returns the staging budget.
 int64_t cap_staging(const futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t budget) {
-  const bool huge = (int64_t)(p->n - 1) * 64 > ((int64_t)8 << 20);
+  const bool huge = n_inner_of(p) * 64 > ((int64_t)8 << 20);
   // the carve-out granule below the maximum is 196 KB (sm_90: 228 KB of shared memory + L1 per SM): staying under it
   // leaves the SM 32 KB of L1 instead of ~0
   const int64_t queues = (int64_t)ctx->max_smem_optin - 512 - budget;
@@ -239,7 +240,7 @@ int64_t cap_staging(const futhark_context *ctx, const futhark_opaque_prepared_sc
 
 // Staging area of `budget` bytes: BFS prefix of the node array, then the sphere records if they all fit.
 void split_staging(const futhark_opaque_prepared_scene *p, int64_t budget, int32_t &smem_nodes, int32_t &smem_spheres) {
-  const int32_t n_inner = (int32_t)(p->n - 1), n_leaves = (int32_t)p->n;
+  const int32_t n_inner = (int32_t)n_inner_of(p), n_leaves = (int32_t)n_leaves_of(p);
   const int64_t nodes_fit = std::max<int64_t>(0, budget / 64);
   smem_nodes = (int32_t)std::min<int64_t>(n_inner, nodes_fit);
   const int64_t left = budget - (int64_t)smem_nodes * 64;
@@ -263,7 +264,7 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
     int ncap_cfg = ctx->cfg.wq_ncap, warps_cfg = ctx->cfg.wq_warps;
     bool auto_k2 = false;
     if (ctx->cfg.wq_k == 0 && pass == 0) {
-      const int64_t scene_bytes = 128 + (int64_t)(p->n - 1) * 64 + (int64_t)p->n * 16;
+      const int64_t scene_bytes = 128 + n_inner_of(p) * 64 + n_leaves_of(p) * 16;
       const int64_t pw2 = (int64_t)wq_warp_bytes(2, wq_node_capacity(2, p->max_depth, kAutoK2Ncap), false, will_spread);
       int64_t w2 = ((int64_t)ctx->max_smem_optin - scene_bytes - 512 - 128) / pw2;   // as many warps as still leave the scene whole
       if (w2 > kWqMaxWarps) w2 = kWqMaxWarps;
@@ -292,7 +293,7 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
       while (wq_w > 1 && wq_w * per_warp + 8192 > (int64_t)ctx->max_smem_optin) wq_w--;
       if (want_packet >= 0) break;
       const int64_t b = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512 - 128;
-      const bool fully_staged = b / 64 >= (int64_t)(p->n - 1);
+      const bool fully_staged = b / 64 >= n_inner_of(p);
       want_packet = (!fully_staged && coherent) ? 24 : 0;
       if (want_packet != 0) break;  // the first plan (with packets) stands
     }
@@ -306,7 +307,7 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
     split_staging(p, cap_staging(ctx, p, budget), P.smem_nodes, P.smem_spheres);
     // belt and braces: the K = 2 plan is only worth anything when the scene is staged whole (a scene that just misses
     // fetches its lower nodes from L2 with half the warps); if anything above left it short, plan again with K = 1
-    if (!auto_k2 || (P.smem_nodes == (int32_t)(p->n - 1) && P.smem_spheres == (int32_t)p->n)) break;
+    if (!auto_k2 || (P.smem_nodes == (int32_t)n_inner_of(p) && P.smem_spheres == (int32_t)n_leaves_of(p))) break;
   }
   return 0;
 }
@@ -982,3 +983,24 @@ int ray_b200_count_work(struct futhark_context *ctx, int64_t h, int64_t w, int32
 }
 
 }  // extern "C"
+
+extern "C" int ray_b200_render_scene_batch_into(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int64_t h,
+                                                int64_t w, int32_t spp, int32_t *out_pix_dev, float *out_rgb_dev) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  const char *what = "render_scene_batch_into";
+  if (!ctx->peers.empty()) { set_error(ctx, "%s: not available on a single-process multi-GPU context (RAY_GPUS > 1)", what); return 1; }
+  if (ctx->cfg.world > 1) { set_error(ctx, "%s: not available with a shard set (rank %d of %d)", what, ctx->cfg.rank, ctx->cfg.world); return 1; }
+  if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
+  if (!out_pix_dev) { set_error(ctx, "%s: out_pix_dev is required", what); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  // one launch over every member's tree: the scene half of the parameters comes from all of them (fill_scene_params over
+  // n_inner_of / n_leaves_of), and each member's camera and root box from the batch's device tables
+  Frame f{&b->scene, h, w, spp, 0, 1, out_pix_dev, out_rgb_dev};
+  f.kind = Query::kSceneBatch;
+  f.q.n_views = b->scene.scenes;
+  f.q.cams = b->scene.dev.cams;
+  f.q.root_boxes = reinterpret_cast<const float *>(b->scene.dev.results);
+  f.q.scene_inner = (int32_t)(b->scene.n - 1);
+  return render_frame(ctx, f);
+}

@@ -89,7 +89,7 @@ void free_prepared_device(futhark_context *ctx, futhark_opaque_prepared_scene *p
 int build_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p, const float *d_spheres, int64_t n, bool drop_order) {
   const int32_t sweeps = (int32_t)log2f((float)n) + 2;  // bvh.fut:47, host libm as in the reference's C backend
   DeviceBvh fresh;
-  cudaError_t e = build_bvh_device(d_spheres, n, sweeps, fresh, ctx->d_build_result, ctx->stream, &ctx->launches);
+  cudaError_t e = build_bvh_device(d_spheres, n, 1, sweeps, fresh, ctx->d_build_result, ctx->stream, &ctx->launches);
   // the host needs the tree depth (stack sizing) and the root box (kernel parameter) before the first render
   if (e == cudaSuccess)
     e = cudaMemcpyAsync(ctx->h_build_result, ctx->d_build_result, sizeof(BvhBuildResult), cudaMemcpyDeviceToHost, ctx->stream);
@@ -593,6 +593,154 @@ void ray_b200_host_sample_offsets(int32_t spp, float *table) {
   std::vector<float> t;
   sample_offsets(spp, t);
   memcpy(table, t.data(), t.size() * sizeof(float));
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------ scene batches
+namespace {
+
+// The checks every batch entry point shares (an error here changes nothing)
+int check_batch_context(futhark_context *ctx, const char *what) {
+  if (!ctx->peers.empty()) { set_error(ctx, "%s: not available on a single-process multi-GPU context (RAY_GPUS > 1)", what); return 1; }
+  if (ctx->cfg.world > 1) { set_error(ctx, "%s: not available with a shard set (rank %d of %d)", what, ctx->cfg.rank, ctx->cfg.world); return 1; }
+  if (ctx->cfg.host_build) { set_error(ctx, "%s: a scene batch has no host build (RAY_HOST_BUILD / tuning host_build is set)", what); return 1; }
+  return 0;
+}
+
+// The trees of bt's B scenes of n spheres from the records at spheres_dev and the cameras cams7 (host [B][7]) made for
+// bt's (h, w): built into a new block, then the old one is released behind the renders still reading it.  One read-back
+// of the B build results ends the call.  A failed build leaves bt as it was.
+int build_batch(futhark_context *ctx, ray_b200_scene_batch *bt, const float *spheres_dev, int32_t B, int64_t n, const float *cams7) {
+  futhark_opaque_prepared_scene *p = &bt->scene;
+  const int32_t sweeps = (int32_t)log2f((float)n) + 2;  // bvh.fut:47, as build_on_device
+  const size_t cam_bytes = (size_t)B * sizeof(CameraRec), res_bytes = (size_t)B * sizeof(BvhBuildResult);
+  static_assert(sizeof(CameraRec) == 48 && sizeof(BvhBuildResult) == 32, "the batch's device tables");
+  if (acquire_pinned(ctx, p, cam_bytes + res_bytes)) return 1;
+  CameraRec *cams = reinterpret_cast<CameraRec *>(p->pinned);
+  BvhBuildResult *res = reinterpret_cast<BvhBuildResult *>(p->pinned + cam_bytes);
+  for (int32_t b = 0; b < B; b++) {  // what prepare_scene makes of the camera: make_camera for the build's (h, w)
+    HostScene s;
+    const float *c = cams7 + 7 * (size_t)b;
+    memcpy(s.look_from, c, 12); memcpy(s.look_at, c + 3, 12); s.fov = c[6];
+    cams[b] = make_camera(s, bt->h, bt->w);
+  }
+  DeviceBvh fresh;
+  cudaError_t e = build_bvh_device(spheres_dev, n, B, sweeps, fresh, nullptr, ctx->stream, &ctx->launches);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(fresh.cams, cams, cam_bytes, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(res, fresh.results, res_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaEventRecord(p->pinned_event, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) {
+    if (fresh.block) cudaFreeAsync(fresh.block, ctx->stream);
+    set_error(ctx, "scene_batch: device LBVH build failed: %s", cudaGetErrorString(e));
+    return 1;
+  }
+  if (release_scene_block(ctx, p, true)) { cudaFreeAsync(fresh.block, ctx->stream); return 1; }
+  p->dev = fresh;
+  p->n = n;
+  p->scenes = B;
+  p->refit_sweeps = sweeps;
+  memset(p->root_box, 0, sizeof p->root_box);  // (each member's is in p->dev.results)
+  p->max_depth = 0;
+  for (int32_t b = 0; b < B; b++) p->max_depth = std::max(p->max_depth, res[b].max_depth);
+  p->host_current = false;
+  p->host_built = false;
+  bt->results.assign(res, res + B);
+  if (cams7 != bt->cams7.data()) bt->cams7.assign(cams7, cams7 + 7 * (size_t)B);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ray_b200_scene_batch_new_device(struct futhark_context *ctx, struct ray_b200_scene_batch **out, int64_t h, int64_t w,
+                                    const float *spheres_dev, int32_t n_scenes, int64_t n, const float *cams7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  const char *what = "scene_batch_new_device";
+  if (!out || !cams7_host) { set_error(ctx, "%s: null argument", what); return 1; }
+  if (h <= 0 || w <= 0) { set_error(ctx, "%s: bad image size", what); return 1; }
+  if (n_scenes < 1) { set_error(ctx, "%s: n_scenes must be >= 1, got %d", what, n_scenes); return 1; }
+  if (check_batch_context(ctx, what)) return 1;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (check_device_records(ctx, what, spheres_dev, n)) return 1;
+  if ((int64_t)n_scenes * n > ((int64_t)1 << 26)) {
+    set_error(ctx, "%s: %d scenes of %lld spheres exceed 2^26 spheres (this build packs leaf indices into 26 bits)", what, n_scenes, (long long)n);
+    return 1;
+  }
+  if ((int64_t)n_scenes * tiles_total(h, w) > ((int64_t)1 << 25)) {
+    set_error(ctx, "%s: %d frames of %lldx%lld exceed 2^30 padded pixels", what, n_scenes, (long long)h, (long long)w);
+    return 1;
+  }
+  ray_b200_scene_batch *bt = new ray_b200_scene_batch;
+  bt->h = bt->scene.h = h;
+  bt->w = bt->scene.w = w;
+  if (build_batch(ctx, bt, spheres_dev, n_scenes, n, cams7_host)) { free_prepared_device(ctx, &bt->scene); delete bt; return 1; }
+  *out = bt;
+  return 0;
+}
+
+int ray_b200_scene_batch_update(struct futhark_context *ctx, struct ray_b200_scene_batch *b, const float *spheres_dev,
+                                const float *cams7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  const char *what = "scene_batch_update";
+  if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
+  if (check_batch_context(ctx, what)) return 1;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (check_device_records(ctx, what, spheres_dev, b->scene.n)) return 1;
+  return build_batch(ctx, b, spheres_dev, b->scene.scenes, b->scene.n, cams7_host ? cams7_host : b->cams7.data());
+}
+
+int ray_b200_scene_batch_free(struct futhark_context *ctx, struct ray_b200_scene_batch *b) {
+  if (!b) return 0;
+  if (ctx && ctx->ok) {
+    std::lock_guard<std::mutex> g(ctx->mu);
+    cudaSetDevice(ctx->cfg.device);
+    free_prepared_device(ctx, &b->scene);  // stream-ordered behind the renders that read it, on either lane
+  }
+  delete b;
+  return 0;
+}
+
+int ray_b200_scene_batch_shape(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t *n_scenes, int64_t *n) {
+  if (bad_ctx(ctx)) return 1;
+  if (!b) { set_error(ctx, "scene_batch_shape: invalid scene batch"); return 1; }
+  if (n_scenes) *n_scenes = b->scene.scenes;
+  if (n) *n = b->scene.n;
+  return 0;
+}
+
+int ray_b200_scene_batch_member(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t s,
+                                struct futhark_opaque_prepared_scene **out) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  const char *what = "scene_batch_member";
+  if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
+  if (!out) { set_error(ctx, "%s: null argument", what); return 1; }
+  if (s < 0 || s >= b->scene.scenes) { set_error(ctx, "%s: member %d is outside [0, %d)", what, s, b->scene.scenes); return 1; }
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  futhark_opaque_prepared_scene *p = new futhark_opaque_prepared_scene;
+  p->h = b->h; p->w = b->w;
+  set_camera(p, b->cams7.data() + 7 * (size_t)s);
+  const cudaError_t e = extract_scene_device(b->scene.dev, s, b->scene.n, p->dev, ctx->stream, &ctx->launches);
+  if (e != cudaSuccess) {
+    set_error(ctx, "%s: %s", what, cudaGetErrorString(e));
+    free_prepared_device(ctx, p); delete p;
+    return 1;
+  }
+  ctx->lane(0);
+  if (record_scene_use(ctx, &b->scene, 0)) { free_prepared_device(ctx, p); delete p; return 1; }  // an update or free waits for the copy
+  const BvhBuildResult &r = b->results[(size_t)s];
+  memcpy(p->root_box, r.root_box, sizeof p->root_box);
+  p->max_depth = r.max_depth; p->stale_nodes = r.stale_nodes; p->refit_sweeps = b->scene.refit_sweeps;
+  p->n = b->scene.n;
+  p->host_current = false;
+  p->host_built = false;
+  *out = p;
+  return 0;
 }
 
 }  // extern "C"

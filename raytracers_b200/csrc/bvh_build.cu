@@ -12,6 +12,14 @@
 //                                                       the reference renders with the stale boxes this leaves)
 //   layout                           (ours)            node depth by parent walk, stable sort by depth (= order by
 //                                                       (depth, Karras index), the same order pack_bvh uses), pack
+//
+// Scene batches (DESIGN.md §5b): B scenes of n spheres each, side by side in one sphere array, are built in the same
+// launches.  Every kernel knows its element's scene (k / n for spheres, i / (n - 1) for inner nodes): one box per scene
+// for the Morton keys, one stable sort on (scene << 32 | key), which is each scene's own stable sort, the radix tree of
+// each scene's key segment with global child, leaf and parent indices, and one stable sort on (scene, depth) for the
+// layout, so scene b's nodes are one block in its own (depth, Karras index) order and its root is node b (n - 1).  The
+// refit only follows child indices and is the same for one scene or many.  B = 1 is the single-scene build, with its
+// 32-bit key sorts.
 #include "bvh_build.h"
 
 #include <cub/cub.cuh>
@@ -44,25 +52,39 @@ __device__ __forceinline__ SphereBox sphere_box(const float *sp) {
   return b;
 }
 
-// bvh.fut:31-37: centre of every sphere box (prim.fut:47-50) and the six min/max reductions over them.
-__global__ void centres_minmax_kernel(const float *__restrict__ spheres, int n, float *__restrict__ cx,
-                                      float *__restrict__ cy, float *__restrict__ cz, int *__restrict__ minmax /* [6] ordered ints */) {
-  float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    const SphereBox b = sphere_box(spheres + 7 * (size_t)k);
-    const float c[3] = {b.lo[0] + 0.5f * (b.hi[0] - b.lo[0]), b.lo[1] + 0.5f * (b.hi[1] - b.lo[1]),
-                        b.lo[2] + 0.5f * (b.hi[2] - b.lo[2])};
-    cx[k] = c[0]; cy[k] = c[1]; cz[k] = c[2];
-    for (int a = 0; a < 3; a++) { lo[a] = fminf(lo[a], c[a]); hi[a] = fmaxf(hi[a], c[a]); }
+// Identity elements of the min / max reductions, as ordered ints (any real float beats them), and zeroed per-scene
+// results: minmax [scenes][6], result [scenes][2]
+__global__ void init_build_kernel(int *__restrict__ minmax, int *__restrict__ result, int scenes) {
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < scenes; s += gridDim.x * blockDim.x) {
+    for (int a = 0; a < 3; a++) { minmax[6 * (size_t)s + a] = 0x7fffffff; minmax[6 * (size_t)s + 3 + a] = (int)0x80000000; }
+    result[2 * (size_t)s] = 0;
+    result[2 * (size_t)s + 1] = 0;
   }
-  for (int a = 0; a < 3; a++) {
-    for (int o = 16; o > 0; o >>= 1) {
-      lo[a] = fminf(lo[a], __shfl_down_sync(0xffffffffu, lo[a], o));
-      hi[a] = fmaxf(hi[a], __shfl_down_sync(0xffffffffu, hi[a], o));
+}
+
+// bvh.fut:31-37: centre of every sphere box (prim.fut:47-50) and the six min/max reductions over them, per scene: the
+// y blocks walk the scenes, the x blocks stride over one scene's n spheres as they do over a single scene's.
+__global__ void centres_minmax_kernel(const float *__restrict__ spheres, int n, int scenes, float *__restrict__ cx,
+                                      float *__restrict__ cy, float *__restrict__ cz, int *__restrict__ minmax /* [scenes][6] ordered ints */) {
+  for (int sc = blockIdx.y; sc < scenes; sc += gridDim.y) {
+    const size_t base = (size_t)sc * n;
+    float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+    for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+      const SphereBox b = sphere_box(spheres + 7 * (base + k));
+      const float c[3] = {b.lo[0] + 0.5f * (b.hi[0] - b.lo[0]), b.lo[1] + 0.5f * (b.hi[1] - b.lo[1]),
+                          b.lo[2] + 0.5f * (b.hi[2] - b.lo[2])};
+      cx[base + k] = c[0]; cy[base + k] = c[1]; cz[base + k] = c[2];
+      for (int a = 0; a < 3; a++) { lo[a] = fminf(lo[a], c[a]); hi[a] = fmaxf(hi[a], c[a]); }
     }
-    if ((threadIdx.x & 31) == 0) {
-      atomicMin(minmax + a, float_to_ordered(lo[a]));
-      atomicMax(minmax + 3 + a, float_to_ordered(hi[a]));
+    for (int a = 0; a < 3; a++) {
+      for (int o = 16; o > 0; o >>= 1) {
+        lo[a] = fminf(lo[a], __shfl_down_sync(0xffffffffu, lo[a], o));
+        hi[a] = fmaxf(hi[a], __shfl_down_sync(0xffffffffu, hi[a], o));
+      }
+      if ((threadIdx.x & 31) == 0) {
+        atomicMin(minmax + 6 * (size_t)sc + a, float_to_ordered(lo[a]));
+        atomicMax(minmax + 6 * (size_t)sc + 3 + a, float_to_ordered(hi[a]));
+      }
     }
   }
 }
@@ -78,25 +100,41 @@ __device__ __forceinline__ uint32_t quantise10(float t) {  // bvh.fut:16-18; NaN
   return (uint32_t)fminf(fmaxf(t * 1024.0f, 0.0f), 1023.0f);
 }
 
-// bvh.fut:38-41 + morton_3D (bvh.fut:15-22)
-__global__ void morton_kernel(const float *__restrict__ cx, const float *__restrict__ cy, const float *__restrict__ cz, int n,
-                              const int *__restrict__ minmax, uint32_t *__restrict__ key, int32_t *__restrict__ idx) {
+// bvh.fut:38-41 + morton_3D (bvh.fut:15-22) over `total` spheres, with the box of each sphere's scene (n per scene).
+// A batch (key64 != NULL) writes the scene above the key: sorting (scene, key) stably sorts every scene on its own.
+__global__ void morton_kernel(const float *__restrict__ cx, const float *__restrict__ cy, const float *__restrict__ cz, int total,
+                              int n, const int *__restrict__ minmax_all, uint32_t *__restrict__ key, uint64_t *__restrict__ key64,
+                              int32_t *__restrict__ idx) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= n) return;
+  if (k >= total) return;
+  const int sc = k / n;
+  const int *minmax = minmax_all + 6 * (size_t)sc;
   const float lo[3] = {ordered_to_float(minmax[0]), ordered_to_float(minmax[1]), ordered_to_float(minmax[2])};
   const float hi[3] = {ordered_to_float(minmax[3]), ordered_to_float(minmax[4]), ordered_to_float(minmax[5])};
   const uint32_t qx = quantise10((cx[k] - lo[0]) / (hi[0] - lo[0]));
   const uint32_t qy = quantise10((cy[k] - lo[1]) / (hi[1] - lo[1]));
   const uint32_t qz = quantise10((cz[k] - lo[2]) / (hi[2] - lo[2]));
-  key[k] = spread10(qx) * 4u + spread10(qy) * 2u + spread10(qz);
+  const uint32_t m = spread10(qx) * 4u + spread10(qy) * 2u + spread10(qz);
+  if (key64) key64[k] = (uint64_t)sc << 32 | m;
+  else key[k] = m;
   idx[k] = k;
 }
 
-// mk_radix_tree (radixtree.fut:11-72): one thread per inner node.
-__global__ void karras_kernel(const uint32_t *__restrict__ M, int n, int32_t *__restrict__ left, int32_t *__restrict__ right,
-                              int32_t *__restrict__ parent) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n - 1) return;
+// a batch's sorted (scene, key) pairs -> the 32-bit keys the radix tree reads
+__global__ void low_keys_kernel(const uint64_t *__restrict__ key64, int total, uint32_t *__restrict__ key) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < total) key[k] = (uint32_t)key64[k];
+}
+
+// mk_radix_tree (radixtree.fut:11-72): one thread per inner node of `scenes` trees over n keys each.  Scene sc's thread i
+// works on its scene's keys with local indices and writes global ones: inner node i -> sc (n - 1) + i, leaf i -> sc n + i.
+__global__ void karras_kernel(const uint32_t *__restrict__ M_all, int n, int scenes, int32_t *__restrict__ left,
+                              int32_t *__restrict__ right, int32_t *__restrict__ parent) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= scenes * (n - 1)) return;
+  const int sc = g / (n - 1), i = g - sc * (n - 1);
+  const int inner0 = sc * (n - 1), leaf0 = sc * n;
+  const uint32_t *M = M_all + leaf0;
   auto delta = [&](int a, int b) -> int {  // radixtree.fut:13-21
     if (b < 0 || b >= n) return -1;
     const uint32_t x = M[a], y = M[b];
@@ -119,12 +157,12 @@ __global__ void karras_kernel(const uint32_t *__restrict__ M, int n, int32_t *__
     if (delta(i, i + (split + step) * d) > node_cp) split += step;
   }
   const int gamma = i + split * d + min(d, 0);                   // :51
-  const int l = (min(i, j) == gamma) ? ~gamma : gamma;           // :54-57
-  const int r = (max(i, j) == gamma + 1) ? ~(gamma + 1) : gamma + 1;  // :59-62
-  left[i] = l;
-  right[i] = r;
-  if (l >= 0) parent[l] = i;                                     // :66-70 (scatter; the root keeps -1)
-  if (r >= 0) parent[r] = i;
+  const int l = (min(i, j) == gamma) ? ~(leaf0 + gamma) : inner0 + gamma;             // :54-57
+  const int r = (max(i, j) == gamma + 1) ? ~(leaf0 + gamma + 1) : inner0 + gamma + 1;  // :59-62
+  left[g] = l;
+  right[g] = r;
+  if (l >= 0) parent[l] = g;                                     // :66-70 (scatter; the root keeps -1)
+  if (r >= 0) parent[r] = g;
 }
 
 // The min / max of enclosing (prim.fut:38-45) with -0.0 below +0.0, as the host builder and the oracle define it:
@@ -156,15 +194,20 @@ __global__ void refit_kernel(const float *__restrict__ src, float *__restrict__ 
   for (int c = 0; c < 3; c++) { o[c] = min_num(a[c], b[c]); o[3 + c] = max_num(a[3 + c], b[3 + c]); }  // enclosing, prim.fut:38-45
 }
 
-// diagnostics + layout keys: depth of every inner node (root = 0) and how many boxes are not the union of their children
+// diagnostics + layout keys: depth of every inner node (root = 0) and how many boxes are not the union of their children,
+// per scene (ni_scene inner nodes each).  A batch (key64 != NULL) writes (scene, depth) as the layout key.
 __global__ void depth_stale_kernel(const float *__restrict__ boxes, const int32_t *__restrict__ left, const int32_t *__restrict__ right,
                                    const int32_t *__restrict__ parent, const float *__restrict__ spheres, const int32_t *__restrict__ perm,
-                                   int ni, uint32_t *__restrict__ depth, int32_t *__restrict__ node_id, int *__restrict__ result /* [0]=max depth,[1]=stale */) {
+                                   int ni, int ni_scene, uint32_t *__restrict__ depth, uint64_t *__restrict__ key64,
+                                   int32_t *__restrict__ node_id, int *__restrict__ result_all /* [scenes][2]: max depth, stale */) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= ni) return;
+  const int sc = k / ni_scene;
+  int *result = result_all + 2 * (size_t)sc;
   int d = 0;
   for (int p = parent[k]; p >= 0; p = parent[p]) d++;
-  depth[k] = (uint32_t)d;
+  if (key64) key64[k] = (uint64_t)sc << 8 | (uint32_t)d;
+  else depth[k] = (uint32_t)d;
   node_id[k] = k;
   atomicMax(result, d + 1);  // + the leaf level
   float a[6], b[6];
@@ -235,33 +278,68 @@ __global__ void gather_spheres_kernel(const float4 *__restrict__ geom, const flo
   s[6] = g.w;
 }
 
-__global__ void finish_kernel(const float *__restrict__ boxes, const int *__restrict__ result, BvhBuildResult *__restrict__ out) {
-  for (int c = 0; c < 6; c++) out->root_box[c] = boxes[c];
-  out->max_depth = result[0];
-  out->stale_nodes = result[1];
+// per scene: its root box (its Karras root, inner node sc (ni_scene)), depth and stale count
+__global__ void finish_kernel(const float *__restrict__ boxes, const int *__restrict__ result, int scenes, int ni_scene,
+                              BvhBuildResult *__restrict__ out) {
+  for (int sc = blockIdx.x * blockDim.x + threadIdx.x; sc < scenes; sc += gridDim.x * blockDim.x) {
+    const float *b = boxes + 6 * (size_t)sc * ni_scene;
+    for (int c = 0; c < 6; c++) out[sc].root_box[c] = b[c];
+    out[sc].max_depth = result[2 * (size_t)sc];
+    out[sc].stale_nodes = result[2 * (size_t)sc + 1];
+  }
+}
+
+// Scene s of a batch as a scene of its own: its blocks of every array, indices made local to it
+__device__ __forceinline__ int32_t local_ptr(int32_t p, int32_t inner0, int32_t leaf0) { return p >= 0 ? p - inner0 : ~(~p - leaf0); }
+
+__global__ void extract_scene_kernel(const DeviceBvh src, int32_t s, int n, const DeviceBvh dst) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  const int ni = n - 1, inner0 = s * ni, leaf0 = s * n;
+  if (k < ni) {
+    float4 q[4];
+    for (int c = 0; c < 4; c++) q[c] = src.nodes[4 * ((size_t)inner0 + k) + c];
+    q[0].w = __int_as_float(local_ptr(__float_as_int(q[0].w), inner0, leaf0));
+    q[1].w = __int_as_float(local_ptr(__float_as_int(q[1].w), inner0, leaf0));
+    for (int c = 0; c < 4; c++) {
+      dst.nodes[4 * (size_t)k + c] = q[c];
+      dst.nodes_soa[(size_t)c * ni + k] = q[c];
+    }
+    dst.left[k] = local_ptr(src.left[inner0 + k], inner0, leaf0);
+    dst.right[k] = local_ptr(src.right[inner0 + k], inner0, leaf0);
+    const int32_t par = src.parent[inner0 + k];
+    dst.parent[k] = par < 0 ? par : par - inner0;
+    for (int c = 0; c < 6; c++) dst.boxes[6 * (size_t)k + c] = src.boxes[6 * ((size_t)inner0 + k) + c];
+  }
+  if (k < n) {
+    dst.geom[k] = src.geom[(size_t)leaf0 + k];
+    dst.colour[k] = src.colour[(size_t)leaf0 + k];
+    dst.morton[k] = src.morton[(size_t)leaf0 + k];
+    dst.perm[k] = src.perm[(size_t)leaf0 + k] - leaf0;
+  }
 }
 
 size_t align_up(size_t v) { return (v + 255) & ~(size_t)255; }
 
 }  // namespace
 
-size_t device_bvh_bytes(int64_t n) {
-  const size_t ni = (size_t)(n - 1);
+size_t device_bvh_bytes(int64_t n, int32_t scenes, bool tables) {
+  const size_t ni = (size_t)scenes * (size_t)(n - 1), nl = (size_t)scenes * (size_t)n;
   size_t b = 0;
   b += 2 * align_up(ni * 64);       // nodes, nodes_soa
-  b += 2 * align_up((size_t)n * 16);  // geom, colour
-  b += 2 * align_up((size_t)n * 4);   // morton, perm
+  b += 2 * align_up(nl * 16);       // geom, colour
+  b += 2 * align_up(nl * 4);        // morton, perm
   b += 3 * align_up(ni * 4);        // left, right, parent
   b += align_up(ni * 24);           // boxes
+  if (tables) b += align_up((size_t)scenes * sizeof(BvhBuildResult)) + align_up((size_t)scenes * 48);  // results, cameras
   return b;
 }
 
-void carve_device_bvh(unsigned char *block, int64_t n64, DeviceBvh &out) {
-  const size_t n = (size_t)n64, ni = n - 1;
+void carve_device_bvh(unsigned char *block, int64_t n64, DeviceBvh &out, int32_t scenes, bool tables) {
+  const size_t ni = (size_t)scenes * (size_t)(n64 - 1), n = (size_t)scenes * (size_t)n64;
   unsigned char *p = block;
   auto carve = [&](size_t bytes) { unsigned char *r = p; p += align_up(bytes); return r; };
   out.block = block;
-  out.block_bytes = device_bvh_bytes(n64);
+  out.block_bytes = device_bvh_bytes(n64, scenes, tables);
   out.nodes = (float4 *)carve(ni * 64);
   out.nodes_soa = (float4 *)carve(ni * 64);
   out.geom = (float4 *)carve(n * 16);
@@ -272,59 +350,81 @@ void carve_device_bvh(unsigned char *block, int64_t n64, DeviceBvh &out) {
   out.right = (int32_t *)carve(ni * 4);
   out.parent = (int32_t *)carve(ni * 4);
   out.boxes = (float *)carve(ni * 24);
+  if (tables) {
+    out.results = (BvhBuildResult *)carve((size_t)scenes * sizeof(BvhBuildResult));
+    out.cams = (float *)carve((size_t)scenes * 48);
+  }
   out.n = (int32_t)n;
 }
 
-cudaError_t build_bvh_device(const float *d_spheres, int64_t n64, int32_t refit_sweeps, DeviceBvh &out, BvhBuildResult *d_result,
-                             cudaStream_t stream, int64_t *launches) {
-  const int n = (int)n64, ni = n - 1;
+cudaError_t build_bvh_device(const float *d_spheres, int64_t n64, int32_t scenes, int32_t refit_sweeps, DeviceBvh &out,
+                             BvhBuildResult *d_result, cudaStream_t stream, int64_t *launches) {
+  const int n = (int)n64, ni_scene = n - 1, total = scenes * n, ni = scenes * ni_scene;
+  const bool batch = scenes > 1;
+  int key_bits = 32, scene_bits = 0;  // a batch sorts (scene, key) and (scene, depth): the scene takes bits(scenes - 1)
+  while (batch && ((int64_t)1 << scene_bits) < scenes) scene_bits++;
+  key_bits += scene_bits;
   cudaError_t e;
   // ---- persistent outputs: one block, carved
   unsigned char *blk = nullptr;
-  if ((e = cudaMallocAsync(&blk, device_bvh_bytes(n), stream)) != cudaSuccess) return e;
-  carve_device_bvh(blk, n, out);
+  const bool tables = d_result == nullptr;  // a scene batch: the results go to its own table
+  if ((e = cudaMallocAsync(&blk, device_bvh_bytes(n, scenes, tables), stream)) != cudaSuccess) return e;
+  carve_device_bvh(blk, n, out, scenes, tables);
+  if (tables) d_result = out.results;
   unsigned char *p = nullptr;
   auto carve = [&](size_t bytes) { unsigned char *r = p; p += align_up(bytes); return r; };
 
   // ---- scratch: one block, freed (stream-ordered) at the end
   size_t sort_tmp = 0, sort_tmp2 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const int32_t *)nullptr,
-                                  (int32_t *)nullptr, n, 0, 32, stream);
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp2, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const int32_t *)nullptr,
-                                  (int32_t *)nullptr, ni, 0, 8, stream);
+  if (batch) {
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const int32_t *)nullptr,
+                                    (int32_t *)nullptr, total, 0, key_bits, stream);
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp2, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const int32_t *)nullptr,
+                                    (int32_t *)nullptr, ni, 0, 8 + scene_bits, stream);
+  } else {
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const int32_t *)nullptr,
+                                    (int32_t *)nullptr, n, 0, 32, stream);
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp2, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const int32_t *)nullptr,
+                                    (int32_t *)nullptr, ni, 0, 8, stream);
+  }
   const size_t cub_bytes = sort_tmp > sort_tmp2 ? sort_tmp : sort_tmp2;
-  const size_t scratch_bytes = 3 * align_up((size_t)n * 4) /* cx cy cz */ + 2 * align_up((size_t)n * 4) /* key idx */ +
-                               align_up((size_t)ni * 24) /* boxes ping-pong */ + 4 * align_up((size_t)ni * 4) /* depth ids order newidx */ +
-                               align_up((size_t)ni * 4) /* depth sorted */ + align_up(64) + align_up(cub_bytes);
+  const size_t kw = batch ? 8 : 4;  // bytes of a sort key
+  const size_t scratch_bytes = 3 * align_up((size_t)total * 4) /* cx cy cz */ + 2 * align_up((size_t)total * kw) /* key, sorted key (batch) */ +
+                               align_up((size_t)total * 4) /* idx */ + align_up((size_t)ni * 24) /* boxes ping-pong */ +
+                               3 * align_up((size_t)ni * 4) /* ids order newidx */ + 2 * align_up((size_t)ni * kw) /* depth, depth sorted */ +
+                               align_up((size_t)scenes * 24) /* min/max */ + align_up((size_t)scenes * 8) /* depth, stale */ + align_up(cub_bytes);
   unsigned char *scratch = nullptr;
   if ((e = cudaMallocAsync(&scratch, scratch_bytes, stream)) != cudaSuccess) return e;
   p = scratch;
-  float *cx = (float *)carve((size_t)n * 4), *cy = (float *)carve((size_t)n * 4), *cz = (float *)carve((size_t)n * 4);
-  uint32_t *key = (uint32_t *)carve((size_t)n * 4);
-  int32_t *idx = (int32_t *)carve((size_t)n * 4);
+  float *cx = (float *)carve((size_t)total * 4), *cy = (float *)carve((size_t)total * 4), *cz = (float *)carve((size_t)total * 4);
+  void *key = carve((size_t)total * kw), *key_sorted = carve((size_t)total * kw);
+  int32_t *idx = (int32_t *)carve((size_t)total * 4);
   float *boxes_b = (float *)carve((size_t)ni * 24);
-  uint32_t *depth = (uint32_t *)carve((size_t)ni * 4);
+  void *depth = carve((size_t)ni * kw), *depth_sorted = carve((size_t)ni * kw);
   int32_t *node_id = (int32_t *)carve((size_t)ni * 4);
   int32_t *order = (int32_t *)carve((size_t)ni * 4);
   int32_t *newidx = (int32_t *)carve((size_t)ni * 4);
-  uint32_t *depth_sorted = (uint32_t *)carve((size_t)ni * 4);
-  int *small = (int *)carve(64);  // [0..5] min/max as ordered ints, [8] max depth, [9] stale
+  int *minmax = (int *)carve((size_t)scenes * 24);  // [scenes][6] min/max as ordered ints
+  int *result = (int *)carve((size_t)scenes * 8);   // [scenes][2] max depth, stale
   void *cub_tmp = carve(cub_bytes);
 
   // ---- bvh.fut:31-41
-  const int init[6] = {0x7fffffff, 0x7fffffff, 0x7fffffff, (int)0x80000000, (int)0x80000000, (int)0x80000000};
-  // ordered-int identity elements: +inf-ish for min, -inf-ish for max (any real float beats them)
-  cudaMemsetAsync(small, 0, 64, stream);
-  cudaMemcpyAsync(small, init, sizeof init, cudaMemcpyHostToDevice, stream);
+  init_build_kernel<<<blocks_for(scenes), kThreads, 0, stream>>>(minmax, result, scenes);
   unsigned rb = blocks_for(n);
   if (rb > 1056) rb = 1056;  // 132 SMs x 8: grid-stride reduction
-  centres_minmax_kernel<<<rb, kThreads, 0, stream>>>(d_spheres, n, cx, cy, cz, small);
-  morton_kernel<<<blocks_for(n), kThreads, 0, stream>>>(cx, cy, cz, n, small, key, idx);
-  // ---- bvh.fut:43 stable sort by the 32-bit key
-  cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp, key, out.morton, idx, out.perm, n, 0, 32, stream);
+  centres_minmax_kernel<<<dim3(rb, scenes < 65535 ? scenes : 65535), kThreads, 0, stream>>>(d_spheres, n, scenes, cx, cy, cz, minmax);
+  morton_kernel<<<blocks_for(total), kThreads, 0, stream>>>(cx, cy, cz, total, n, minmax, (uint32_t *)key,
+                                                            batch ? (uint64_t *)key : nullptr, idx);
+  // ---- bvh.fut:43 stable sort by the 32-bit key (a batch: by (scene, key))
+  if (batch) {
+    cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp, (uint64_t *)key, (uint64_t *)key_sorted, idx, out.perm, total, 0, key_bits, stream);
+    low_keys_kernel<<<blocks_for(total), kThreads, 0, stream>>>((const uint64_t *)key_sorted, total, out.morton);
+  } else {
+    cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp, (uint32_t *)key, out.morton, idx, out.perm, n, 0, 32, stream);
+  }
   // ---- radixtree.fut
   cudaMemsetAsync(out.parent, 0xff, (size_t)ni * 4, stream);
-  karras_kernel<<<blocks_for(ni), kThreads, 0, stream>>>(out.morton, n, out.left, out.right, out.parent);
+  karras_kernel<<<blocks_for(ni), kThreads, 0, stream>>>(out.morton, n, scenes, out.left, out.right, out.parent);
   // ---- bvh.fut:44-58 fixed number of Jacobi sweeps from zero boxes; the last sweep must land in out.boxes
   float *src = (refit_sweeps % 2 == 0) ? out.boxes : boxes_b, *dst = (refit_sweeps % 2 == 0) ? boxes_b : out.boxes;
   cudaMemsetAsync(src, 0, (size_t)ni * 24, stream);
@@ -333,21 +433,34 @@ cudaError_t build_bvh_device(const float *d_spheres, int64_t n64, int32_t refit_
     float *t = src; src = dst; dst = t;
   }
   // (src now points at the final boxes == out.boxes)
-  // ---- layout: order nodes by (depth, Karras index), pack
-  depth_stale_kernel<<<blocks_for(ni), kThreads, 0, stream>>>(out.boxes, out.left, out.right, out.parent, d_spheres, out.perm, ni, depth,
-                                                               node_id, small + 8);
-  cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp2, depth, depth_sorted, node_id, order, ni, 0, 8, stream);
+  // ---- layout: order nodes by (depth, Karras index) (a batch: by (scene, depth, Karras index)), pack
+  depth_stale_kernel<<<blocks_for(ni), kThreads, 0, stream>>>(out.boxes, out.left, out.right, out.parent, d_spheres, out.perm, ni, ni_scene,
+                                                               (uint32_t *)depth, batch ? (uint64_t *)depth : nullptr, node_id, result);
+  if (batch)
+    cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp2, (uint64_t *)depth, (uint64_t *)depth_sorted, node_id, order, ni, 0, 8 + scene_bits, stream);
+  else
+    cub::DeviceRadixSort::SortPairs(cub_tmp, sort_tmp2, (uint32_t *)depth, (uint32_t *)depth_sorted, node_id, order, ni, 0, 8, stream);
   invert_kernel<<<blocks_for(ni), kThreads, 0, stream>>>(order, ni, newidx);
   pack_nodes_kernel<<<blocks_for(ni), kThreads, 0, stream>>>(out.boxes, out.left, out.right, order, newidx, ni, out.nodes, out.nodes_soa);
-  pack_spheres_kernel<<<blocks_for(n), kThreads, 0, stream>>>(d_spheres, out.perm, n, out.geom, out.colour);
-  finish_kernel<<<1, 1, 0, stream>>>(out.boxes, small + 8, d_result);
-  if (launches) *launches += 9 + refit_sweeps + 2 /* cub passes are counted as one each */;
+  pack_spheres_kernel<<<blocks_for(total), kThreads, 0, stream>>>(d_spheres, out.perm, total, out.geom, out.colour);
+  finish_kernel<<<blocks_for(scenes), kThreads, 0, stream>>>(out.boxes, result, scenes, ni_scene, d_result);
+  if (launches) *launches += 10 + (batch ? 1 : 0) + refit_sweeps + 2 /* cub passes are counted as one each */;
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   return cudaFreeAsync(scratch, stream);
 }
 
 cudaError_t gather_spheres_device(const DeviceBvh &bvh, int64_t n, float *d_out, cudaStream_t stream, int64_t *launches) {
   gather_spheres_kernel<<<blocks_for(n), kThreads, 0, stream>>>(bvh.geom, bvh.colour, bvh.perm, n, d_out);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+cudaError_t extract_scene_device(const DeviceBvh &batch, int32_t s, int64_t n, DeviceBvh &out, cudaStream_t stream, int64_t *launches) {
+  cudaError_t e;
+  unsigned char *blk = nullptr;
+  if ((e = cudaMallocAsync(&blk, device_bvh_bytes(n), stream)) != cudaSuccess) return e;
+  carve_device_bvh(blk, n, out);
+  extract_scene_kernel<<<blocks_for(n), kThreads, 0, stream>>>(batch, s, (int)n, out);
   if (launches) *launches += 1;
   return cudaGetLastError();
 }

@@ -192,12 +192,12 @@ __device__ __forceinline__ Ray camera_ray(const float *c, const float u, const f
 // at s = 0 of the frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  The adaptive
 // kinds: s is relative to the pixel's own first sample c, and the offsets of its sample c + s are computed here exactly as
 // sample_offsets computes them on the host (the same f32 products, floorf and differences; -fmad=false keeps them apart):
-// each pixel continues from its own count, so there is no one table for the launch.  Query::kViews: the camera is
-// view_cam, the pixel's view's 12 floats of RayQuery::cams, instead of P.cam.
+// each pixel continues from its own count, so there is no one table for the launch.  Query::kViews and kSceneBatch: the
+// camera is view_cam, the pixel's view's (scene's) 12 floats of RayQuery::cams, instead of P.cam.
 template <Query kKind = Query::kPixels>
 __device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, int s, const float *view_cam = nullptr,
                                            int c = 0) {
-  constexpr bool kAccum = kKind == Query::kAccumulate, kViews = kKind == Query::kViews;
+  constexpr bool kAccum = kKind == Query::kAccumulate, kViews = is_multi_frame(kKind);
   float u, v;
   if constexpr (is_adaptive(kKind)) {
     const float a = (float)(c + s) * 0.7548776662f, b = (float)(c + s) * 0.5698402909f;
@@ -264,11 +264,12 @@ __device__ __forceinline__ int claim_to_item(const RenderParams &P, int c) {
 
 // Query::kAccumulate: the sum of a progressive frame's samples [0, s_end), always scaled by P.inv_spp = 1/s_end (1 * x = x
 // when s_end = 1; a NaN stays some NaN), and the pixel frame is optional (row-major only).  The adaptive kinds: as
-// kAccumulate, with s_end = n, the pixel's own sample count after the launch.  Query::kViews: pixel (i, j) of view `view`,
-// whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the float frames 12 GiB)
+// kAccumulate, with s_end = n, the pixel's own sample count after the launch.  Query::kViews and kSceneBatch: pixel
+// (i, j) of view (scene) `view`, whose frames follow each other (row-major; 64-bit offsets: V x H x W reaches 2^30, the
+// float frames 12 GiB)
 template <Query kKind = Query::kPixels>
 __device__ __forceinline__ void write_pixel(const RenderParams &P, int k, int i, int j, V3 sum, int view = 0, int n = 0) {
-  constexpr bool kProg = is_progressive(kKind), kViews = kKind == Query::kViews;
+  constexpr bool kProg = is_progressive(kKind), kViews = is_multi_frame(kKind);
   const float inv = is_adaptive(kKind) ? 1.0f / (float)n : P.inv_spp;
   const V3 col = (!kProg && P.spp == 1) ? sum : vscale(inv, sum);
   const int pix = pack_pixel(col);
@@ -449,6 +450,7 @@ cudaError_t with_query(F &&f, Query q) {
     case Query::kAdaptive: return f(std::integral_constant<Query, Query::kAdaptive>{});
     case Query::kAdaptiveVar: return f(std::integral_constant<Query, Query::kAdaptiveVar>{});
     case Query::kGBuffer: return f(std::integral_constant<Query, Query::kGBuffer>{});
+    case Query::kSceneBatch: return f(std::integral_constant<Query, Query::kSceneBatch>{});
     default: return cudaErrorInvalidValue;
   }
 }

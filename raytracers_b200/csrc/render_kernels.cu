@@ -264,6 +264,15 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // sample into the pixel's sums; a slot owns its pixel (pixel-bound only, the launcher never gives this kind a
 // finished-sample buffer), and p_sum / p_light carry the normal and albedo sums, so no shared memory is added and the
 // plan, the staging and wq_warp_bytes are those of a pixel-bound Query::kPixels frame.
+//
+// Query::kSceneBatch, one frame of each scene of a scene batch (include/ray_b200.h ray_b200_render_scene_batch_into): the
+// work items, cameras and outputs of a views launch (frame b = scene b), over B trees that lie side by side in P's arrays
+// with global child and leaf indices, so a ray that starts at scene b's root only ever reaches scene b's nodes and
+// spheres.  What depends on the scene is where a segment starts: its set-up tests scene b's root box (Q.root_boxes, not
+// P.root_box) and pushes scene b's root node b * Q.scene_inner, for camera rays and bounces alike; b is the slot's work
+// item's tile over Q.view_tiles, so the slot carries nothing more.  The packet walk takes the new rays of one scene, the
+// first new ray's; the others of the round start in the item queue.  Nodes and spheres are staged as for one tree (a BFS prefix of the concatenated node array, or all of
+// it), the plan is made over the totals and the deepest member, and the claim order is the plain chunk permutation.
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -279,9 +288,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                                                                    const int packet_min, const int refill_min, const int nlow,
                                                                    const __grid_constant__ RayQuery Q) {
   constexpr bool kRays = is_ray_query(kQuery);  // ray mode
-  constexpr bool kAccum = kQuery == Query::kAccumulate, kViews = kQuery == Query::kViews;
+  constexpr bool kAccum = kQuery == Query::kAccumulate;
   constexpr bool kProg = is_progressive(kQuery), kAdapt = is_adaptive(kQuery), kVar = kQuery == Query::kAdaptiveVar;
-  constexpr bool kGBuf = kQuery == Query::kGBuffer;
+  constexpr bool kGBuf = kQuery == Query::kGBuffer, kBatch = kQuery == Query::kSceneBatch, kFrames = is_multi_frame(kQuery);
   static_assert(!kRays || (!kSpread && !kPacket), "ray mode traces one ray per slot without spread samples or the packet walk");
   static_assert(!is_pixel_bound(kQuery) || !kSpread, "a pixel-bound kind is launched without a finished-sample buffer");
   static_assert(!kRanged || kRays, "per-ray intervals belong to ray queries");
@@ -351,14 +360,17 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   [[maybe_unused]] auto count_of = [&](const int pi, const int pj) { return Q.sample_counts + ((size_t)pj * P.W + pi); };
   // kVar: the M2 of pixel (row pj, column pi), laid out as its sum
   [[maybe_unused]] auto m2_of = [&](const int pi, const int pj) { return Q.m2 + 3 * ((size_t)pj * P.W + pi); };
-  // pixel item -> (view, column, row), false for a padding pixel; the view is 0 unless kViews
+  // pixel item -> (view, column, row), false for a padding pixel; the view (kSceneBatch: the scene) is 0 unless kFrames
   auto pixel_of = [&](const int item, int &pv, int &pi, int &pj) {
-    if constexpr (kViews) return item_view_pixel(P, item, pv, pi, pj);
+    if constexpr (kFrames) return item_view_pixel(P, item, pv, pi, pj);
     pv = 0;
     return item_pixel(P, item, pi, pj);
   };
-  // kViews: the camera of view pv (its 12 floats of Q.cams)
-  [[maybe_unused]] auto view_cam = [&](const int pv) -> const float * { return kViews ? Q.cams + 12 * (size_t)pv : nullptr; };
+  // kFrames: the camera of view (scene) pv (its 12 floats of Q.cams)
+  [[maybe_unused]] auto view_cam = [&](const int pv) -> const float * { return kFrames ? Q.cams + 12 * (size_t)pv : nullptr; };
+  // kSceneBatch: the scene of the pixel in `slot` (work-item tiles [b view_tiles, (b + 1) view_tiles) are scene b's), so
+  // neither the slot nor wq_warp_bytes carries it
+  [[maybe_unused]] auto scene_of = [&](const int slot) { return (int)((unsigned)(p_item[slot] >> 5) / (unsigned)Q.view_tiles); };
   // The first sample c of pixel (row pj, column pi) in this launch: 0 for a whole frame or views, the chunk's first sample
   // (kAccum), the pixel's own count (kAdapt).  Sample s of the launch is sample c + s of the pixel (primary_ray<kQuery>
   // makes its ray), and the pixel's in-order sum continues from Q.accum exactly when c > 0; otherwise its sample 0 starts it.
@@ -730,7 +742,15 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             r.d = v3(rd.x, rd.y, rd.z);
             const RayInv q = ray_invariants(r);
             const float lo = kRanged ? ro.w : t_lo, hi = kRanged ? rd.w : t_hi;
-            if (box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, lo, hi)) {
+            bool root_hit;
+            if constexpr (kBatch) {  // every segment starts at its scene's root: that scene's box (two 16-byte loads)
+              const float4 *bx = reinterpret_cast<const float4 *>(Q.root_boxes) + 2 * (size_t)scene_of(slot);
+              const float4 b0 = __ldg(bx), b1 = __ldg(bx + 1);
+              root_hit = box_hit(b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, r, q, lo, hi);
+            } else {
+              root_hit = box_hit(P.root_box[0], P.root_box[1], P.root_box[2], P.root_box[3], P.root_box[4], P.root_box[5], r, q, lo, hi);
+            }
+            if (root_hit) {
               if constexpr (kRanged) {
                 ray_i[slot] = make_float4(q.ix, q.iy, q.iz, hi);
                 ray_d[slot] = make_float4(rd.x, rd.y, rd.z, q.a);
@@ -928,9 +948,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     // a shared-memory broadcast), each lane testing its own slot's ray, leaf children tested inline by the owner lanes
     // (plain read-modify-write of their own `best` word).  As soon as fewer than `packet_min` lanes are left on a node
     // the remaining (ray, node) pairs are handed to the item queue, where lanes are bound to items instead of rays.
-    [[maybe_unused]] auto packet_walk = [&](const int k, unsigned mask) {
+    [[maybe_unused]] auto packet_walk = [&](const int k, unsigned mask, const int root) {
       const int slot = lane + 32 * k;
-      int cur = 0, psp = 0;
+      int cur = root, psp = 0;
       for (;;) {
         const int cnt = __popc(mask);
         bool descended = false;
@@ -1000,12 +1020,31 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     for (int k = 0; k < K; k++) {
       const unsigned gm = k == 0 ? gomask0 : gomask1;
       if (kPacket && packet_min > 0) {
-        if constexpr (kPacket) {
-          if (gm) packet_walk(k, gm);
+        if constexpr (kPacket && kBatch) {
+          // a packet walks one tree: the rays of the first new ray's scene go as a packet, the others (a warp's tiles
+          // straddle at most a few scene boundaries) start at their own scene's root in the item queue
+          if (gm) {
+            const bool go = (gm >> lane) & 1u;
+            const int root = go ? scene_of(lane + 32 * k) * Q.scene_inner : -1;
+            const int r0 = __shfl_sync(kFullMask, root, __ffs(gm) - 1);
+            const unsigned same = __ballot_sync(kFullMask, root == r0) & gm, other = gm & ~same;
+            if (other) {
+              if (ntop + 32 + 96 > ncap) drain();
+              if ((other >> lane) & 1u) nstk[ntop + __popc(other & lt_mask)] = ((uint32_t)(lane + 32 * k) << kSlotShift) | (uint32_t)root;
+              ntop += __popc(other);
+            }
+            packet_walk(k, same, r0);
+          }
+        } else if constexpr (kPacket) {
+          if (gm) packet_walk(k, gm, 0);
         }
       } else {
         const bool go = (gm >> lane) & 1u;
-        if (go) nstk[ntop + __popc(gm & lt_mask)] = (uint32_t)(lane + 32 * k) << kSlotShift;  // (slot, root node 0)
+        if constexpr (kBatch) {  // (slot, its scene's root node)
+          if (go) nstk[ntop + __popc(gm & lt_mask)] = ((uint32_t)(lane + 32 * k) << kSlotShift) | (uint32_t)(scene_of(lane + 32 * k) * Q.scene_inner);
+        } else {
+          if (go) nstk[ntop + __popc(gm & lt_mask)] = (uint32_t)(lane + 32 * k) << kSlotShift;  // (slot, root node 0)
+        }
         ntop += __popc(gm);
       }
     }
@@ -1165,9 +1204,9 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
       }, k == 2, all_nodes, sph, ranged);
     else
       return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {
-        // (the adaptive and pixel-bound kinds are not built for every sphere staged without every node, which
-        // split_staging never plans; the pixel-bound kinds have no spread variants)
-        if constexpr ((is_adaptive(query) || is_pixel_bound(query)) && s && !a) return cudaErrorInvalidValue;
+        // (the adaptive, pixel-bound and scene-batch kinds are not built for every sphere staged without every node,
+        // which split_staging never plans; the pixel-bound kinds have no spread variants)
+        if constexpr ((is_adaptive(query) || is_pixel_bound(query) || query == Query::kSceneBatch) && s && !a) return cudaErrorInvalidValue;
         else if constexpr (is_pixel_bound(query) && sp) return cudaErrorInvalidValue;
         else
           return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, sp, pk, a, s, query>>(

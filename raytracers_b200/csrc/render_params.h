@@ -67,9 +67,10 @@ struct RenderParams {
 // progressive frame, each from its own sample count (accum, sample_counts, mask, sel, n_sel).  kAdaptiveVar: kAdaptive
 // that also keeps each pixel's running sum of squared deviations (m2).  kGBuffer, a pixel kind: the first hit of every
 // camera ray of a frame (its sphere, t, normal and albedo), reduced per pixel into the guide buffers (gb_id, gb_depth,
-// gb_normal, gb_albedo, gb_coverage).  New kinds go at the end: kernel names carry the values, and tools/sass_compare.py
-// reads older builds' names by them.
-enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar, kGBuffer };
+// gb_normal, gb_albedo, gb_coverage).  kSceneBatch, a pixel kind: one frame of each scene of a scene batch (cams, n_views,
+// view_tiles as kViews, root_boxes, scene_inner).  New kinds go at the end: kernel names carry the values, and
+// tools/sass_compare.py reads older builds' names by them.
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar, kGBuffer, kSceneBatch };
 __host__ __device__ constexpr bool is_ray_query(Query q) {
   return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
 }
@@ -85,7 +86,10 @@ __host__ __device__ constexpr bool is_progressive(Query q) { return q == Query::
 __host__ __device__ constexpr bool is_pixel_bound(Query q) { return q == Query::kGBuffer; }
 // Pixel kinds that claim the frame's tiles in the plain chunk permutation: a launch uses neither the heavy-first probe
 // nor the learned claim order, and leaves the learned order as it found it
-__host__ __device__ constexpr bool is_plain_order(Query q) { return is_progressive(q) || q == Query::kGBuffer; }
+__host__ __device__ constexpr bool is_plain_order(Query q) { return is_progressive(q) || q == Query::kGBuffer || q == Query::kSceneBatch; }
+// Pixel kinds whose work items are the tiles of several frames, one after the other (RayQuery::view_tiles each), each
+// frame drawn with its own camera of RayQuery::cams and written at its own offset
+__host__ __device__ constexpr bool is_multi_frame(Query q) { return q == Query::kViews || q == Query::kSceneBatch; }
 
 // The fields of a launch that RenderParams does not carry (see Query for which kind reads which).  A block of its own,
 // passed after the kernel's scalar parameters: new fields at the end of RenderParams would move those parameters, and
@@ -134,6 +138,13 @@ struct RayQuery {
   float *gb_normal;
   float *gb_albedo;
   int32_t *gb_coverage;
+  // a scene batch (Query::kSceneBatch; include/ray_b200.h ray_b200_render_scene_batch_into): n_views = B frames as kViews
+  // lays them out, frame b of scene b with the camera cams[b].  The B trees lie side by side in P's arrays with global
+  // indices, scene_inner inner nodes each, so scene b's root is node b * scene_inner; its root box is the first 6 floats of
+  // root_boxes[8 b .. 8 b + 8) (struct BvhBuildResult records, 32-byte aligned), tested at every segment's set-up instead
+  // of P.root_box
+  const float *root_boxes;
+  int32_t scene_inner;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.
