@@ -79,11 +79,14 @@ int ray_b200_context_warp_trace(struct futhark_context *ctx, float *exit_us, int
  * selected pixels of an adaptive progressive frame (ADAPTIVE_VAR: with their sample variance), the first hits of a frame's
  * camera rays (GBUFFER: ray_b200_render_gbuffer), one frame of each scene of a scene batch (SCENE_BATCH:
  * ray_b200_render_scene_batch_into), or the caller's rays to their closest hit or along their path (trace_hits /
- * trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit). */
+ * trace_paths), to their first hit (occlusion), or to their k nearest hits (multi-hit), and the same three kinds of ray
+ * query on the scenes of a scene batch (SCENE_BATCH_CLOSEST for hits and paths, SCENE_BATCH_ANYHIT, SCENE_BATCH_MULTIHIT:
+ * ray_b200_scene_batch_trace_*). */
 enum ray_b200_query {
   RAY_B200_QUERY_PIXELS = 0, RAY_B200_QUERY_CLOSEST = 1, RAY_B200_QUERY_ANYHIT = 2, RAY_B200_QUERY_MULTIHIT = 3,
   RAY_B200_QUERY_ACCUMULATE = 4, RAY_B200_QUERY_VIEWS = 5, RAY_B200_QUERY_ADAPTIVE = 6, RAY_B200_QUERY_ADAPTIVE_VAR = 7,
-  RAY_B200_QUERY_GBUFFER = 8, RAY_B200_QUERY_SCENE_BATCH = 9
+  RAY_B200_QUERY_GBUFFER = 8, RAY_B200_QUERY_SCENE_BATCH = 9, RAY_B200_QUERY_SCENE_BATCH_CLOSEST = 10,
+  RAY_B200_QUERY_SCENE_BATCH_ANYHIT = 11, RAY_B200_QUERY_SCENE_BATCH_MULTIHIT = 12
 };
 /* The plan of the last render kernel launch on the context: the last frame, progressive chunk, views call or ray query
  * (for ray_b200_render_batch, its last job), as it was launched.  Calls that launch no render kernel (a query of n = 0
@@ -249,6 +252,47 @@ int ray_b200_scene_batch_member(struct futhark_context *ctx, const struct ray_b2
                                 struct futhark_opaque_prepared_scene **out);
 int ray_b200_render_scene_batch_into(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int64_t h,
                                      int64_t w, int32_t spp, int32_t *out_pix_dev, float *out_rgb_dev);
+/* Ray queries of a scene batch: range sensors, line of sight, shadow rays, picking and depth-complexity lists traced in
+ * every scene of a batch in one launch, one entry point for each single-scene ray query ("ray queries" below).  There are
+ * m rays per scene: rays_dev is device float[B][m][6] (ranged: struct ray_b200_ray[B][m]), so ray i of the flat array
+ * belongs to scene i / m, and the outputs follow the same order: hits_dev struct ray_b200_hit[B][m], rgb_dev
+ * float[B][m][3], segments_dev int32[B][m] (or NULL), occluded_dev uint8_t[B][m], multi-hit hits_dev
+ * struct ray_b200_hit[B][m][k] and counts_dev int32[B][m] (or NULL); record offsets are 64-bit.  A caller with fewer rays
+ * in some scenes pads them with ranged rays whose interval is empty, such as (0, 0): they get the empty answer.
+ *   Exactness.  The answer for ray j of scene b is bit for bit what the single-scene entry point returns for that ray on
+ *   ray_b200_scene_batch_member(b), and so on ray_b200_prepare_scene_device of scene b's records: every word of every
+ *   hit record (sphere is the index into scene b's own records, in [0, n)), the colours including their NaNs, segments,
+ *   occluded and counts.  Every interval rule of the single-scene queries holds as it is (epsilon 0.1 and the
+ *   re-intersection of trace_hits, no epsilon for occlusion and multi-hit, (0, 1e9) for paths, the empty answer for an
+ *   invalid per-ray interval).
+ *   One launch.  Each call is one launch of the warp-queue kernel over the B m rays, each ray traced from its own scene's
+ *   root, planned over all B trees together; asynchronous on the context's stream.  ray_b200_context_last_plan reports
+ *   RAY_B200_QUERY_SCENE_BATCH_CLOSEST (hits and paths), _ANYHIT or _MULTIHIT, with n_inner and n_leaves the batch's
+ *   totals; last_render_ms and launch_count count it as a single-scene query.  A shard setting is ignored.
+ *   Updates and freeing.  A query enqueued before ray_b200_scene_batch_update reads the old trees, one enqueued after it
+ *   the new ones; the batch may be freed while a query that reads it is in flight.
+ *   Errors (nonzero return and a message; the context stays usable): those of the single-scene query (a non-finite
+ *   interval or t_min < 0 in the per-call forms, max_depth outside [0, 65535], k outside [1, 64], a NULL buffer with
+ *   m > 0), and a NULL or invalid batch, m < 0 and B m > 2^30.  m == 0 does nothing; max_depth == 0 writes zeros without
+ *   a launch. */
+struct ray_b200_hit;
+struct ray_b200_ray;
+int ray_b200_scene_batch_trace_hits(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, const float *rays_dev,
+                                    int64_t m, float t_min, float t_max, struct ray_b200_hit *hits_dev);
+int ray_b200_scene_batch_trace_paths(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, const float *rays_dev,
+                                     int64_t m, int32_t max_depth, float *rgb_dev, int32_t *segments_dev);
+int ray_b200_scene_batch_trace_occluded(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, const float *rays_dev,
+                                        int64_t m, float t_min, float t_max, uint8_t *occluded_dev);
+int ray_b200_scene_batch_trace_multi_hits(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                          const float *rays_dev, int64_t m, float t_min, float t_max, int32_t k,
+                                          struct ray_b200_hit *hits_dev, int32_t *counts_dev);
+int ray_b200_scene_batch_trace_hits_ranged(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                           const struct ray_b200_ray *rays_dev, int64_t m, struct ray_b200_hit *hits_dev);
+int ray_b200_scene_batch_trace_occluded_ranged(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                               const struct ray_b200_ray *rays_dev, int64_t m, uint8_t *occluded_dev);
+int ray_b200_scene_batch_trace_multi_hits_ranged(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                                 const struct ray_b200_ray *rays_dev, int64_t m, int32_t k,
+                                                 struct ray_b200_hit *hits_dev, int32_t *counts_dev);
 
 /* ---- render extensions -------------------------------------------------------------------------- */
 /* render with explicit spp; optional float framebuffer.  out_pix_dev: device int32[h][w] (REQUIRED);

@@ -66,7 +66,8 @@ class Plan(C.Structure):
 
 
 # enum ray_b200_query: what a launch traces (Plan.query)
-QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var", "gbuffer", "scene_batch")
+QUERIES = ("pixels", "closest", "anyhit", "multihit", "accumulate", "views", "adaptive", "adaptive_var", "gbuffer", "scene_batch",
+           "scene_batch_closest", "scene_batch_anyhit", "scene_batch_multihit")
 
 
 class RenderJob(C.Structure):
@@ -181,6 +182,13 @@ def load_library(variant=""):
         "ray_b200_scene_batch_shape": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i64)]),
         "ray_b200_scene_batch_member": (C.c_int, [vp, vp, i32, pp]),
         "ray_b200_render_scene_batch_into": (C.c_int, [vp, vp, i64, i64, i32, vp, vp]),
+        "ray_b200_scene_batch_trace_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
+        "ray_b200_scene_batch_trace_paths": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_scene_batch_trace_occluded": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, vp]),
+        "ray_b200_scene_batch_trace_multi_hits": (C.c_int, [vp, vp, vp, i64, C.c_float, C.c_float, i32, vp, vp]),
+        "ray_b200_scene_batch_trace_hits_ranged": (C.c_int, [vp, vp, vp, i64, vp]),
+        "ray_b200_scene_batch_trace_occluded_ranged": (C.c_int, [vp, vp, vp, i64, vp]),
+        "ray_b200_scene_batch_trace_multi_hits_ranged": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
         "ray_b200_shard_tiles": (i64, [i64, i64, i32, i32]),
         "ray_b200_shard_tiles_padded": (i64, [i64, i64, i32]),
         "ray_b200_render_shard_into": (C.c_int, [vp, vp, i64, i64, i32, vp]),
@@ -515,8 +523,8 @@ class PreparedScene(_Handle):
 
 
 class SceneBatch(_Handle):
-    """B scenes of n spheres each, built together from device memory and rendered in one launch
-    (include/ray_b200.h "scene batches")."""
+    """B scenes of n spheres each, built together from device memory, rendered in one launch and traced by ray queries
+    in one launch (include/ray_b200.h "scene batches"; Context.render_scene_batch, Context.trace_scene_batch_*)."""
     _free_fn = "ray_b200_scene_batch_free"
 
     @property
@@ -1206,6 +1214,126 @@ class Context:
         else:
             self.trace_multi_hits_into(rays.data_ptr(), n, prepared, k, buf.data_ptr(), count.data_ptr(), t_min=_or(t_min, 0.0),
                                        t_max=_or(t_max, 1e9))
+        self.sync()
+        return {"t": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "p": buf[..., 2:5], "normal": buf[..., 5:8],
+                "count": count}
+
+    # -- ray queries of a scene batch (include/ray_b200.h "scene batches"): m rays per scene, all B scenes in one launch
+    def trace_scene_batch_hits_into(self, rays_dev, m, batch, hits_dev, t_min=0.0, t_max=1e9):
+        """trace_hits_into for every scene of a SceneBatch: rays_dev = device float[B][m][6], ray j of scene b at b m + j,
+        hits_dev = device Hit[B][m]; sphere is the index into the ray's own scene's records.  One launch, asynchronous on
+        the context's stream."""
+        self._check(self.lib.ray_b200_scene_batch_trace_hits(self.handle, batch.handle, _ptr(rays_dev), int(m), float(t_min),
+                                                             float(t_max), _ptr(hits_dev)))
+
+    def trace_scene_batch_paths_into(self, rays_dev, m, batch, rgb_dev, segments_dev=None, max_depth=50):
+        """trace_paths_into for every scene of a SceneBatch: rgb_dev = device float[B][m][3], segments_dev = device
+        int32[B][m] or None."""
+        self._check(self.lib.ray_b200_scene_batch_trace_paths(self.handle, batch.handle, _ptr(rays_dev), int(m), int(max_depth),
+                                                              _ptr(rgb_dev), _ptr(segments_dev)))
+
+    def trace_scene_batch_occluded_into(self, rays_dev, m, batch, out_dev, t_min=0.0, t_max=1e9):
+        """trace_occluded_into for every scene of a SceneBatch: out_dev = device uint8[B][m]."""
+        self._check(self.lib.ray_b200_scene_batch_trace_occluded(self.handle, batch.handle, _ptr(rays_dev), int(m), float(t_min),
+                                                                 float(t_max), _ptr(out_dev)))
+
+    def trace_scene_batch_multi_hits_into(self, rays_dev, m, batch, k, hits_dev, counts_dev=None, t_min=0.0, t_max=1e9):
+        """trace_multi_hits_into for every scene of a SceneBatch: hits_dev = device Hit[B][m][k], counts_dev = device
+        int32[B][m] or None."""
+        self._check(self.lib.ray_b200_scene_batch_trace_multi_hits(self.handle, batch.handle, _ptr(rays_dev), int(m), float(t_min),
+                                                                   float(t_max), int(k), _ptr(hits_dev), _ptr(counts_dev)))
+
+    def trace_scene_batch_hits_ranged_into(self, rays_dev, m, batch, hits_dev):
+        """trace_scene_batch_hits_into for rays that carry their own interval: rays_dev = device Ray[B][m]."""
+        self._check(self.lib.ray_b200_scene_batch_trace_hits_ranged(self.handle, batch.handle, _ptr(rays_dev), int(m), _ptr(hits_dev)))
+
+    def trace_scene_batch_occluded_ranged_into(self, rays_dev, m, batch, out_dev):
+        """trace_scene_batch_occluded_into for rays that carry their own interval (device Ray[B][m])."""
+        self._check(self.lib.ray_b200_scene_batch_trace_occluded_ranged(self.handle, batch.handle, _ptr(rays_dev), int(m),
+                                                                        _ptr(out_dev)))
+
+    def trace_scene_batch_multi_hits_ranged_into(self, rays_dev, m, batch, k, hits_dev, counts_dev=None):
+        """trace_scene_batch_multi_hits_into for rays that carry their own interval (device Ray[B][m])."""
+        self._check(self.lib.ray_b200_scene_batch_trace_multi_hits_ranged(self.handle, batch.handle, _ptr(rays_dev), int(m), int(k),
+                                                                          _ptr(hits_dev), _ptr(counts_dev)))
+
+    def _batch_rays_tensor(self, batch, rays, ranged_ok=False, t_min=None, t_max=None):
+        """Checks a tensor of rays of a scene batch: [B, m, 6] or, where ranged_ok, [B, m, 8] (Ray), with B the batch's
+        own, m rays per scene and B m <= 2^30; [B, m, 8] rays take no t_min= / t_max=.  Returns (torch, ranged, m)."""
+        import torch
+        widths = (6, 8) if ranged_ok else (6,)
+        shapes = " or ".join(f"[B, m, {w}]" for w in widths)
+        if isinstance(rays, torch.Tensor) and (rays.dim() != 3 or rays.shape[2] not in widths):
+            raise ValueError(f"rays must be a contiguous float32 tensor of shape {shapes}, got {rays.dtype} {tuple(rays.shape)}")
+        ranged = isinstance(rays, torch.Tensor) and rays.shape[2] == 8
+        if ranged and (t_min is not None or t_max is not None):
+            raise ValueError("rays of shape [B, m, 8] carry their own (t_min, t_max): pass t_min= / t_max= only with [B, m, 6] rays")
+        if not isinstance(rays, torch.Tensor) or rays.device.type != "cuda" or rays.device.index != self.device:
+            raise ValueError(f"rays must be a CUDA tensor on cuda:{self.device}")
+        if rays.dtype != torch.float32 or not rays.is_contiguous():
+            raise ValueError(f"rays must be a contiguous float32 tensor of shape {shapes}, got {rays.dtype} {tuple(rays.shape)}")
+        B, m = int(rays.shape[0]), int(rays.shape[1])
+        if B != batch.shape[0]:
+            raise ValueError(f"rays must have one row per scene of the batch ({batch.shape[0]}), got {B}")
+        if B * m > 1 << 30:
+            raise ValueError(f"a batch query traces at most 2^30 rays, got {B} x {m}")
+        # the rays may still be in flight on torch's stream, which the context's own stream is not ordered after
+        torch.cuda.current_stream(rays.device).synchronize()
+        return torch, ranged, m
+
+    def trace_scene_batch_hits(self, batch, rays, t_min=None, t_max=None):
+        """Closest hits in every scene of a SceneBatch: rays is a [B, m, 6] float32 CUDA tensor, m rays per scene, traced in
+        (t_min, t_max) (default (0, 1e9)), or a [B, m, 8] one whose rays carry their own interval (Ray).  Returns dict(t
+        [B, m], sphere [B, m] int32, p [B, m, 3], normal [B, m, 3]) as trace_hits does, sphere indexing the ray's own
+        scene's records.  Waits for torch's current stream before, and synchronises the context after the query."""
+        torch, ranged, m = self._batch_rays_tensor(batch, rays, True, t_min, t_max)
+        buf = torch.empty((rays.shape[0], m, 8), dtype=torch.float32, device=rays.device)
+        if ranged:
+            self.trace_scene_batch_hits_ranged_into(rays.data_ptr(), m, batch, buf.data_ptr())
+        else:
+            self.trace_scene_batch_hits_into(rays.data_ptr(), m, batch, buf.data_ptr(), t_min=_or(t_min, 0.0), t_max=_or(t_max, 1e9))
+        self.sync()
+        return {"t": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "p": buf[..., 2:5], "normal": buf[..., 5:8]}
+
+    def trace_scene_batch_paths(self, batch, rays, max_depth=50):
+        """Colours of a [B, m, 6] float32 CUDA tensor of rays, each in its own scene of a SceneBatch: (rgb [B, m, 3]
+        float32, segments [B, m] int32).  Waits for torch's current stream before, and synchronises the context after."""
+        torch, _, m = self._batch_rays_tensor(batch, rays)
+        B = rays.shape[0]
+        rgb = torch.empty((B, m, 3), dtype=torch.float32, device=rays.device)
+        seg = torch.empty((B, m), dtype=torch.int32, device=rays.device)
+        self.trace_scene_batch_paths_into(rays.data_ptr(), m, batch, rgb.data_ptr(), seg.data_ptr(), max_depth=max_depth)
+        self.sync()
+        return rgb, seg
+
+    def trace_scene_batch_occluded(self, batch, rays, t_min=None, t_max=None):
+        """Occlusion in every scene of a SceneBatch of [B, m, 6] rays in (t_min, t_max) (default (0, 1e9)), or of [B, m, 8]
+        rays with their own intervals: torch.bool [B, m].  Waits for torch's current stream before, and synchronises the
+        context after the query."""
+        torch, ranged, m = self._batch_rays_tensor(batch, rays, True, t_min, t_max)
+        out = torch.empty((rays.shape[0], m), dtype=torch.bool, device=rays.device)
+        if ranged:
+            self.trace_scene_batch_occluded_ranged_into(rays.data_ptr(), m, batch, out.data_ptr())
+        else:
+            self.trace_scene_batch_occluded_into(rays.data_ptr(), m, batch, out.data_ptr(), t_min=_or(t_min, 0.0),
+                                                 t_max=_or(t_max, 1e9))
+        self.sync()
+        return out
+
+    def trace_scene_batch_multi_hits(self, batch, rays, k, t_min=None, t_max=None):
+        """The k nearest sphere intersections in every scene of a SceneBatch of [B, m, 6] rays in (t_min, t_max) (default
+        (0, 1e9)), or of [B, m, 8] rays with their own intervals.  Returns dict(t [B, m, k], sphere [B, m, k] int32,
+        p [B, m, k, 3], normal [B, m, k, 3], count [B, m] int32).  Waits for torch's current stream before, and
+        synchronises the context after the query."""
+        torch, ranged, m = self._batch_rays_tensor(batch, rays, True, t_min, t_max)
+        B = rays.shape[0]
+        buf = torch.empty((B, m, int(k), 8), dtype=torch.float32, device=rays.device)
+        count = torch.empty((B, m), dtype=torch.int32, device=rays.device)
+        if ranged:
+            self.trace_scene_batch_multi_hits_ranged_into(rays.data_ptr(), m, batch, k, buf.data_ptr(), count.data_ptr())
+        else:
+            self.trace_scene_batch_multi_hits_into(rays.data_ptr(), m, batch, k, buf.data_ptr(), count.data_ptr(),
+                                                   t_min=_or(t_min, 0.0), t_max=_or(t_max, 1e9))
         self.sync()
         return {"t": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "p": buf[..., 2:5], "normal": buf[..., 5:8],
                 "count": count}

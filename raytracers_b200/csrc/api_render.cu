@@ -74,7 +74,10 @@ static_assert((int)Query::kPixels == RAY_B200_QUERY_PIXELS && (int)Query::kClose
                   (int)Query::kAnyHit == RAY_B200_QUERY_ANYHIT && (int)Query::kMultiHit == RAY_B200_QUERY_MULTIHIT &&
                   (int)Query::kAccumulate == RAY_B200_QUERY_ACCUMULATE && (int)Query::kViews == RAY_B200_QUERY_VIEWS &&
                   (int)Query::kAdaptive == RAY_B200_QUERY_ADAPTIVE && (int)Query::kAdaptiveVar == RAY_B200_QUERY_ADAPTIVE_VAR &&
-                  (int)Query::kGBuffer == RAY_B200_QUERY_GBUFFER && (int)Query::kSceneBatch == RAY_B200_QUERY_SCENE_BATCH,
+                  (int)Query::kGBuffer == RAY_B200_QUERY_GBUFFER && (int)Query::kSceneBatch == RAY_B200_QUERY_SCENE_BATCH &&
+                  (int)Query::kBatchClosest == RAY_B200_QUERY_SCENE_BATCH_CLOSEST &&
+                  (int)Query::kBatchAnyHit == RAY_B200_QUERY_SCENE_BATCH_ANYHIT &&
+                  (int)Query::kBatchMultiHit == RAY_B200_QUERY_SCENE_BATCH_MULTIHIT,
               "enum ray_b200_query names the values of Query");
 static_assert(sizeof(struct ray_b200_plan) == 80, "struct ray_b200_plan is 16 int32 and 2 int64");
 

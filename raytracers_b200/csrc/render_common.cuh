@@ -451,6 +451,9 @@ cudaError_t with_query(F &&f, Query q) {
     case Query::kAdaptiveVar: return f(std::integral_constant<Query, Query::kAdaptiveVar>{});
     case Query::kGBuffer: return f(std::integral_constant<Query, Query::kGBuffer>{});
     case Query::kSceneBatch: return f(std::integral_constant<Query, Query::kSceneBatch>{});
+    case Query::kBatchClosest: return f(std::integral_constant<Query, Query::kBatchClosest>{});
+    case Query::kBatchAnyHit: return f(std::integral_constant<Query, Query::kBatchAnyHit>{});
+    case Query::kBatchMultiHit: return f(std::integral_constant<Query, Query::kBatchMultiHit>{});
     default: return cudaErrorInvalidValue;
   }
 }

@@ -273,6 +273,13 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // item's tile over Q.view_tiles, so the slot carries nothing more.  The packet walk takes the new rays of one scene, the
 // first new ray's; the others of the round start in the item queue.  Nodes and spheres are staged as for one tree (a BFS prefix of the concatenated node array, or all of
 // it), the plan is made over the totals and the deepest member, and the claim order is the plain chunk permutation.
+//
+// Query::kBatchClosest, kBatchAnyHit and kBatchMultiHit, the ray queries of a scene batch (include/ray_b200.h
+// ray_b200_scene_batch_trace_*): kClosest, kAnyHit and kMultiHit (kSingle, the kind each computes) over the trees of a
+// scene batch.  Ray c of the claims is scene b = c / Q.rays_per_scene's, so scene_of reads the slot's work item as it does
+// for kSceneBatch, and every segment's set-up (a path query's bounces too) tests scene b's root box and pushes scene b's
+// root node, the same code.  Leaves are scene b's own in their own order, shifted by b n, so the closest-hit tie-break
+// and the multi-hit key order are those of the scene alone; the finish takes b n off perm's global index (sphere_of).
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -282,6 +289,10 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 #endif
 constexpr int kAnyHitLeafMin = RAYB200_ANYHIT_LEAF_MIN;
 static_assert(kAnyHitLeafMin >= 1 && kAnyHitLeafMin <= 32, "a leaf batch takes 1 to 32 items");
+
+// What a launch of kind q computes per ray or pixel, single_scene_kind(q), as the constant the kernel's tests name (a
+// local constant of the kernel in its place changes the generated code of every existing instantiation)
+template <Query q> constexpr Query kSingle = single_scene_kind(q);
 
 template <int K, bool kSpread, bool kPacket, bool kAllNodes, bool kSpheres, Query kQuery = Query::kPixels, bool kRanged = false>
 __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(const __grid_constant__ RenderParams P, const int ncap_arg,
@@ -369,8 +380,19 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   // kFrames: the camera of view (scene) pv (its 12 floats of Q.cams)
   [[maybe_unused]] auto view_cam = [&](const int pv) -> const float * { return kFrames ? Q.cams + 12 * (size_t)pv : nullptr; };
   // kSceneBatch: the scene of the pixel in `slot` (work-item tiles [b view_tiles, (b + 1) view_tiles) are scene b's), so
-  // neither the slot nor wq_warp_bytes carries it
-  [[maybe_unused]] auto scene_of = [&](const int slot) { return (int)((unsigned)(p_item[slot] >> 5) / (unsigned)Q.view_tiles); };
+  // neither the slot nor wq_warp_bytes carries it; a batch ray kind: the scene of the ray in `slot` (rays [b rays_per_scene,
+  // (b + 1) rays_per_scene) are scene b's)
+  [[maybe_unused]] auto scene_of = [&](const int slot) {
+    if constexpr (is_batch_ray(kQuery)) return (int)((unsigned)p_item[slot] / (unsigned)Q.rays_per_scene);
+    else return (int)((unsigned)(p_item[slot] >> 5) / (unsigned)Q.view_tiles);
+  };
+  // ray mode: the caller's index of the sphere of Morton-sorted leaf `leaf`, reached by the ray in `slot`; a batch ray
+  // kind: the index into the ray's own scene's records, perm's global index less the b n spheres of the scenes before it
+  [[maybe_unused]] auto sphere_of = [&](const int slot, const auto leaf) {
+    const int s = __ldg(Q.perm + leaf);
+    if constexpr (is_batch_ray(kQuery)) return s - scene_of(slot) * (Q.scene_inner + 1);
+    else return s;
+  };
   // The first sample c of pixel (row pj, column pi) in this launch: 0 for a whole frame or views, the chunk's first sample
   // (kAccum), the pixel's own count (kAdapt).  Sample s of the launch is sample c + s of the pixel (primary_ray<kQuery>
   // makes its ray), and the pixel's in-order sum continues from Q.accum exactly when c > 0; otherwise its sample 0 starts it.
@@ -539,7 +561,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const uint32_t leaf = h[8 * j + 1];
         const float4 g = sc.sphere((int)leaf);
         t = __uint_as_float(h[8 * j]);
-        sphere = __ldg(Q.perm + leaf);
+        sphere = sphere_of(slot, leaf);
         p = vadd(o, vscale(t, d));                                // point_at_param, ray.fut:14-15
         n = vscale(1.0f / g.w, vsub(p, v3(g.x, g.y, g.z)));       // ray.fut:42-43
       }
@@ -743,7 +765,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             const RayInv q = ray_invariants(r);
             const float lo = kRanged ? ro.w : t_lo, hi = kRanged ? rd.w : t_hi;
             bool root_hit;
-            if constexpr (kBatch) {  // every segment starts at its scene's root: that scene's box (two 16-byte loads)
+            if constexpr (kBatch || is_batch_ray(kQuery)) {  // every segment starts at its scene's root: that scene's box (two 16-byte loads)
               const float4 *bx = reinterpret_cast<const float4 *>(Q.root_boxes) + 2 * (size_t)scene_of(slot);
               const float4 b0 = __ldg(bx), b1 = __ldg(bx + 1);
               root_hit = box_hit(b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, r, q, lo, hi);
@@ -758,19 +780,19 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
                 ray_o[slot] = make_float4(ro.x, ro.y, ro.z, q.a);
                 ray_i[slot] = make_float4(q.ix, q.iy, q.iz, 0.0f);
               }
-              best_t[slot] = kQuery == Query::kMultiHit ? 0u : kItemNoHit;  // multi-hit: no accepted leaf yet
+              best_t[slot] = kSingle<kQuery> == Query::kMultiHit ? 0u : kItemNoHit;  // multi-hit: no accepted leaf yet
               go = true;
               break;
             }
             // the root box already misses: a one-segment query has its answer
-            if constexpr (kQuery == Query::kAnyHit) {  // not occluded
+            if constexpr (kSingle<kQuery> == Query::kAnyHit) {  // not occluded
               Q.occluded[p_item[slot]] = 0;
               p_item[slot] = -1;
               continue;
-            } else if constexpr (kQuery == Query::kMultiHit) {  // k empty records, count 0
+            } else if constexpr (kSingle<kQuery> == Query::kMultiHit) {  // k empty records, count 0
               finish_multi(slot, 0u);
               continue;
-            } else if (kQuery == Query::kClosest && (kRanged || Q.hits)) {  // no hit (paths have no ranged form)
+            } else if (kSingle<kQuery> == Query::kClosest && (kRanged || Q.hits)) {  // no hit (paths have no ranged form)
               finish_hit(slot, -1.0f, -1, v3(0.0f, 0.0f, 0.0f), v3(0.0f, 0.0f, 0.0f));
               continue;
             }
@@ -817,7 +839,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       // up to 32 (ray, sphere) pairs: closest_hit (ray.fut:78-81) for pixels and closest-hit queries; sphere_hit L[i] r
       // t_min t_max with the query's own t_min (no epsilon) for any-hit and multi-hit queries
       constexpr bool kFull = decltype(full_tag)::value;
-      constexpr bool kEpsilon = !kRays || kQuery == Query::kClosest;
+      constexpr bool kEpsilon = !kRays || kSingle<kQuery> == Query::kClosest;
       const int n = kFull ? 32 : n_part;
       bool hit = false;
       uint32_t tb = 0;
@@ -826,7 +848,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const uint32_t it = lstk[ltop - 1 - lane];
         slot = (int)(it >> kSlotShift);
         li = (int)(it & kIndexMask);
-        if (kQuery != Query::kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: items of a marked ray are skipped
+        if (kSingle<kQuery> != Query::kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: items of a marked ray are skipped
           const float4 ro = ray_o[slot], rd = ray_d[slot];
           const float4 g = sc.sphere(li);
           Ray r;
@@ -844,9 +866,9 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         }
       }
       ltop -= n;
-      if constexpr (kQuery == Query::kAnyHit) {
+      if constexpr (kSingle<kQuery> == Query::kAnyHit) {
         if (hit) best_t[slot] = 0u;  // any value but kItemNoHit: occluded
-      } else if constexpr (kQuery == Query::kMultiHit) {
+      } else if constexpr (kSingle<kQuery> == Query::kMultiHit) {
         if (__any_sync(kFullMask, hit)) {
           // every hit into its slot's list: lanes that hit the same slot insert in rounds, the r-th lane of each slot's
           // group in round r
@@ -874,7 +896,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         const uint32_t it = nstk[ring(kDeque && bottom ? nhead + lane : ntop + ~lane)];
         tag = it & ~kIndexMask;
         const int slot = (int)(it >> kSlotShift), cur = (int)(it & kIndexMask);
-        if (kQuery != Query::kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: a marked ray pushes nothing, its subtree is pruned
+        if (kSingle<kQuery> != Query::kAnyHit || best_t[slot] == kItemNoHit) {  // any-hit: a marked ray pushes nothing, its subtree is pruned
           const float4 ro = ray_o[slot], ri = ray_i[slot];
           float4 q0, q1, q2, q3;
           sc.node(cur, q0, q1, q2, q3);
@@ -925,7 +947,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     auto drain = [&]() {
       __syncwarp();
       const int nroom = ncap - 96;
-      constexpr int kLeafMin = kQuery == Query::kAnyHit ? kAnyHitLeafMin : 32;  // leaf items that make a leaf batch due
+      constexpr int kLeafMin = kSingle<kQuery> == Query::kAnyHit ? kAnyHitLeafMin : 32;  // leaf items that make a leaf batch due
       for (;;) {
         // the common case first and alone in its loop: full node batches while nothing else is due (the general
         // dispatch below costs ~12 instructions per batch).  One copy of the batch body for both pop directions.
@@ -1040,7 +1062,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         }
       } else {
         const bool go = (gm >> lane) & 1u;
-        if constexpr (kBatch) {  // (slot, its scene's root node)
+        if constexpr (kBatch || is_batch_ray(kQuery)) {  // (slot, its scene's root node)
           if (go) nstk[ntop + __popc(gm & lt_mask)] = ((uint32_t)(lane + 32 * k) << kSlotShift) | (uint32_t)(scene_of(lane + 32 * k) * Q.scene_inner);
         } else {
           if (go) nstk[ntop + __popc(gm & lt_mask)] = (uint32_t)(lane + 32 * k) << kSlotShift;  // (slot, root node 0)
@@ -1055,11 +1077,11 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     for (int k = 0; k < K; k++) {
       if (!((trav >> k) & 1u)) continue;
       const int slot = lane + 32 * k;
-      if constexpr (kQuery == Query::kAnyHit) {
+      if constexpr (kSingle<kQuery> == Query::kAnyHit) {
         Q.occluded[p_item[slot]] = best_t[slot] != kItemNoHit ? 1 : 0;
         p_item[slot] = -1;
         continue;
-      } else if constexpr (kQuery == Query::kMultiHit) {
+      } else if constexpr (kSingle<kQuery> == Query::kMultiHit) {
         finish_multi(slot, best_t[slot]);
         continue;
       }
@@ -1072,7 +1094,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       int depth = __float_as_int(pl.w);
       const int j = bt == kItemNoHit ? -1 : (int)best_l[slot];
       const float tb = __uint_as_float(bt);
-      if (kQuery == Query::kClosest && (kRanged || Q.hits)) {
+      if (kSingle<kQuery> == Query::kClosest && (kRanged || Q.hits)) {
         // objs_hit, second half (ray.fut:83-85) with the query's (kRanged: the ray's) t_min; a failed re-intersection is
         // no hit
         float t = -1.0f;
@@ -1086,7 +1108,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             n = vscale(1.0f / g.w, vsub(p, v3(g.x, g.y, g.z)));       // ray.fut:42-43
           }
         }
-        if (t >= 0.0f) finish_hit(slot, t, __ldg(Q.perm + j), p, n);
+        if (t >= 0.0f) finish_hit(slot, t, sphere_of(slot, j), p, n);
         else finish_hit(slot, -1.0f, -1, p, n);
         continue;
       }
@@ -1199,8 +1221,11 @@ cudaError_t launch_warpqueue(const RenderParams &p, Query kind, bool ranged, con
   const cudaError_t e = with_query([&](auto query) {
     if constexpr (is_ray_query(query))
       return with_flags([&](auto k2, auto a, auto s, auto rg) {
-        return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, query, rg>>(
-            lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
+        // (a scene batch's kinds are not built for every sphere staged without every node, as for kSceneBatch)
+        if constexpr (is_batch_ray(query) && s && !a) return cudaErrorInvalidValue;
+        else
+          return launch_opted_in<render_warpqueue_kernel<k2 ? 2 : 1, false, false, a, s, query, rg>>(
+              lc.max_dynamic_smem, (unsigned)ctas, wthreads, wsmem, stream, p, ncap, 0, 1, nlow, q);
       }, k == 2, all_nodes, sph, ranged);
     else
       return with_flags([&](auto k2, auto sp, auto pk, auto a, auto s) {

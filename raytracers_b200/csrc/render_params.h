@@ -68,11 +68,26 @@ struct RenderParams {
 // that also keeps each pixel's running sum of squared deviations (m2).  kGBuffer, a pixel kind: the first hit of every
 // camera ray of a frame (its sphere, t, normal and albedo), reduced per pixel into the guide buffers (gb_id, gb_depth,
 // gb_normal, gb_albedo, gb_coverage).  kSceneBatch, a pixel kind: one frame of each scene of a scene batch (cams, n_views,
-// view_tiles as kViews, root_boxes, scene_inner).  New kinds go at the end: kernel names carry the values, and
-// tools/sass_compare.py reads older builds' names by them.
-enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar, kGBuffer, kSceneBatch };
+// view_tiles as kViews, root_boxes, scene_inner).  kBatchClosest, kBatchAnyHit and kBatchMultiHit, ray kinds: the
+// single-scene ray kind over the trees of a scene batch, rays_per_scene rays per scene (root_boxes, scene_inner as
+// kSceneBatch).  New kinds go at the end: kernel names carry the values, and tools/sass_compare.py reads older builds'
+// names by them.
+enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar, kGBuffer, kSceneBatch,
+                   kBatchClosest, kBatchAnyHit, kBatchMultiHit };
+// The ray kinds of a scene batch
+__host__ __device__ constexpr bool is_batch_ray(Query q) {
+  return q == Query::kBatchClosest || q == Query::kBatchAnyHit || q == Query::kBatchMultiHit;
+}
+// What a launch of kind q computes per ray or pixel: a scene batch's ray kind is its single-scene kind, every other kind
+// itself.  The kernel tests this, not q, for what the single-scene ray kinds do, so that each is named once.
+__host__ __device__ constexpr Query single_scene_kind(Query q) {
+  return q == Query::kBatchClosest ? Query::kClosest
+       : q == Query::kBatchAnyHit ? Query::kAnyHit
+       : q == Query::kBatchMultiHit ? Query::kMultiHit : q;
+}
 __host__ __device__ constexpr bool is_ray_query(Query q) {
-  return q == Query::kClosest || q == Query::kAnyHit || q == Query::kMultiHit;
+  const Query s = single_scene_kind(q);
+  return s == Query::kClosest || s == Query::kAnyHit || s == Query::kMultiHit;
 }
 // Pixel kinds whose pixels each continue from their own sample count (Q.sample_counts): a selection pass in front of the
 // render kernel lists the pixels, which the kernel claims from Q.sel; each sample's offsets are computed on the device, so
@@ -145,6 +160,10 @@ struct RayQuery {
   // of P.root_box
   const float *root_boxes;
   int32_t scene_inner;
+  // the ray kinds of a scene batch (Query::kBatchClosest / kBatchAnyHit / kBatchMultiHit; include/ray_b200.h
+  // ray_b200_scene_batch_trace_*): rays [b * rays_per_scene, (b + 1) * rays_per_scene) are scene b's, traced from its root
+  // node b * scene_inner and root box as kSceneBatch; n = B * rays_per_scene, and the outputs follow the rays' order
+  int32_t rays_per_scene;
 };
 
 // Wavefront ray queues (SoA in HBM, 48 B per live ray): two ping-pong queues indexed by bounce parity.

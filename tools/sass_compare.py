@@ -45,7 +45,8 @@ def functions(path):
 
 WARPQUEUE = re.compile(r"render_warpqueue_kernel<([^<>]*)>\(")
 PROBE = re.compile(r"tile_probe(_views)?_kernel(?:<\(.*Query\)(\d+)>)?\(")
-KINDS = ("pixels", "closest", "any-hit", "multi-hit", "accumulate", "views", "adaptive", "adaptive-var", "gbuffer", "scene-batch")   # the values of the Query enum, in order
+KINDS = ("pixels", "closest", "any-hit", "multi-hit", "accumulate", "views", "adaptive", "adaptive-var", "gbuffer", "scene-batch",
+         "batch-closest", "batch-any-hit", "batch-multi-hit")   # the values of the Query enum, in order
 
 
 def canonical(name):
