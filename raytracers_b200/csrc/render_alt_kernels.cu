@@ -136,6 +136,7 @@ __global__ void __launch_bounds__(256, 2) wavefront_bounce_kernel(const __grid_c
         r.o = v3(a.x, a.y, a.z);
         r.d = v3(d.x, d.y, d.z);
         light = v3(l.x, l.y, l.z);
+        depth = __float_as_int(l.w);  // the path state word (render_common.cuh)
         pid = __float_as_int(a.w);
       }
     }
@@ -172,7 +173,7 @@ __global__ void __launch_bounds__(256, 2) wavefront_bounce_kernel(const __grid_c
         const int o = obase + __popc(alive & lt_mask);
         B.ray_o[qo][o] = make_float4(r.o.x, r.o.y, r.o.z, __int_as_float(pid));
         B.ray_d[qo][o] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
-        B.light[qo][o] = make_float4(light.x, light.y, light.z, 0.0f);
+        B.light[qo][o] = make_float4(light.x, light.y, light.z, __int_as_float(depth));
       }
     }
   }
@@ -205,7 +206,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_streamqueue_kernel(co
   float4 *ray_o = reinterpret_cast<float4 *>(wbase);   // {o.xyz, a = dot d d}
   float4 *ray_i = ray_o + R;                           // {1/d.xyz, 0}
   float4 *ray_d = ray_i + R;                           // {d.xyz, 0}
-  float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth)}
+  float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth word, render_common.cuh)}
   float4 *p_sum = p_light + R;                         // {sum.rgb, bits(sample)} / spread: w = bits(ring << 16 | sample)
   unsigned long long *best = reinterpret_cast<unsigned long long *>(p_sum + R);  // (bits(t) << 32 | leaf) min-folded
   int *p_item = reinterpret_cast<int *>(best + R);     // pixel item of the slot, -1 = idle

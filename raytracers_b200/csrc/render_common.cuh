@@ -123,10 +123,33 @@ __device__ __forceinline__ void find_closest(const Scene &sc, const float *root_
 }
 
 // ------------------------------------------------------------------ one ray_colour iteration (ray.fut:130-148)
+// The path state word `depth`: bits 3 and up count the scatters so far (a depth limit is at most 65535), bits 0-2 are
+// the sign of ray_colour's `colour` per channel (x, y, z).  That colour starts at +0 and is only ever multiplied by the
+// light (ray.fut:133-137), so it is always +0, -0 or NaN: -0 after an odd number of lights with the sign bit set, NaN
+// once a light multiplied in was not finite.  A non-finite light stays non-finite (inf * 0 = NaN, inf * x = inf,
+// NaN * x = NaN), so `light * (the signed zero)` at an end is exactly the reference's `light * colour`, NaN included,
+// without carrying the colour itself.  With the count in the high bits, "one more scatter is below the limit" stays one
+// comparison: word + 8 < max_depth * 8 exactly when scatters + 1 < max_depth.
+constexpr int kDepthShift = 3;
+
+__device__ __forceinline__ int path_depth(const int depth) { return depth >> kDepthShift; }
+
+// ray_colour's `colour` before the end: +0 or -0 per channel, from the sign bits of the state word
+__device__ __forceinline__ V3 path_zero(const int depth) {
+  const unsigned w = (unsigned)depth;
+  return v3(__uint_as_float(w << 31), __uint_as_float((w << 30) & 0x80000000u), __uint_as_float((w << 29) & 0x80000000u));
+}
+
+// the state word's sign bits after `colour = light * colour` (ray.fut:135): each XORed with the light's sign bit
+__device__ __forceinline__ int path_signs(const int depth, const V3 light) {
+  return depth ^ (int)((__float_as_uint(light.x) >> 31) | ((__float_as_uint(light.y) >> 30) & 2u) |
+                       ((__float_as_uint(light.z) >> 29) & 4u));
+}
+
 // The part of a ray_colour iteration after the closest-hit search: given the fold result (j, tb),
 // re-intersect, scatter or shade the sky.  `a` = dot r.d r.d.  Returns true if the path continues
-// (r/light/depth updated), false if it ended with `colour` set.  `max_depth`: ray_colour's depth limit (ray.fut:154
-// passes 50; a path query passes its own).
+// (r/light/depth updated), false if it ended with `colour` set.  `depth` is the path state word above (0 at a path's
+// start).  `max_depth`: ray_colour's depth limit (ray.fut:154 passes 50; a path query passes its own).
 template <class Scene>
 __device__ __forceinline__ bool shade_segment(const Scene &sc, const RenderParams &P, Ray &r, const float a, const int j,
                                               const float tb, V3 &light, int &depth, V3 &colour,
@@ -146,13 +169,17 @@ __device__ __forceinline__ bool shade_segment(const Scene &sc, const RenderParam
         const float4 col = __ldg(P.colour + j);
         r.o = p;
         r.d = refl;
+        const V3 old = light;
         light = vmul(light, v3(col.x, col.y, col.z));               // ray.fut:135
-        depth = depth + 1;
-        if (depth < max_depth) return true;
-        colour = v3(0.0f, 0.0f, 0.0f);                              // loop exit with colour = light*0 (ray.fut:136)
+        if (depth + (1 << kDepthShift) < (max_depth << kDepthShift)) {
+          depth = path_signs(depth, old) + (1 << kDepthShift);
+          return true;
+        }
+        colour = vmul(old, path_zero(depth));                       // loop exit with colour = light_old * colour (ray.fut:135-136)
+        depth = depth + (1 << kDepthShift);
         return false;
       }
-      colour = v3(0.0f, 0.0f, 0.0f);                                // ray.fut:137-140
+      colour = vmul(light, path_zero(depth));                       // colour = light * colour (ray.fut:137-140)
       return false;
     }
   }

@@ -337,7 +337,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
   float4 *ray_o = reinterpret_cast<float4 *>(wbase);   // {o.xyz, a = dot d d}     kRanged: {o.xyz, t_min}
   float4 *ray_i = ray_o + R;                           // {1/d.xyz, 0}             kRanged: {1/d.xyz, t_max}
   float4 *ray_d = ray_i + R;                           // {d.xyz, 0}               kRanged: {d.xyz, a} (t_max until the root test)
-  float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth)}   owner lane only
+  float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth word, render_common.cuh)}   owner lane only
   float4 *p_sum = p_light + R;                         // pixel-bound samples: {sum.rgb, bits(sample)}
   int *p_ms = reinterpret_cast<int *>(p_light + R);    // spread samples: ring entry << 16 | sample (4 bytes per slot instead of 16)
   uint32_t *best_t = kSpread ? reinterpret_cast<uint32_t *>(p_ms + R)   // bits(t) of the closest accepted hit (kItemNoHit = none) ...
@@ -804,7 +804,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
             V3 light = v3(pl.x, pl.y, pl.z), colour;
             int depth = __float_as_int(pl.w);
             shade_segment(sc, P, r, q.a, -1, 0.0f, light, depth, colour);
-            finish_path(slot, colour, depth + 1);
+            finish_path(slot, colour, path_depth(depth) + 1);
           }
         }
         const unsigned m = __ballot_sync(kFullMask, go);
@@ -1139,7 +1139,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
         ray_d[slot] = make_float4(r.d.x, r.d.y, r.d.z, 0.0f);
         p_light[slot] = make_float4(light.x, light.y, light.z, __int_as_float(depth));
       } else {
-        finish_path(slot, colour, depth + 1);
+        finish_path(slot, colour, path_depth(depth) + 1);
       }
     }
     __syncwarp();

@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_lanewalk_kernel(const
   float4 *ray_o = reinterpret_cast<float4 *>(wbase);   // {o.xyz, a = dot d d}
   float4 *ray_i = ray_o + R;                           // {1/d.xyz, 0}
   float4 *ray_d = ray_i + R;                           // {d.xyz, 0}
-  float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth)}
+  float4 *p_light = ray_d + R;                         // {light.rgb, bits(depth word, render_common.cuh)}
   uint32_t *best_t = reinterpret_cast<uint32_t *>(p_light + R);  // bits(t) of the closest accepted hit, kLwNoHit = none
   uint32_t *best_l = best_t + R;                       // its leaf (lowest index among equal t)
   int *p_item = reinterpret_cast<int *>(best_l + R);   // pixel item of the slot

@@ -325,9 +325,11 @@ def test_ray_query_oracle_paths(name, max_depth):
 def judge_paths(ref, rays, max_depth, rgb, seg):
     col, want_seg, _, err, judged = ref.judged_paths(rays[:, :3].astype(np.float64), rays[:, 3:].astype(np.float64),
                                                      max_depth)
+    rgb = np.asarray(rgb, np.float64)
     with np.errstate(invalid="ignore"):
-        far = np.abs(np.asarray(rgb, np.float64) - col) > (4 * err + 1e-6)[:, None] * np.maximum(1.0, np.abs(col))
-    bad = judged & ((np.asarray(seg) != want_seg) | far.any(1))
+        far = np.abs(rgb - col) > (4 * err + 1e-6)[:, None] * np.maximum(1.0, np.abs(col))
+    # NaN on one side only is a disagreement (a comparison with NaN is False, so `far` alone never sees it)
+    bad = judged & ((np.asarray(seg) != want_seg) | (far | (np.isnan(rgb) != np.isnan(col))).any(1))
     return float(judged.mean()), int(bad.sum()), _msg(f"paths max_depth={max_depth}", judged, bad)
 
 

@@ -15,7 +15,6 @@ import pytest
 
 import ray_query_oracle as Q
 from ray_query_cases import INTERVALS, T24, _dev, _np, _torch, bits_differ, hits_differ, max_hit_t, random_rays
-from test_input_ranges import ALL_SCENES
 from test_scene_batch import STAGING, mixed_batch, random_batch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -243,9 +242,9 @@ def test_header_declares_and_binding_binds_the_batch_queries(R):
 # ------------------------------------------------------------------------------------------ GPU: exactness
 
 
-def check_batch(ctx, batch, s, rays6, rays8, k, t, max_depth, refs, oracles=None, members=None, what="", path_oracle=None):
+def check_batch(ctx, batch, s, rays6, rays8, k, t, max_depth, refs, oracles=None, members=None, what=""):
     """Every entry point on the batch against run_single on each scene's prepared scenes in refs, and against the oracle
-    where oracles is given (path colours only on the members in path_oracle, None = all)"""
+    where oracles is given"""
     B, m = rays6.shape[:2]
     n = s.shape[1]
     d6, d8 = _dev(rays6), _dev(rays8)
@@ -267,7 +266,7 @@ def check_batch(ctx, batch, s, rays6, rays8, k, t, max_depth, refs, oracles=None
             for ref_name, prs in refs.items():
                 want = run_single(ctx, prs[b], kind, rays[b], **kw)
                 assert_same(mine, want, f"{tag} scene {b} vs {ref_name}")
-            if oracles is not None and (kind != "paths" or path_oracle is None or b in path_oracle):
+            if oracles is not None:
                 want = run_oracle(oracles[b], kind, (rays8 if rg else rays6)[b], **kw)
                 assert_same(mine, want, f"{tag} scene {b} vs the oracle")
 
@@ -277,9 +276,6 @@ def check_batch(ctx, batch, s, rays6, rays8, k, t, max_depth, refs, oracles=None
 def test_mixed_batch_every_kind_equals_members_and_independent_scenes(R, n):
     s, cams = mixed_batch(n)
     B = len(s)
-    # the path colours of the input-range members are checked against the single-scene query only: its own tests compare
-    # them with the oracle on camera rays, not on arbitrary rays cut at a small depth
-    path_oracle = {0, 1} | set(range(2 + len(ALL_SCENES), B))
     with R.Context() as ctx:
         batch = ctx.prepare_scene_batch(H, W, _dev(s), cams)
         refs = {"member": [batch.member(b) for b in range(B)],
@@ -288,8 +284,7 @@ def test_mixed_batch_every_kind_equals_members_and_independent_scenes(R, n):
             r6 = batch_rays(s, m, seed=100 * n + i)
             r8 = ranged(r6, seed=i)
             oracles = [Q.prepare_custom(s[b], cams[b], H, W) for b in range(B)] if n <= 64 and 0 < m <= 31 else None
-            check_batch(ctx, batch, s, r6, r8, k, INTERVALS[i % len(INTERVALS)], depth, refs, oracles, what=f"n={n}",
-                        path_oracle=path_oracle)
+            check_batch(ctx, batch, s, r6, r8, k, INTERVALS[i % len(INTERVALS)], depth, refs, oracles, what=f"n={n}")
 
 
 @pytest.mark.gpu
