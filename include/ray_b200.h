@@ -45,7 +45,7 @@ extern "C" {
 
 /* Render kernels (tuning param "kernel" / env RAY_KERNEL). */
 enum ray_b200_kernel {
-  RAY_B200_KERNEL_AUTO = 0,       /* the fastest measured variant (see resolve_kernel in api.cu) */
+  RAY_B200_KERNEL_AUTO = 0,       /* the fastest measured variant (see resolve_kernel in api_render.cu) */
   RAY_B200_KERNEL_MEGA = 1,       /* one thread per pixel, whole ray_colour loop (parity anchor) */
   RAY_B200_KERNEL_PERSISTENT = 2, /* persistent CTAs, TMA-staged BVH, per-lane dynamic path refill */
   RAY_B200_KERNEL_WAVEFRONT = 3,  /* per-bounce persistent kernel + global ray queues + warp-vote compaction */

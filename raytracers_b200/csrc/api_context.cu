@@ -28,15 +28,11 @@ int env_int(const char *name, int dflt) {
   return atoi(v);
 }
 
+// A kernel's name (kKernels) or its number
 int parse_kernel(const char *v, int dflt) {
   if (!v || !*v) return dflt;
-  if (!strcmp(v, "auto")) return RAY_B200_KERNEL_AUTO;
-  if (!strcmp(v, "mega")) return RAY_B200_KERNEL_MEGA;
-  if (!strcmp(v, "persistent")) return RAY_B200_KERNEL_PERSISTENT;
-  if (!strcmp(v, "wavefront")) return RAY_B200_KERNEL_WAVEFRONT;
-  if (!strcmp(v, "warpqueue")) return RAY_B200_KERNEL_WARPQUEUE;
-  if (!strcmp(v, "streamqueue")) return RAY_B200_KERNEL_STREAMQUEUE;
-  if (!strcmp(v, "lanewalk")) return RAY_B200_KERNEL_LANEWALK;
+  for (int k = 0; k < kNumKernels; k++)
+    if (!strcmp(v, kKernels[k].name)) return k;
   return atoi(v);
 }
 
@@ -351,7 +347,7 @@ int ray_b200_context_set_spp(struct futhark_context *ctx, int32_t spp) {
 }
 int ray_b200_context_set_kernel(struct futhark_context *ctx, int32_t k) {
   if (bad_ctx(ctx)) return 1;
-  if (k < RAY_B200_KERNEL_AUTO || k > RAY_B200_KERNEL_LANEWALK) { set_error(ctx, "unknown kernel %d", k); return 1; }
+  if (k < 0 || k >= kNumKernels) { set_error(ctx, "unknown kernel %d", k); return 1; }
   ctx->cfg.kernel = k;
   return 0;
 }

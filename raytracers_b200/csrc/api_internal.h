@@ -187,7 +187,6 @@ inline int64_t tiles_of_rank(int64_t h, int64_t w, int32_t rank, int32_t world) 
 }
 
 // api_render.cu
-int resolve_kernel(const futhark_context *ctx);
 // One pixel launch as its caller describes it: every entry point that renders fills one Frame, and fill_params and
 // do_render read everything about the launch from it.
 struct Frame {
@@ -202,6 +201,23 @@ struct Frame {
   RayQuery q{};                // the fields of q that kind reads (render_params.h RayQuery); fill_params sets view_tiles,
                                // the adaptive entry point sel / n_sel once allocated
 };
+// One render kernel as the host path sees it: its tuning name, what a launch of it needs from do_render, and its plan.
+// kKernels[k] describes kernel k of enum ray_b200_kernel (entry RAY_B200_KERNEL_AUTO only names "auto"), and
+// kKernels[kNumKernels] any other id.
+struct KernelInfo {
+  const char *name;        // tuning / RAY_KERNEL name
+  bool claims_cursor;      // claims work from the lane's cursor, which is zeroed before the launch
+  bool sample_buf;         // spreads a pixel's samples over its slots when it gets a finished-sample buffer ...
+  bool needs_sample_buf;   // ... and cannot trace spp > 1 without one
+  bool claim_order;        // claims tiles heavy-first or in the learned order when those are on
+  bool self_signal;        // bumps the frame's done flag itself (last warp out); else a 1-thread kernel follows it
+  bool warp_trace;         // records when each warp runs out of work (ray_b200_context_trace_warps)
+  bool wavefront_queues;   // uses the context's one set of wavefront ray queues, so its frames run on lane 0 only
+  // fills the LaunchConfig fields the kernel's launcher reads and P's staging split, for frame f
+  int (*plan)(futhark_context *ctx, const Frame &f, RenderParams &P, LaunchConfig &lc);
+};
+constexpr int kNumKernels = RAY_B200_KERNEL_LANEWALK + 1;
+extern const KernelInfo kKernels[];
 // The parameter block of frame f and its launch plan (kernel, warps, K, node-queue cap, packet threshold, lane-walk
 // slots, ...), which the caller hands to do_render with f; sets f.q.view_tiles of a kViews frame.
 int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &lc);

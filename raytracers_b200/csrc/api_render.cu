@@ -38,8 +38,6 @@ int ensure_offsets(futhark_context *ctx, int32_t spp) {
   return 0;
 }
 
-int resolve_kernel(const futhark_context *ctx);
-
 // Zeroes the kernel parameter block and fills its scene half from a prepared scene.
 void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P) {
   memset(&P, 0, sizeof P);
@@ -49,24 +47,12 @@ void fill_scene_params(const futhark_opaque_prepared_scene *p, RenderParams &P) 
   memcpy(P.root_box, p->root_box, sizeof P.root_box);
 }
 
-// The launch plan every kernel's own planning starts from: the context's tuning, one warp, K = 1, no packet walk.
+// The launch plan every kernel's plan starts from: the kernel and the device's limits, every other field 0
 static LaunchConfig launch_config(const futhark_context *ctx, int kernel) {
-  LaunchConfig lc;
+  LaunchConfig lc{};
   lc.kernel = kernel;
-  lc.blocks_per_sm = ctx->cfg.blocks_per_sm;
   lc.sm_count = ctx->sm_count;
-  lc.refill_min = ctx->cfg.refill_min;
-  lc.wq_warps = 1;
-  lc.wq_k = 1;
-  lc.wq_refill = ctx->cfg.wq_refill < 1 ? 1 : (ctx->cfg.wq_refill > 32 ? 32 : ctx->cfg.wq_refill);
-  lc.wq_low = ctx->cfg.wq_low;
-  lc.wq_packet = 0;
-  lc.wq_ncap = ctx->cfg.wq_ncap;
-  lc.lw_slots = 0;
-  lc.lw_idle_min = ctx->cfg.lw_idle_min;
-  lc.lw_passes = ctx->cfg.lw_passes;
   lc.max_dynamic_smem = ctx->max_smem_optin;
-  lc.stage_budget = 0;
   return lc;
 }
 
@@ -113,8 +99,90 @@ static size_t spread_bytes(const futhark_context *ctx, int warps, int32_t spp) {
   return need <= kSpreadBudget ? need : 0;
 }
 
-// Fills the kernel parameter block for frame f, and the frame's launch plan.  Every kind but kPixels runs on the warp-queue
-// kernel whatever the context's kernel is, planned as a frame of f.spp samples (spread or pixel-bound by that count).
+// K0, K1, K2: a staging area of the smem_budget tuning; K1 / K2 run blocks_per_sm CTAs per SM, K1 refills at refill_min
+static int plan_staging(futhark_context *ctx, const Frame &f, RenderParams &P, LaunchConfig &lc) {
+  lc.blocks_per_sm = ctx->cfg.blocks_per_sm;
+  lc.refill_min = ctx->cfg.refill_min;
+  lc.stage_budget = std::min<int64_t>(ctx->cfg.smem_budget, ctx->max_smem_optin - 1024) - 128;
+  split_staging(f.scene, lc.stage_budget, P.smem_nodes, P.smem_spheres);
+  return 0;
+}
+
+// K3 frames: samples will be spread if the finished-sample buffer fits the budget (do_render allocates it; a failed
+// allocation there falls back to pixel-bound samples, whose bigger slots are checked again at launch)
+static int plan_warpqueue_frame(futhark_context *ctx, const Frame &f, RenderParams &P, LaunchConfig &lc) {
+  const bool will_spread = !is_pixel_bound(f.kind) && spread_bytes(ctx, kWqMaxWarps, f.spp) != 0;
+  // the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame (a warp's tile
+  // lies in one view: the density is that of a view, however many there are)
+  const bool coherent = f.spp > 1 || f.h * f.w >= ((int64_t)1 << 22);
+  return plan_warpqueue(ctx, f.scene, will_spread, coherent, false, "render", P, lc);
+}
+
+static int plan_streamqueue(futhark_context *ctx, const Frame &f, RenderParams &P, LaunchConfig &lc) {
+  const futhark_opaque_prepared_scene *p = f.scene;
+  const int k = 1;
+  const int64_t per_warp = (int64_t)sq_warp_bytes(k, wq_node_capacity(k, p->max_depth));
+  int64_t wq_w = ctx->cfg.wq_warps < 1 ? 24 : (ctx->cfg.wq_warps > kWqMaxWarps ? kWqMaxWarps : ctx->cfg.wq_warps);
+  while (wq_w > 1 && wq_w * per_warp + 8192 > (int64_t)ctx->max_smem_optin) wq_w--;
+  const int64_t budget = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512;
+  if (budget < 256) { set_error(ctx, "render: stream-queue kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
+  lc.wq_warps = (int32_t)wq_w;
+  lc.wq_refill = std::min(std::max(ctx->cfg.wq_refill, 1), 32);
+  lc.stage_budget = budget;
+  split_staging(p, budget, P.smem_nodes, P.smem_spheres);
+  return 0;
+}
+
+// K5: one CTA per SM, lw_warps warps (32 unless told otherwise) x lw_slots path slots each (48 unless told otherwise,
+// 32..64); slots are given up first, then warps, until the queues leave room for staging the top of the tree
+static int plan_lanewalk(futhark_context *ctx, const Frame &f, RenderParams &P, LaunchConfig &lc) {
+  const futhark_opaque_prepared_scene *p = f.scene;
+  const int scap = lw_stack_capacity(p->max_depth);
+  int64_t w = ctx->cfg.lw_warps < 1 ? 32 : std::min<int64_t>(ctx->cfg.lw_warps, kWqMaxWarps);
+  int64_t r = ctx->cfg.lw_slots < 1 ? 48 : (ctx->cfg.lw_slots >= 64 ? 64 : (ctx->cfg.lw_slots >= 48 ? 48 : 32));  // 32 / 48 / 64 are built
+  const int64_t full_stage = 128 + n_inner_of(p) * 64 + n_leaves_of(p) * 16;
+  const int64_t want_stage = std::min<int64_t>(full_stage, 16 * 1024);
+  while (w * (int64_t)lw_warp_bytes((int)r, scap) + want_stage + 1024 > (int64_t)ctx->max_smem_optin) {
+    if (r > 32) r -= 16;
+    else if (w > 1) w--;
+    else { set_error(ctx, "render: lane-walk kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
+  }
+  const int64_t budget = (int64_t)ctx->max_smem_optin - w * (int64_t)lw_warp_bytes((int)r, scap) - 512;
+  lc.wq_warps = (int32_t)w;
+  lc.lw_slots = (int32_t)r;
+  lc.lw_idle_min = ctx->cfg.lw_idle_min;
+  lc.lw_passes = ctx->cfg.lw_passes;
+  lc.stage_budget = budget;
+  split_staging(p, cap_staging(ctx, p, budget), P.smem_nodes, P.smem_spheres);
+  return 0;
+}
+
+const KernelInfo kKernels[] = {  // name, claims_cursor, sample_buf, needs_sample_buf, claim_order, self_signal, warp_trace, wavefront_queues, plan
+    {"auto",        false, false, false, false, false, false, false, nullptr},               // RAY_B200_KERNEL_AUTO
+    {"mega",        false, false, false, false, false, false, false, plan_staging},          // K0 RAY_B200_KERNEL_MEGA
+    {"persistent",  true,  false, false, false, false, false, false, plan_staging},          // K1 RAY_B200_KERNEL_PERSISTENT
+    {"wavefront",   false, false, false, false, false, false, true,  plan_staging},          // K2 RAY_B200_KERNEL_WAVEFRONT
+    {"warpqueue",   true,  true,  false, true,  true,  true,  false, plan_warpqueue_frame},  // K3 RAY_B200_KERNEL_WARPQUEUE
+    {"streamqueue", true,  true,  false, false, false, false, false, plan_streamqueue},      // K4 RAY_B200_KERNEL_STREAMQUEUE
+    {"lanewalk",    true,  true,  true,  false, true,  true,  false, plan_lanewalk},         // K5 RAY_B200_KERNEL_LANEWALK
+    {"",            false, false, false, false, false, false, false, plan_staging},          // any other id (kernel_info)
+};
+static_assert(sizeof kKernels / sizeof kKernels[0] == kNumKernels + 1, "one entry per enum ray_b200_kernel, and one more");
+
+// The tuning "kernel" and RAY_KERNEL take any number: an id outside the enum is planned with the staging plan, and
+// launch_render refuses it
+static const KernelInfo &kernel_info(int k) { return kKernels[k >= 0 && k < kNumKernels ? k : kNumKernels]; }
+
+// The kernel of a pixel launch of kind `kind` and spp samples.  Every kind but kPixels runs on the warp-queue kernel, the
+// fastest measured variant on every BASELINE config, and so do AUTO and a kernel that needs the finished-sample buffer
+// (K5: 0.54 MB per sample on an H100) at spp > 1 when there can be none (spreading switched off, or over the budget).
+static int resolve_kernel(const futhark_context *ctx, Query kind, int32_t spp) {
+  const int k = kind != Query::kPixels || ctx->cfg.kernel == RAY_B200_KERNEL_AUTO ? RAY_B200_KERNEL_WARPQUEUE : ctx->cfg.kernel;
+  return kernel_info(k).needs_sample_buf && spp > 1 && !spread_bytes(ctx, kWqMaxWarps, spp) ? RAY_B200_KERNEL_WARPQUEUE : k;
+}
+
+// Fills the kernel parameter block for frame f, and the frame's launch plan: that of resolve_kernel's kernel, made by its
+// kKernels entry.  Every kind is planned as a frame of f.spp samples (spread or pixel-bound by that count).
 // Query::kAccumulate reads the offset table of the whole frame from the chunk's first sample on and scales by 1/s_end.
 // Query::kViews and kSceneBatch: the work items are the tiles of all q.n_views frames, so the plan (K, staging, the sample
 // buffer) is that of one frame of n_views x tiles(h, w) tiles (a scene batch's over all its trees, see n_inner_of).  The adaptive kinds are planned over all tiles, an upper bound on
@@ -177,55 +245,8 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   P.counters = ctx->counters;
   P.warp_trace = nullptr;
   P.tile_order = nullptr;
-  // shared-memory staging plan: BFS prefix of the node array, then the sphere records if they all fit.
-  // The warp-queue kernel runs one CTA per SM and gives the staging area whatever its queues leave.
-  int64_t budget = std::min<int64_t>(ctx->cfg.smem_budget, ctx->max_smem_optin - 1024) - 128;
-  int kern = f.kind != Query::kPixels ? RAY_B200_KERNEL_WARPQUEUE : resolve_kernel(ctx);
-  // K5 traces one sample per slot and needs the finished-sample buffer (0.54 MB per sample on an H100); without it (spreading
-  // switched off, or a sample count whose buffer exceeds the budget) the frame runs on the warp-queue kernel
-  if (kern == RAY_B200_KERNEL_LANEWALK && spp > 1 && !spread_bytes(ctx, kWqMaxWarps, spp)) kern = RAY_B200_KERNEL_WARPQUEUE;
-  lc = launch_config(ctx, kern);
-  if (kern == RAY_B200_KERNEL_STREAMQUEUE) {
-    const int k = 1;
-    const int64_t per_warp = (int64_t)sq_warp_bytes(k, wq_node_capacity(k, p->max_depth));
-    int64_t wq_w = ctx->cfg.wq_warps < 1 ? 24 : (ctx->cfg.wq_warps > kWqMaxWarps ? kWqMaxWarps : ctx->cfg.wq_warps);
-    while (wq_w > 1 && wq_w * per_warp + 8192 > (int64_t)ctx->max_smem_optin) wq_w--;
-    budget = (int64_t)ctx->max_smem_optin - wq_w * per_warp - 512;
-    if (budget < 256) { set_error(ctx, "render: stream-queue kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
-    lc.wq_warps = (int32_t)wq_w;
-  }
-  if (kern == RAY_B200_KERNEL_WARPQUEUE) {
-    // samples will be spread if the finished-sample buffer fits the budget (do_render allocates it; a failed allocation
-    // there falls back to pixel-bound samples, whose bigger slots are checked again at launch)
-    const bool will_spread = !is_pixel_bound(f.kind) && spread_bytes(ctx, kWqMaxWarps, spp) != 0;
-    // the rays a warp holds are coherent: samples of one pixel (spp > 1) or primary rays of a dense frame (a warp's tile
-    // lies in one view: the density is that of a view, however many there are)
-    const bool coherent = spp > 1 || h * w >= ((int64_t)1 << 22);
-    return plan_warpqueue(ctx, p, will_spread, coherent, false, "render", P, lc);
-  }
-  if (kern == RAY_B200_KERNEL_LANEWALK) {
-    // one CTA per SM: lw_warps warps (32 unless told otherwise) x lw_slots path slots each (48 unless told otherwise,
-    // 32..64); slots are given up first, then warps, until the queues leave room for staging the top of the tree
-    const int scap = lw_stack_capacity(p->max_depth);
-    int64_t w = ctx->cfg.lw_warps < 1 ? 32 : std::min<int64_t>(ctx->cfg.lw_warps, kWqMaxWarps);
-    int64_t r = ctx->cfg.lw_slots < 1 ? 48 : (ctx->cfg.lw_slots >= 64 ? 64 : (ctx->cfg.lw_slots >= 48 ? 48 : 32));  // 32 / 48 / 64 are built
-    const int64_t full_stage = 128 + n_inner_of(p) * 64 + n_leaves_of(p) * 16;
-    const int64_t want_stage = std::min<int64_t>(full_stage, 16 * 1024);
-    while (w * (int64_t)lw_warp_bytes((int)r, scap) + want_stage + 1024 > (int64_t)ctx->max_smem_optin) {
-      if (r > 32) r -= 16;
-      else if (w > 1) w--;
-      else { set_error(ctx, "render: lane-walk kernel does not fit shared memory (tree depth %d)", p->max_depth); return 1; }
-    }
-    budget = (int64_t)ctx->max_smem_optin - w * (int64_t)lw_warp_bytes((int)r, scap) - 512;
-    lc.wq_warps = (int32_t)w;
-    lc.lw_slots = (int32_t)r;
-    lc.stage_budget = budget;
-    budget = cap_staging(ctx, p, budget);
-  } else {
-    lc.stage_budget = budget;
-  }
-  split_staging(p, budget, P.smem_nodes, P.smem_spheres);
-  return 0;
+  lc = launch_config(ctx, resolve_kernel(ctx, f.kind, spp));
+  return kernel_info(lc.kernel).plan(ctx, f, P, lc);
 }
 
 // Shared memory not used by the warp-queue / lane-walk kernels stays L1: a tree far larger than the caches gains more from
@@ -306,6 +327,8 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
     lc.wq_warps = (int32_t)wq_w;
     lc.wq_k = k;
     lc.wq_ncap = ncap_cfg;
+    lc.wq_refill = std::min(std::max(ctx->cfg.wq_refill, 1), 32);
+    lc.wq_low = ctx->cfg.wq_low;
     lc.stage_budget = budget;
     split_staging(p, cap_staging(ctx, p, budget), P.smem_nodes, P.smem_spheres);
     // belt and braces: the K = 2 plan is only worth anything when the scene is staged whole (a scene that just misses
@@ -313,12 +336,6 @@ int plan_warpqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p,
     if (!auto_k2 || (P.smem_nodes == (int32_t)n_inner_of(p) && P.smem_spheres == (int32_t)n_leaves_of(p))) break;
   }
   return 0;
-}
-
-int resolve_kernel(const futhark_context *ctx) {
-  int k = ctx->cfg.kernel;
-  if (k == RAY_B200_KERNEL_AUTO) k = RAY_B200_KERNEL_WARPQUEUE;  // fastest measured variant on every BASELINE config
-  return k;
 }
 
 void free_wavefront(futhark_context *ctx) {
@@ -402,10 +419,10 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
     if (P.local_tiles < padded)
       CUDA_TRY(ctx, cudaMemsetAsync(f.out_pix + P.local_tiles * kTilePixels, 0, (size_t)(padded - P.local_tiles) * kTilePixels * 4, L.stream));
   }
-  if (lc.kernel == RAY_B200_KERNEL_WAVEFRONT && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
+  const KernelInfo &K = kernel_info(lc.kernel);
+  if (K.wavefront_queues && ensure_wavefront(ctx, P.local_tiles * kTilePixels)) return 1;
   P.sample_buf = nullptr;
-  const bool slot_kernel = lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_STREAMQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK;
-  const size_t need = slot_kernel && !is_pixel_bound(f.kind) ? spread_bytes(ctx, lc.wq_warps, P.spp) : 0;
+  const size_t need = K.sample_buf && !is_pixel_bound(f.kind) ? spread_bytes(ctx, lc.wq_warps, P.spp) : 0;
   if (need) {
     // samples of a pixel are spread over a warp's slots; finished colours wait here for the in-order sum
     // (0.54 MB per sample on an H100's 132 SMs with 32 warps).  Above a memory budget, or when the allocation fails, the frame falls
@@ -419,14 +436,14 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
       else { L.sample_buf = nullptr; cudaGetLastError(); }
     }
     P.sample_buf = have ? L.sample_buf : nullptr;
-    if (!have && lc.kernel == RAY_B200_KERNEL_LANEWALK) { set_error(ctx, "render: out of device memory for the finished-sample buffer (%zu bytes)", need); return 1; }
+    if (!have && K.needs_sample_buf) { set_error(ctx, "render: out of device memory for the finished-sample buffer (%zu bytes)", need); return 1; }
   }
-  // heavy-first claim order (warp-queue kernel): worth its probe pass when a frame is long enough to have a tail to lose
+  // heavy-first claim order (K.claim_order): worth its probe pass when a frame is long enough to have a tail to lose
   // — more than one sample per pixel — and pointless when every tile is claimed in the first wave anyway.
   // A progressive or G-buffer launch uses neither this nor the learned order below (DESIGN.md, progressive rendering).  A views launch
   // probes its tiles with their views' cameras; it does not use the learned order either, which is recorded for one camera.
   const int hf = ctx->cfg.heavy_first;
-  const bool heavy_first = !is_plain_order(f.kind) && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
+  const bool heavy_first = !is_plain_order(f.kind) && K.claim_order && P.local_tiles > 1 && P.local_tiles < (1ll << 26) &&
                            (hf > 0 || (hf < 0 && P.spp > 1));
   if (heavy_first) {
     P.probes_per_tile = hf >= 4 ? 4 : (hf >= 2 ? 2 : 1);
@@ -441,7 +458,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
   bool record_order = false;
   // (Frames of more than 2^24 tile-samples do not end on their longest paths any more, and un-mixing cheap and expensive
   // tiles costs them more than the shorter tail saves.)
-  if (!heavy_first && f.kind == Query::kPixels && ctx->cfg.learn_order && lc.kernel == RAY_B200_KERNEL_WARPQUEUE && P.local_tiles > 64 &&
+  if (!heavy_first && f.kind == Query::kPixels && ctx->cfg.learn_order && K.claim_order && P.local_tiles > 64 &&
       P.local_tiles < (1ll << 26) && (ctx->cfg.learn_order > 1 || P.local_tiles * (int64_t)P.spp <= ((int64_t)1 << 24))) {
     auto &oc = f.scene->order_cache;
     const bool same = oc.state == 1 && oc.h == P.H && oc.w == P.W && oc.spp == P.spp && oc.rank == P.rank && oc.world == P.world && oc.tiles == P.local_tiles;
@@ -471,7 +488,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
     }
   }
   P.work_cursor = L.work_cursor;
-  if (ctx->warp_trace && (lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK) && lane_id == 0) {
+  if (ctx->warp_trace && K.warp_trace && lane_id == 0) {
     const size_t n = 1 + (size_t)lc.sm_count * kWqMaxWarps;
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->warp_trace, 0, n * sizeof(unsigned long long), L.stream));
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->warp_trace, 0xff, sizeof(unsigned long long), L.stream));
@@ -479,11 +496,8 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
     ctx->trace_warps = lc.wq_warps;
   }
   if (timed) CUDA_TRY(ctx, cudaEventRecord(ctx->ev_start, L.stream));
-  if (lc.kernel == RAY_B200_KERNEL_PERSISTENT || lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_STREAMQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK)
-    CUDA_TRY(ctx, cudaMemsetAsync(L.work_cursor, 0, 2 * sizeof(int32_t), L.stream));  // [0] work cursor, [1] departed warps
-  // the default kernels publish the frame themselves (last warp out); for the others a 1-thread kernel follows the launch
-  const bool self_signal = lc.kernel == RAY_B200_KERNEL_WARPQUEUE || lc.kernel == RAY_B200_KERNEL_LANEWALK;
-  P.frame_flag = (ff && self_signal) ? ff->done_flag : nullptr;
+  if (K.claims_cursor) CUDA_TRY(ctx, cudaMemsetAsync(L.work_cursor, 0, 2 * sizeof(int32_t), L.stream));  // [0] work cursor, [1] departed warps
+  P.frame_flag = (ff && K.self_signal) ? ff->done_flag : nullptr;
   if (ff && ff->wait_flag) launch_flag_wait(ff->wait_flag, ff->wait_value, (long long)ctx->flag_timeout_ms * 1000000ll, ctx->flag_timeouts, L.stream);
   if (heavy_first) launch_tile_order(P, L.tile_order_plan, L.stream, &ctx->launches, f.kind, f.q);
   if (is_adaptive(f.kind)) {
@@ -506,7 +520,7 @@ int do_render(futhark_context *ctx, const Frame &f, RenderParams &P, const Launc
     CUDA_TRY(ctx, cudaEventRecord(f.scene->order_cache.ready, L.stream));
     f.scene->order_cache.state = 1;
   }
-  if (ff && ff->done_flag && !self_signal) launch_flag_bump(ff->done_flag, L.stream);
+  if (ff && ff->done_flag && !K.self_signal) launch_flag_bump(ff->done_flag, L.stream);
   CUDA_TRY(ctx, cudaGetLastError());
   if (record_scene_use(ctx, f.scene, lane_id)) return 1;
   if (timed) {
@@ -795,9 +809,8 @@ int ray_b200_render_batch(struct futhark_context *ctx, const struct ray_b200_ren
     if (!jobs[i].out_dev) { set_error(ctx, "render_batch: job %d has no output buffer", i); return 1; }
     if (jobs[i].shard_layout && jobs[i].out_rgb_dev) { set_error(ctx, "render_batch: job %d: no float output in the shard layout", i); return 1; }
   }
-  const int kernel = resolve_kernel(ctx);
   // the wavefront kernel's ray queues and the warp trace exist once per context: those batches run in order on lane 0
-  const bool lanes_ok = kernel != RAY_B200_KERNEL_WAVEFRONT && !ctx->warp_trace;
+  const bool lanes_ok = !kernel_info(resolve_kernel(ctx, Query::kPixels, 1)).wavefront_queues && !ctx->warp_trace;
   const bool pipe = ctx->pipeline && lanes_ok;   // frames alternate lanes across calls, no join at the end
   const bool two_lanes = lanes_ok && (n > 1 || pipe);
   futhark_context::Lane &L1 = ctx->lanes[1];

@@ -1,8 +1,8 @@
 // The alternative kernels (slower than K3, see DESIGN.md §5), kept with their parity tests: K1
 // persistent + lane refill, K2 per-bounce wavefront with global ray queues (the north-star design as specified), K4
 // stream queue (K3 without rounds).  Compiled into libray_b200_all.so (-DRAYB200_ALL_KERNELS: the library the test-suite
-// loads for these kernels); the product library libray_b200.so carries only K0 / K3 / K5 and reports an error for the
-// others, so it stays small and futhark_context_new stays fast.
+// loads for these kernels, with K5 from render_lanewalk.cu); the product library libray_b200.so carries only K0 / K3 and
+// reports an error for the others, so it stays small and futhark_context_new stays fast.
 #include <cub/cub.cuh>
 #include "render_common.cuh"
 
@@ -564,7 +564,8 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
   const bool all_nodes = p.smem_nodes == p.n_inner, sph = p.smem_spheres == p.n_leaves && p.smem_spheres > 0;
   long long want = (long long)lc.sm_count * lc.blocks_per_sm;
   cudaError_t e = cudaSuccess;
-  if (lc.kernel == 3) {  // RAY_B200_KERNEL_WAVEFRONT: per sample pass, one launch per bounce up to the tail bounce
+  switch (lc.kernel) {
+  case RAY_B200_KERNEL_WAVEFRONT: {  // per sample pass, one launch per bounce up to the tail bounce
     const long long max_useful = (items + 31) / 32;
     if (want > max_useful) want = max_useful;
     const int tail = wf->tail_from < 0 ? 0 : (wf->tail_from > kMaxDepth - 1 ? kMaxDepth - 1 : wf->tail_from);
@@ -589,7 +590,7 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
     }
     return e;
   }
-  if (lc.kernel == 5) {  // RAY_B200_KERNEL_STREAMQUEUE: one CTA per SM, rays refilled continuously (no rounds); 32 rays per warp
+  case RAY_B200_KERNEL_STREAMQUEUE: {  // one CTA per SM, rays refilled continuously (no rounds); 32 rays per warp
     constexpr int k = 1;
     const int wthreads = 32 * lc.wq_warps;
     const int ncap = wq_node_capacity(k, p.max_depth);
@@ -606,8 +607,9 @@ cudaError_t launch_alt_kernel(const RenderParams &p, const LaunchConfig &lc, con
     if (e == cudaSuccess) (*launches)++;
     return e;
   }
-  if (lc.kernel != 2) return cudaErrorInvalidValue;
-  // RAY_B200_KERNEL_PERSISTENT
+  case RAY_B200_KERNEL_PERSISTENT: break;
+  default: return cudaErrorInvalidValue;
+  }
   const long long max_useful = (items + threads - 1) / threads;
   if (want > max_useful) want = max_useful;
   const int refill = lc.refill_min < 1 ? 1 : (lc.refill_min > 32 ? 32 : lc.refill_min);

@@ -1193,16 +1193,18 @@ cudaError_t launch_render(const RenderParams &p, const LaunchConfig &lc, const W
                           int64_t *launches, Query kind, const RayQuery &q) {
   const long long items = p.local_tiles * kTilePixels;
   if (items <= 0) return cudaSuccess;
-  if (lc.kernel == 1) {  // RAY_B200_KERNEL_MEGA
+  switch (lc.kernel) {
+  case RAY_B200_KERNEL_MEGA: {
     const int threads = 128;
     const unsigned blocks = (unsigned)((items + threads - 1) / threads);
     render_mega_kernel<false><<<blocks, threads, 0, stream>>>(p);
     (*launches)++;
     return cudaSuccess;
   }
-  if (lc.kernel == 6) return launch_lanewalk(p, lc, stream, launches);             // RAY_B200_KERNEL_LANEWALK
-  if (lc.kernel != 4) return launch_alt_kernel(p, lc, wf, stream, launches);       // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
-  return launch_warpqueue(p, kind, false, q, lc, stream, launches);                // RAY_B200_KERNEL_WARPQUEUE
+  case RAY_B200_KERNEL_WARPQUEUE: return launch_warpqueue(p, kind, false, q, lc, stream, launches);
+  case RAY_B200_KERNEL_LANEWALK: return launch_lanewalk(p, lc, stream, launches);
+  default: return launch_alt_kernel(p, lc, wf, stream, launches);  // K1 / K2 / K4 (RAYB200_ALL_KERNELS builds)
+  }
 }
 
 // K3: one CTA per SM, wq_warps warps, 32*wq_k rays in flight per warp.  A launch of pixel kind `kind`, or a ray query of

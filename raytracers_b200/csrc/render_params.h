@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include "../../include/ray_b200.h"   // enum ray_b200_kernel (LaunchConfig::kernel)
 
 namespace rayb200 {
 
@@ -18,7 +19,7 @@ struct RenderParams {
   const float4 *geom;
   const float4 *colour;
   int32_t n_inner, n_leaves;
-  int32_t smem_nodes;    // first smem_nodes BFS nodes are staged in shared memory (persistent/wavefront kernels)
+  int32_t smem_nodes;    // first smem_nodes BFS nodes are staged in shared memory (every kernel but K0)
   int32_t smem_spheres;  // first smem_spheres sphere records staged (0 or n_leaves)
   int32_t max_depth;     // depth of the deepest leaf (root = 0): bounds the traversal stacks
   float root_box[6];
