@@ -316,7 +316,8 @@ int ray_b200_render_host(struct futhark_context *ctx, int32_t *out_pix_host, flo
  *   Exactness: any chain of calls [0, a), [a, b), ..., [y, S) on one buffer leaves the same accum as one call [0, S), bit
  *   for bit, and its pixels and float framebuffer equal ray_b200_render_into(spp = S) (NaN-aware: a NaN is some NaN).
  *   The sum read at s_begin > 0 is whatever the caller left in the buffer; the result is the f32 arithmetic above on it.
- *   Sample s is sample s of the spp semantics above, whatever the chunking.
+ *   Sample s is sample s of the spp semantics above, whatever the chunking.  A call's sample offsets take host and device
+ *   memory in proportion to s_end - s_begin, wherever the range starts.
  *   The call is asynchronous on the context's stream; stream order, the pipeline lanes, freeing the prepared scene while
  *   the call is in flight, ray_b200_context_last_render_ms and ray_b200_context_launch_count (one launch per call) behave
  *   as for ray_b200_render_into.  With a shard set (world > 1) only this rank's pixels of accum and of the outputs are

@@ -59,9 +59,8 @@ struct futhark_context {
   unsigned long long *warp_trace = nullptr; // device [1 + SMs * kWqMaxWarps] when tracing is on (ray_b200_context_trace_warps)
   int trace_warps = 0;                      // warps per CTA of the last traced launch
   float *offsets = nullptr;                 // device sample-offset table of the frame being set up (an entry of offset_tables)
-  int32_t offsets_spp = 0;
-  struct OffsetTable { int32_t spp; float *dev; };
-  std::vector<OffsetTable> offset_tables;   // per-spp cache (ensure_offsets)
+  struct OffsetTable { int32_t s_begin, s_end; float *dev; };
+  std::vector<OffsetTable> offset_tables;   // cache per sample range [s_begin, s_end) (ensure_offsets)
   int64_t launches = 0;
   ray_b200_plan last_plan{};                // plan of the last render kernel launch (ray_b200_context_last_plan)
   WavefrontBuffers wf;                     // ray queues of the wavefront kernel (grown on demand)

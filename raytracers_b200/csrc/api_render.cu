@@ -7,16 +7,18 @@ using namespace rayb200_api;
 
 namespace rayb200_api {
 
-// Device copy of the sample-offset table for `spp` (SURVEY.md 8d: offset (0,0) at sample 0).  Tables are cached per spp
-// (render_batch mixes sample counts) and never freed while a frame may still read them.  A new table is copied from a
-// page-locked staging buffer on the context's stream and the stream is synchronised before it is handed out, so the
-// data has landed whichever lane's stream the reading kernel is launched on (a pageable cudaMemcpy on the legacy stream
-// only guarantees staging, and nothing would order a non-blocking stream after its DMA).
-int ensure_offsets(futhark_context *ctx, int32_t spp) {
+// Device copy of the sample-offset table of samples [s_begin, s_end) (SURVEY.md 8d: offset (0,0) at sample 0): a frame's
+// is [0, spp), a progressive chunk's its own samples only, so a chunk far into a frame costs memory and host time in
+// proportion to its length.  Tables are cached per range (render_batch mixes sample counts) and never freed while a
+// frame may still read them.  A new table is copied from a page-locked staging buffer on the context's stream and the
+// stream is synchronised before it is handed out, so the data has landed whichever lane's stream the reading kernel is
+// launched on (a pageable cudaMemcpy on the legacy stream only guarantees staging, and nothing would order a non-blocking
+// stream after its DMA).
+static int ensure_offsets(futhark_context *ctx, int32_t s_begin, int32_t s_end) {
   for (auto &e : ctx->offset_tables)
-    if (e.spp == spp) { ctx->offsets = e.dev; ctx->offsets_spp = spp; return 0; }
+    if (e.s_begin == s_begin && e.s_end == s_end) { ctx->offsets = e.dev; return 0; }
   std::vector<float> table;
-  sample_offsets(spp, table);
+  sample_offsets(s_begin, s_end, table);
   const size_t bytes = table.size() * sizeof(float);
   float *stage = nullptr, *dev = nullptr;
   CUDA_TRY(ctx, cudaMallocHost(&stage, bytes));
@@ -32,9 +34,8 @@ int ensure_offsets(futhark_context *ctx, int32_t spp) {
     cudaFree(ctx->offset_tables.front().dev);
     ctx->offset_tables.erase(ctx->offset_tables.begin());
   }
-  ctx->offset_tables.push_back({spp, dev});
+  ctx->offset_tables.push_back({s_begin, s_end, dev});
   ctx->offsets = dev;
-  ctx->offsets_spp = spp;
   return 0;
 }
 
@@ -183,7 +184,7 @@ static int resolve_kernel(const futhark_context *ctx, Query kind, int32_t spp) {
 
 // Fills the kernel parameter block for frame f, and the frame's launch plan: that of resolve_kernel's kernel, made by its
 // kKernels entry.  Every kind is planned as a frame of f.spp samples (spread or pixel-bound by that count).
-// Query::kAccumulate reads the offset table of the whole frame from the chunk's first sample on and scales by 1/s_end.
+// Query::kAccumulate reads the offset table of the chunk's samples [s_begin, s_end) and scales by 1/s_end.
 // Query::kViews and kSceneBatch: the work items are the tiles of all q.n_views frames, so the plan (K, staging, the sample
 // buffer) is that of one frame of n_views x tiles(h, w) tiles (a scene batch's over all its trees, see n_inner_of).  The adaptive kinds are planned over all tiles, an upper bound on
 // their work (the selection is on the device).  A pixel-bound kind (Query::kGBuffer) is planned as a frame whose samples
@@ -208,13 +209,13 @@ int fill_params(futhark_context *ctx, Frame &f, RenderParams &P, LaunchConfig &l
   if (p->max_depth > kStackSize - 1) { set_error(ctx, "render: BVH depth %d exceeds the traversal stack", p->max_depth); return 1; }
   const int32_t s_begin = f.kind == Query::kAccumulate ? f.q.s_begin : 0, s_end = s_begin + spp;  // (the entry point keeps s_end in int32)
   const bool adaptive = is_adaptive(f.kind);
-  if (!adaptive && ensure_offsets(ctx, s_end)) return 1;
+  if (!adaptive && ensure_offsets(ctx, s_begin, s_end)) return 1;
   fill_scene_params(p, P);
   // The camera depends on the aspect ratio w/h given to prepare_scene (ray.fut:243-244); render's own
   // h, w only set the pixel grid (ray.fut:246-247) — exactly as in the reference.
   memcpy(P.cam, &p->cam, sizeof P.cam);
   P.W = (int32_t)w; P.H = (int32_t)h; P.spp = spp; P.inv_spp = 1.0f / (float)s_end;
-  P.offsets = adaptive ? nullptr : ctx->offsets + 2 * (size_t)s_begin;
+  P.offsets = adaptive ? nullptr : ctx->offsets;
   P.out_pix = f.out_pix; P.out_rgb = f.out_rgb; P.tile_major = f.tile_major ? 1 : 0;
   P.rank = f.rank; P.world = f.world;
   P.tiles_x = (int32_t)((w + kTileW - 1) / kTileW); P.tiles_y = (int32_t)((h + kTileH - 1) / kTileH);

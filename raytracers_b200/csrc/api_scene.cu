@@ -591,7 +591,7 @@ int ray_b200_host_lbvh(const float *spheres, int64_t n, uint32_t *morton, int32_
 }
 void ray_b200_host_sample_offsets(int32_t spp, float *table) {
   std::vector<float> t;
-  sample_offsets(spp, t);
+  sample_offsets(0, spp, t);
   memcpy(table, t.data(), t.size() * sizeof(float));
 }
 

@@ -215,7 +215,7 @@ __device__ __forceinline__ Ray camera_ray(const float *c, const float u, const f
 
 // get_ray for sample s of pixel (row j, column i): ray.fut:150-154 with pixel j i -> trace_ray (height-j) i
 // (ray.fut:167-168) and the spp extension of ray_b200.h (offset (0,0) at s = 0).  Query::kAccumulate (a chunk of a
-// progressive frame): s is relative to the chunk, P.offsets starts at its first sample and is read even when P.spp == 1;
+// progressive frame): s is relative to the chunk, P.offsets holds the chunk's samples only and is read even when P.spp == 1;
 // at s = 0 of the frame the offset is (0, 0) and f32(i) + 0 is exact, so that is the one-sample ray too.  The adaptive
 // kinds: s is relative to the pixel's own first sample c, and the offsets of its sample c + s are computed here exactly as
 // sample_offsets computes them on the host (the same f32 products, floorf and differences; -fmad=false keeps them apart):
@@ -234,8 +234,10 @@ __device__ __forceinline__ Ray primary_ray(const RenderParams &P, int i, int j, 
     u = (float)i / (float)P.W;
     v = (float)(P.H - j) / (float)P.H;
   } else {
-    u = ((float)i + P.offsets[2 * s]) / (float)P.W;
-    v = ((float)(P.H - j) + P.offsets[2 * s + 1]) / (float)P.H;
+    // 64-bit index: a launch may trace up to INT32_MAX samples of a pixel, and 2 * s passes INT32_MAX from s = 2^30 on
+    const float *o = P.offsets + 2 * (size_t)s;
+    u = ((float)i + o[0]) / (float)P.W;
+    v = ((float)(P.H - j) + o[1]) / (float)P.H;
   }
   if constexpr (kViews) {  // three 16-byte read-only loads (the table is 16-byte aligned, 48 bytes per view)
     const float4 *q = reinterpret_cast<const float4 *>(view_cam);

@@ -27,7 +27,7 @@ struct RenderParams {
   // frame
   int32_t W, H, spp;
   float inv_spp;
-  const float *offsets;  // 2*spp sample offsets (device)
+  const float *offsets;  // 2*spp sample offsets of the launch's samples (device; a chunk's start at its s_begin)
   int32_t *out_pix;      // row-major [H][W] (tile_major == 0) or compact [local_tiles][32] (tile_major == 1)
   float *out_rgb;        // optional [H][W][3]
   int32_t tile_major;

@@ -159,12 +159,12 @@ CameraRec make_camera(const HostScene &s, int64_t h, int64_t w) {
   return cam;
 }
 
-void sample_offsets(int32_t spp, std::vector<float> &table) {
-  table.resize((size_t)spp * 2);
-  for (int32_t s = 0; s < spp; s++) {
+void sample_offsets(int32_t s_begin, int32_t s_end, std::vector<float> &table) {
+  table.resize((size_t)(s_end - s_begin) * 2);
+  for (int32_t s = s_begin; s < s_end; s++) {
     const float a = (float)s * 0.7548776662f, b = (float)s * 0.5698402909f;
-    table[2 * (size_t)s] = a - floorf(a);
-    table[2 * (size_t)s + 1] = b - floorf(b);
+    table[2 * (size_t)(s - s_begin)] = a - floorf(a);
+    table[2 * (size_t)(s - s_begin) + 1] = b - floorf(b);
   }
 }
 

@@ -65,7 +65,8 @@ CameraRec make_camera(const HostScene &s, int64_t h, int64_t w);  // ray.fut:93-
 bool build_lbvh(const HostScene &s, Lbvh &out, std::string *err);
 void pack_bvh(const HostScene &s, const Lbvh &t, PackedBvh &out);
 
-// sample offsets of the spp extension (ray_b200.h header comment); table[2*s] = ox_s, [2*s+1] = oy_s
-void sample_offsets(int32_t spp, std::vector<float> &table);
+// sample offsets of the spp extension (ray_b200.h header comment) for samples [s_begin, s_end);
+// table[2*(s - s_begin)] = ox_s, [2*(s - s_begin)+1] = oy_s
+void sample_offsets(int32_t s_begin, int32_t s_end, std::vector<float> &table);
 
 }  // namespace rayb200

@@ -14,6 +14,9 @@ from oracle import pyoracle as O
 from ray_query_cases import PLANS, _dev, _np, _torch, bits_differ, quantise
 
 SENTINEL = 0x7FA5A5A5      # a NaN payload no kernel writes
+SPREAD_BUDGET = 1 << 30    # bytes of the finished-sample buffer samples may be spread with (kSpreadBudget)
+WQ_RING = 8                # pixels a warp keeps open when its samples are spread (kWqRing)
+BOUNDARY_PLAN = dict(wq_k=1, wq_warps=32)    # the plan whose launches have the warps the spread decision assumes
 SPLITS = {
     "whole": [(0, 64)],
     "ones": [(s, s + 1) for s in range(64)],
@@ -35,6 +38,12 @@ def sequential_sum(colours, s_begin, s_end, start=None):
         for s in range(s_begin + 1, s_end):
             acc = acc + colours[..., s, :]
     return acc.astype(np.float32)
+
+
+def last_spread_spp(sms, warps=32):
+    """The largest sample count whose samples are spread on a GPU of `sms` SMs at `warps` warps per CTA: its
+    finished-sample buffer, SMs x warps x WQ_RING pixels x spp x 16 bytes, fits SPREAD_BUDGET (1985 on 132 SMs)."""
+    return SPREAD_BUDGET // (sms * warps * WQ_RING * 16)
 
 
 def frame_of(acc, s_end):
@@ -128,14 +137,17 @@ def _one_shot(ctx, pr, h, w, spp):
     return _np(pix), _np(rgb)
 
 
-def _chain(ctx, pr, h, w, split, accum=None):
-    """Runs the calls of `split` on one accum buffer (NaN-filled unless given: sample 0 must not read it)."""
+def _chain(ctx, pr, h, w, split, accum=None, plans=None):
+    """Runs the calls of `split` on one accum buffer (NaN-filled unless given: sample 0 must not read it); appends each
+    call's plan to `plans` where given."""
     torch = _torch()
     if accum is None:
         accum = torch.full((h, w, 3), float("nan"), dtype=torch.float32, device="cuda")
     pix = rgb = None
     for a, b in split:
         pix, rgb = ctx.render_accumulate(pr, accum, a, b, want_rgb=True)
+        if plans is not None:
+            plans.append(ctx.last_plan())
     return _np(accum), _np(pix), _np(rgb)
 
 
@@ -201,15 +213,20 @@ def test_caller_supplied_sums(R, chunk):
 @pytest.mark.gpu
 @pytest.mark.parametrize("spread", [1, 0])
 def test_both_sample_paths(R, spread):
-    """Chunks of 1 (pixel-bound), 2 to 1985 (spread) and 1986 (over the 1 GiB finished-sample budget: pixel-bound)."""
+    """Chunks of 1 (pixel-bound), 2 up to the last count whose finished-sample buffer fits the 1 GiB budget at 32 warps
+    on this GPU's SMs (spread) and one more (pixel-bound); with wq_spread 0 all pixel-bound."""
     h, w = 4, 8
-    split = [(0, 1), (1, 3), (3, 10), (10, 11), (11, 75), (75, 2060), (2060, 4046)]
+    last = last_spread_spp(_torch().cuda.get_device_properties(0).multi_processor_count)
+    split = [(0, 1), (1, 3), (3, 10), (10, 11), (11, 75), (75, 75 + last), (75 + last, 76 + 2 * last)]
     S = split[-1][1]
-    ctx, pr = _ctx(R, "irreg", h, w, wq_spread=spread)
+    ctx, pr = _ctx(R, "irreg", h, w, wq_spread=spread, **BOUNDARY_PLAN)
     want_pix, want_rgb = _one_shot(ctx, pr, h, w, S)
     colours = _gpu_colours(R, ctx, pr, h, w, S)
-    acc, pix, rgb = _chain(ctx, pr, h, w, split)
+    plans = []
+    acc, pix, rgb = _chain(ctx, pr, h, w, split, plans=plans)
     _check_against(acc, pix, rgb, sequential_sum(colours, 0, S), want_pix, want_rgb, f"wq_spread={spread}")
+    assert [p["spread"] for p in plans] == [int(spread and 1 < b - a <= last) for a, b in split]
+    assert plans[-2]["spread"] == spread and plans[-1]["spread"] == 0 and {p["warps"] for p in plans} == {32}
     ctx.close()
 
 

@@ -12,7 +12,8 @@ import pytest
 import ray_query_oracle as Q      # tests/ray_query_oracle.py: the CPU oracle of the ray queries
 from oracle import pyoracle as O
 from ray_query_cases import PLANS, _dev, _np, _torch, bits_differ
-from test_render_accumulate import SCENES, _chain, _ctx, _gpu_colours, _one_shot, frame_of, sequential_sum
+from test_render_accumulate import (BOUNDARY_PLAN, SCENES, _chain, _ctx, _gpu_colours, _one_shot, frame_of, last_spread_spp,
+                                    sequential_sum)
 from test_staging_plans import FORCED_PLANS, H, W, check_frame, expect, forced, variant  # noqa: F401 (forced: fixture)
 
 SENTINEL = 0x7FA5A5A5      # a NaN payload no kernel writes
@@ -101,10 +102,10 @@ def test_python_argument_checks(R):
 # ------------------------------------------------------------------------------------------ GPU helpers
 
 
-def _adaptive_chain(ctx, pr, h, w, masks, n_adds, accum=None, counts=None, check_untouched=False):
+def _adaptive_chain(ctx, pr, h, w, masks, n_adds, accum=None, counts=None, check_untouched=False, plans=None):
     """Runs render_adaptive once per (mask, n_add) on one set of buffers (NaN-filled sums, zero counts, sentinel outputs
     unless given).  With check_untouched, asserts after every call that the pixels it did not select kept all four
-    values.  Returns numpy (accum, counts, pixels, rgb)."""
+    values.  Appends each call's plan to `plans` where given.  Returns numpy (accum, counts, pixels, rgb)."""
     torch = _torch()
     accum = torch.full((h, w, 3), float("nan"), dtype=torch.float32, device="cuda") if accum is None else accum
     counts = torch.zeros((h, w), dtype=torch.int32, device="cuda") if counts is None else counts
@@ -115,6 +116,8 @@ def _adaptive_chain(ctx, pr, h, w, masks, n_adds, accum=None, counts=None, check
         m = None if mask is None else (mask if isinstance(mask, torch.Tensor) else torch.from_numpy(np.asarray(mask, bool)).cuda())
         ctx.render_adaptive(pr, accum, counts, n, mask=m, pixels=pix, rgb=rgb)
         assert ctx.last_plan()["query"] == "adaptive"
+        if plans is not None:
+            plans.append(ctx.last_plan())
         if check_untouched and m is not None:
             off = ~m.bool()
             for t0, t in zip(before, (accum, counts, pix, rgb)):
@@ -159,14 +162,19 @@ def test_uniform_counts_equal_render_accumulate(R, scene, h, w):
 @pytest.mark.gpu
 @pytest.mark.parametrize("spread", [1, 0])
 def test_both_sample_paths(R, spread):
-    """Calls of 1 (pixel-bound), 2 to 1985 (spread) and 1986 samples (over the finished-sample budget: pixel-bound)."""
+    """Calls of 1 (pixel-bound), 2 up to the last count whose finished-sample buffer fits the budget at 32 warps on this
+    GPU's SMs (spread) and one more (pixel-bound); with wq_spread 0 all pixel-bound."""
     h, w = 4, 8
-    split = [(0, 1), (1, 3), (3, 10), (10, 11), (11, 75), (75, 2060), (2060, 4046)]
-    ctx, pr = _ctx(R, "irreg", h, w, wq_spread=spread)
+    last = last_spread_spp(_torch().cuda.get_device_properties(0).multi_processor_count)
+    split = [(0, 1), (1, 3), (3, 10), (10, 11), (11, 75), (75, 75 + last), (75 + last, 76 + 2 * last)]
+    ctx, pr = _ctx(R, "irreg", h, w, wq_spread=spread, **BOUNDARY_PLAN)
     want = _chain(ctx, pr, h, w, split)
-    acc, cnt, pix, rgb = _adaptive_chain(ctx, pr, h, w, [None] * len(split), [b - a for a, b in split])
-    assert (cnt == 4046).all()
+    plans = []
+    acc, cnt, pix, rgb = _adaptive_chain(ctx, pr, h, w, [None] * len(split), [b - a for a, b in split], plans=plans)
+    assert (cnt == split[-1][1]).all()
     assert bits_differ(acc, want[0]) == 0 and (pix == want[1]).all() and bits_differ(rgb, want[2]) == 0
+    assert [p["spread"] for p in plans] == [int(spread and 1 < b - a <= last) for a, b in split]
+    assert plans[-2]["spread"] == spread and plans[-1]["spread"] == 0 and {p["warps"] for p in plans} == {32}
     ctx.close()
 
 
