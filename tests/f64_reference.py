@@ -18,10 +18,12 @@ TAU = 1e-5                     # a margin below this is a near-tie: the sample i
 PERTURB = 1e-5                 # relative size of the two perturbations of a path's primary direction
 COLOUR_TOL = 2e-4              # the largest colour error estimate a judged sample may have, relative to max(1, |c|)
 QUANT_TAU = 0.002              # distance of 255.99 c from an integer below which a pixel is not judged
-OFFSET_X, OFFSET_Y = 0.7548776662, 0.5698402909
+OFFSET_X, OFFSET_Y = np.float32(0.7548776662), np.float32(0.5698402909)
 SKY = np.array([0.5, 0.7, 1.0])
+U32 = 2.0 ** -24               # the unit roundoff of f32
 MUTANTS = ("aspect_h_over_w", "v_from_j", "offsets_s_plus_1", "sky_from_x", "no_stale_culling", "no_perm",
-           "reintersect_from_eps")
+           "reintersect_from_eps", "offsets_in_f64", "welford_old_mean", "select_without_count",
+           "gbuffer_depth_last_sample", "gbuffer_id_in_leaf_order", "gbuffer_miss_albedo_black")
 _PAIR_BUDGET = 1 << 21          # rays x spheres per chunk of the dense discriminant pass (8 f64 arrays of this size)
 
 
@@ -53,21 +55,44 @@ def make_camera(cam7, h, w, aspect=None):
 
 
 def sample_offsets(s, mutant=None):
-    """(ox_s, oy_s) = frac(s * 0.7548776662), frac(s * 0.5698402909) in f64 (include/ray_b200.h, spp semantics)."""
-    s = np.asarray(s, np.float64) + (1 if mutant == "offsets_s_plus_1" else 0)
-    return np.modf(s * OFFSET_X)[0], np.modf(s * OFFSET_Y)[0]
+    """(ox_s, oy_s) = frac(f32(s) * 0.7548776662f), frac(f32(s) * 0.5698402909f) for int64 indices s, as f64
+    (include/ray_b200.h, spp semantics).  The rule is discrete: f32(s), the f32 product, its floor and the difference
+    are each one exact or correctly rounded step, so restating it in f32 is the rule itself, not an approximation of
+    it.  From 2^21 / c on the offsets are quarters and halves, and from 2^23 / c on they are 0."""
+    s = np.asarray(s, np.int64) + (1 if mutant == "offsets_s_plus_1" else 0)
+    if mutant == "offsets_in_f64":   # frac(s * c) in f64: right to about 3e-6 below 2^16, wrong by up to 0.99 at 2^21 / c on
+        s = s.astype(np.float64)
+        return np.modf(s * 0.7548776662)[0], np.modf(s * 0.5698402909)[0]
+    sf = s.astype(np.float32)
+    a, b = sf * OFFSET_X, sf * OFFSET_Y
+    return (a - np.floor(a)).astype(np.float64), (b - np.floor(b)).astype(np.float64)
 
 
 def primary_rays(cam7, h, w, j, i, s, mutant=None):
     """Sample s of pixel (row j, column i): u = (i + ox_s) / W, v = (H - j + oy_s) / H, get_ray (ray.fut:109-114)."""
+    ox, oy = sample_offsets(s, mutant)
+    return offset_rays(cam7, h, w, j, i, ox, oy, mutant)
+
+
+def offset_rays(cam7, h, w, j, i, ox, oy, mutant=None):
+    """primary_rays with the sample offsets (ox, oy) given."""
     aspect = h / w if mutant == "aspect_h_over_w" else None
     origin, llc, hor, ver = make_camera(cam7, h, w, aspect)
-    ox, oy = sample_offsets(s, mutant)
     j = np.asarray(j, np.float64)
     u = (np.asarray(i, np.float64) + ox) / w
     v = ((j if mutant == "v_from_j" else h - j) + oy) / h
     d = llc + u[:, None] * hor + v[:, None] * ver - origin
     return np.broadcast_to(origin, d.shape).copy(), d
+
+
+def _perturbed(D):
+    """The two directions D perturbed by PERTURB relative, orthogonally to D and to each other."""
+    dn = np.sqrt(_dot(D, D))[:, None]
+    e1 = np.cross(D, [0.0, 0.0, 1.0])
+    e1 = np.where((np.abs(_dot(e1, e1)) < 1e-12 * dn[:, 0] ** 2)[:, None], np.cross(D, [1.0, 0.0, 0.0]), e1)
+    e1 = _normalise(e1)
+    e2 = _normalise(np.cross(D, e1))
+    return D + PERTURB * dn * e1, D + PERTURB * dn * e2
 
 
 # ------------------------------------------------------------------------------------------ quantisation
@@ -376,6 +401,13 @@ class Reference:
 
     # -------------------------------------------------------------------- ray_colour
 
+    def _sky(self, D):
+        """The sky colour of directions D (ray.fut:141-148)."""
+        ud = _normalise(D)
+        t = 0.5 * (ud[:, 0 if self.mutant == "sky_from_x" else 1] + 1.0)
+        with np.errstate(invalid="ignore", over="ignore"):
+            return (1.0 - t)[:, None] + t[:, None] * SKY
+
     def paths(self, O, D, max_depth=50):
         """ray_colour (ray.fut:126-148) in f64: (colour[m][3], segments[m], leaves[m][max_depth] (-1 after the last
         hit), margin[m]).  Every segment searches (0, 1e9)."""
@@ -396,10 +428,8 @@ class Reference:
             leaves[act[hit], depth] = h["leaf"][hit]
             # miss: the sky (ray.fut:141-148)
             miss = act[~hit]
-            ud = _normalise(D[miss])
-            t = 0.5 * (ud[:, 0 if self.mutant == "sky_from_x" else 1] + 1.0)
             with np.errstate(invalid="ignore", over="ignore"):
-                colour[miss] = light[miss] * ((1.0 - t)[:, None] + t[:, None] * SKY)
+                colour[miss] = light[miss] * self._sky(D[miss])
             # hit: scatter (ray.fut:116-124)
             hh = act[hit]
             n = h["normal"][hit]
@@ -426,14 +456,9 @@ class Reference:
         leaves, err, judged); err is relative to max(1, |c|)."""
         col, seg, leaves, margin = self.paths(O, D, max_depth)
         judged = margin > TAU
-        dn = np.sqrt(_dot(D, D))[:, None]
-        e1 = np.cross(D, [0.0, 0.0, 1.0])
-        e1 = np.where((np.abs(_dot(e1, e1)) < 1e-12 * dn[:, 0] ** 2)[:, None], np.cross(D, [1.0, 0.0, 0.0]), e1)
-        e1 = _normalise(e1)
-        e2 = _normalise(np.cross(D, e1))
         err = np.full(len(O), 1e-6)
-        for e in (e1, e2):
-            c2, s2, l2, _ = self.paths(O, D + PERTURB * dn * e, max_depth)
+        for D2 in _perturbed(D):
+            c2, s2, l2, _ = self.paths(O, D2, max_depth)
             with np.errstate(invalid="ignore"):
                 dc = np.nan_to_num(np.abs(c2 - col) / np.maximum(1.0, np.abs(col)), nan=0.0).max(1)
             err = np.maximum(err, dc)
@@ -455,3 +480,98 @@ class Reference:
         pix, qm = quantise(mean)
         scale = np.nan_to_num(np.maximum(1.0, np.abs(mean)).max(1), nan=1.0, posinf=1.0)
         return pix, mean, err, judged.reshape(len(j), spp).all(1) & (qm > QUANT_TAU + 255.99 * err * scale)
+
+    def samples(self, h, w, j, i, s, cam7=None, max_depth=50):
+        """Sample s of pixel (row j, column i) of an h x w frame, for integer arrays j, i, s (broadcast together):
+        (colour [..., 3], err [...], judged [...]) of judged_paths.  Samples of one pixel whose offsets coincide (every
+        sample from 2^23 / c on is the sample-0 ray, and the offsets are quarters or halves from 2^21 / c on) are one
+        ray, traced once."""
+        cam7 = self.cam7 if cam7 is None else cam7
+        j, i, s = np.broadcast_arrays(np.asarray(j, np.int64), np.asarray(i, np.int64), np.asarray(s, np.int64))
+        ox, oy = sample_offsets(s.ravel(), self.mutant)
+        key = np.stack([j.ravel().astype(np.float64), i.ravel().astype(np.float64), ox, oy], 1)
+        uniq, inv = np.unique(key, axis=0, return_inverse=True)
+        inv = inv.reshape(-1)
+        O, D = offset_rays(cam7, h, w, uniq[:, 0], uniq[:, 1], uniq[:, 2], uniq[:, 3], self.mutant)
+        col, _, _, err, judged = self.judged_paths(O, D, max_depth)
+        return col[inv].reshape(s.shape + (3,)), err[inv].reshape(s.shape), judged[inv].reshape(s.shape)
+
+    # -------------------------------------------------------------------- G-buffer
+
+    def gbuffer(self, h, w, j, i, spp, cam7=None):
+        """The first-hit buffers of pixels (row j, column i) of an h x w frame at spp (include/ray_b200.h,
+        ray_b200_render_gbuffer), from closest(ray, 0, 1e9) of every sample's camera ray: id, the caller's index of
+        sample 0's sphere (-1 on a miss); depth, sample 0's t (-1); coverage, how many samples hit; normal and albedo,
+        means over the samples of the hit normal (0 on a miss) and of the hit sphere's colour (the sky colour of the
+        ray on a miss).  Returns (buffers dict, judged [n], records): a pixel is judged when every sample's margin
+        exceeds TAU and both perturbed directions of every sample hit the same sphere; records are closest()'s of
+        every sample, shaped [n, spp, ...], with the rays' origins and directions under "O" and "D"."""
+        cam7 = self.cam7 if cam7 is None else cam7
+        j, i = np.asarray(j), np.asarray(i)
+        n = len(j)
+        O, D = primary_rays(cam7, h, w, np.repeat(j, spp), np.repeat(i, spp), np.tile(np.arange(spp), n), self.mutant)
+        rec = self.closest(O, D, 0.0, 1e9)
+        judged = rec["margin"] > TAU
+        for D2 in _perturbed(D):
+            judged &= self.closest(O, D2, 0.0, 1e9)["leaf"] == rec["leaf"]
+        hit = rec["leaf"] >= 0
+        sky = np.zeros((len(O), 3)) if self.mutant == "gbuffer_miss_albedo_black" else self._sky(D)
+        albedo = np.where(hit[:, None], self.col[np.maximum(rec["leaf"], 0)], sky)
+        rec = {k: v.reshape((n, spp) + v.shape[1:]) for k, v in dict(rec, O=O, D=D).items()}
+        first = -1 if self.mutant == "gbuffer_depth_last_sample" else 0
+        ident = np.where(rec["leaf"][:, 0] >= 0, rec["leaf"][:, 0], -1) if self.mutant == "gbuffer_id_in_leaf_order" \
+            else rec["sphere"][:, 0]
+        out = dict(id=ident, depth=rec["t"][:, first], coverage=hit.reshape(n, spp).sum(1),
+                   normal=rec["normal"].mean(1), albedo=albedo.reshape(n, spp, 3).mean(1))
+        return out, judged.reshape(n, spp).all(1), rec
+
+    # -------------------------------------------------------------------- the noise estimate
+
+    def m2(self, colours):
+        """(sum, M2) of colours float64 [..., n, 3] over their samples (axis -2), by Welford's update in f64: M2 += (x_k -
+        S_k / k) (x_k - S_{k+1} / (k + 1)) after sample k >= 1, which is the sum of squared deviations from the mean, so
+        M2 / (n - 1) is the unbiased sample variance (include/ray_b200.h, ray_b200_render_adaptive_var)."""
+        x = np.asarray(colours, np.float64)
+        S, M = x[..., 0, :].copy(), np.zeros_like(x[..., 0, :])
+        with np.errstate(invalid="ignore", over="ignore"):
+            for k in range(1, x.shape[-2]):
+                xk = x[..., k, :]
+                nxt = S + xk
+                if self.mutant == "welford_old_mean":
+                    M = M + (xk - S / k) ** 2
+                else:
+                    M = M + (xk - S / k) * (xk - nxt / (k + 1))
+                S = nxt
+        return S, M
+
+    def select(self, S, M2, n, rel_err, mean_floor, min_count, max_count):
+        """ray_b200_adaptive_select in f64 on sums S [..., 3] and M2 [..., 3] of n samples (n [...] int): (mask, E, T)
+        where E = sum of M2 / (n (n - 1)), the variance of the mean summed over the channels, T = (rel_err (sum of S / n
+        + mean_floor))^2, and the mask is 0 <= n < max_count and (n < min_count or E > T)."""
+        n = np.asarray(n, np.float64)
+        with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+            v = np.asarray(M2, np.float64).sum(-1)
+            E = v / (n - 1) if self.mutant == "select_without_count" else v / (n * (n - 1))
+            T = (rel_err * (np.asarray(S, np.float64).sum(-1) / n + mean_floor)) ** 2
+            mask = (n >= 0) & (n < max_count) & ((n < min_count) | (E > T))
+        return mask, E, T
+
+
+def m2_bound(x, delta):
+    """A bound on |M2_f32 - M2| per channel, where M2 is the f64 sum of squared deviations of the f64 colours x
+    [..., n, 3] and M2_f32 is Welford's update run in f32 on colours within delta [..., n, 3] of x:
+
+    * the propagated colour error: moving each x_k by at most D = max delta moves each deviation x_k - mean by at most
+      2 D, so M2 moves by at most 4 D sum|x_k - mean| + 4 n D^2;
+    * Welford's f32 error: the running sum S_k is within (k - 1) k u X of its exact value (u = 2^-24, X = max |x_k|), so
+      S_k / k is within (k + 1) u X, each factor x_k - S_k / k within (k + 3) u X and each term within 4 (k + 4) u X^2;
+      over n - 1 terms that is 2 (n + 4)^2 u X^2, and the n - 1 additions of the terms add (n - 1) u M2.
+
+    Twice that sum is returned.  Everything here is finite; NaN colours are compared as NaN."""
+    x = np.asarray(x, np.float64)
+    n = x.shape[-2]
+    D = np.asarray(delta, np.float64).max(-2)
+    X = np.abs(x).max(-2) + D
+    dev = np.abs(x - x.mean(-2, keepdims=True)).sum(-2)
+    M2 = ((x - x.mean(-2, keepdims=True)) ** 2).sum(-2)
+    return 2 * (4 * D * dev + 4 * n * D * D + 2 * (n + 4) ** 2 * U32 * X * X + (n - 1) * U32 * (M2 + 4 * D * dev))

@@ -347,7 +347,16 @@ def _mutant_hits(mutant, name, rays, lo):
     return judge_hits(reference(name, mutant), rays, lo, 1e9, got)
 
 
+def _sample_mutant(mutant):
+    """A mutant of the per-sample, noise-estimate or G-buffer parts, rejected by test_f64_samples' case for it."""
+    import test_f64_samples   # imported here: it imports this module
+    return test_f64_samples.MUTANT_CASES[mutant](mutant)
+
+
 MUTANT_CASES = {
+    "offsets_in_f64": _sample_mutant, "welford_old_mean": _sample_mutant, "select_without_count": _sample_mutant,
+    "gbuffer_depth_last_sample": _sample_mutant, "gbuffer_id_in_leaf_order": _sample_mutant,
+    "gbuffer_miss_albedo_black": _sample_mutant,
     "aspect_h_over_w": lambda m: _mutant_frame(m, "rgbbox", 48, 160, 1),
     "v_from_j": lambda m: _mutant_frame(m, "irreg", 37, 53, 1),
     "offsets_s_plus_1": lambda m: _mutant_frame(m, "irreg", 37, 53, 3),
