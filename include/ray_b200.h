@@ -204,12 +204,26 @@ int ray_b200_prepared_update(struct futhark_context *ctx, struct futhark_opaque_
 int ray_b200_prepared_spheres(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
                               float *spheres_dev, float *cam7_host);
 
-/* ---- scene batches: many small scenes of equal size, built and rendered together ------------------------------------
- * A caller with B scenes of n spheres each in device memory (vectorised environments, a dataset generator, a sweep over
- * a model's outputs) builds all B trees in one pass and renders one frame of every scene in one launch, instead of one
- * prepare and one render call per scene.  spheres_dev: device float[B][n][7], scene b's records at b n 7, each scene in
- * the layout of ray_b200_scene_from_arrays, 4-byte aligned, readable by the context's device; cams7_host: host
- * float[B][7], scene b's camera as there.  B = n_scenes >= 1, 2 <= n, B n <= 2^26; every scene has the same n.
+/* ---- scene batches: many small scenes, built and rendered together ------------------------------------------------
+ * A caller with B scenes in device memory (vectorised environments, a dataset generator, a sweep over a model's
+ * outputs) builds all B trees in one pass and renders one frame of every scene in one launch, instead of one prepare and
+ * one render call per scene.  spheres_dev: device float[B][n][7], scene b's records at b n 7, each scene in the layout
+ * of ray_b200_scene_from_arrays, 4-byte aligned, readable by the context's device; cams7_host: host float[B][7], scene
+ * b's camera as there.  B = n_scenes >= 1, 2 <= n, B n <= 2^26.
+ *   Ragged batches.  ray_b200_scene_batch_new_ragged builds B scenes of different sizes: scene b has counts_host[b] =
+ *   n_b >= 2 spheres (host int64[B], N = n_0 + .. + n_{B-1} <= 2^26), packed back to back in spheres_dev = device
+ *   float[N][7], scene b's records from row off_b = n_0 + .. + n_{b-1}.  Everything below holds for it with S + 7 n b
+ *   read as S + 7 off_b and n as n_b: member b is bit for bit ray_b200_prepare_scene_device(h, w, S + 7 off_b, n_b,
+ *   cams7 + 7 b), including its refit_sweeps, trunc(log2f(n_b)) + 2, and the stale boxes that count leaves (no padding
+ *   sphere could keep them: it would move the box the Morton keys are quantised in).  A uniform batch is a ragged batch
+ *   whose counts are equal: new_device(B, n) and new_ragged with B counts n make the same batch, bit for bit.
+ *   ray_b200_scene_batch_update_ragged rebuilds every member from new records and new counts (B stays; counts may
+ *   differ from the current ones), as update does; ray_b200_scene_batch_update on a batch whose counts differ is an
+ *   error that changes nothing.  ray_b200_scene_batch_shape reports n = the common count, or 0 when the members differ;
+ *   ray_b200_scene_batch_counts writes the B counts to counts_host (host int64[B]).  Frames and every
+ *   ray_b200_scene_batch_trace_* take a ragged batch as they are; the sphere of a hit record indexes scene b's own
+ *   records, in [0, n_b).  Errors, on top of new_device's: a NULL counts_host, a count < 2, N > 2^26, and spheres_dev
+ *   not device-readable.
  *   Exactness.  Member b of ray_b200_scene_batch_new_device(h, w, S, B, n, cams7) is bit for bit the prepared scene
  *   ray_b200_prepare_scene_device(h, w, S + 7 n b, n, cams7 + 7 b) makes: ray_b200_scene_batch_member returns it, and its
  *   prepared_info (every field), prepared_dump, prepared_packed, prepared_spheres, frames and ray queries are that
@@ -242,12 +256,20 @@ int ray_b200_prepared_spheres(struct futhark_context *ctx, const struct futhark_
 struct ray_b200_scene_batch;
 int ray_b200_scene_batch_new_device(struct futhark_context *ctx, struct ray_b200_scene_batch **out, int64_t h, int64_t w,
                                     const float *spheres_dev, int32_t n_scenes, int64_t n, const float *cams7_host);
+int ray_b200_scene_batch_new_ragged(struct futhark_context *ctx, struct ray_b200_scene_batch **out, int64_t h, int64_t w,
+                                    const float *spheres_dev, int32_t n_scenes, const int64_t *counts_host,
+                                    const float *cams7_host);
 int ray_b200_scene_batch_update(struct futhark_context *ctx, struct ray_b200_scene_batch *b, const float *spheres_dev,
                                 const float *cams7_host);
+int ray_b200_scene_batch_update_ragged(struct futhark_context *ctx, struct ray_b200_scene_batch *b, const float *spheres_dev,
+                                       const int64_t *counts_host /* B counts; may differ from the current ones */,
+                                       const float *cams7_host /* NULL keeps the cameras */);
 int ray_b200_scene_batch_free(struct futhark_context *ctx, struct ray_b200_scene_batch *b);
-/* the batch's B and n */
+/* the batch's B and n (0 when its members' counts differ) */
 int ray_b200_scene_batch_shape(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t *n_scenes,
                                int64_t *n);
+/* the batch's B counts */
+int ray_b200_scene_batch_counts(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int64_t *counts_host);
 int ray_b200_scene_batch_member(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t s,
                                 struct futhark_opaque_prepared_scene **out);
 int ray_b200_render_scene_batch_into(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int64_t h,
@@ -261,7 +283,7 @@ int ray_b200_render_scene_batch_into(struct futhark_context *ctx, const struct r
  * in some scenes pads them with ranged rays whose interval is empty, such as (0, 0): they get the empty answer.
  *   Exactness.  The answer for ray j of scene b is bit for bit what the single-scene entry point returns for that ray on
  *   ray_b200_scene_batch_member(b), and so on ray_b200_prepare_scene_device of scene b's records: every word of every
- *   hit record (sphere is the index into scene b's own records, in [0, n)), the colours including their NaNs, segments,
+ *   hit record (sphere is the index into scene b's own records, in [0, n_b)), the colours including their NaNs, segments,
  *   occluded and counts.  Every interval rule of the single-scene queries holds as it is (epsilon 0.1 and the
  *   re-intersection of trace_hits, no epsilon for occlusion and multi-hit, (0, 1e9) for paths, the empty answer for an
  *   invalid per-ray interval).

@@ -22,7 +22,7 @@ import numpy as np
 
 __all__ = ["Context", "RayError", "Hit", "Ray", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
            "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays", "SceneBatch", "scene_batch_rows",
-           "scene_batch_cameras", "scene_batch_frames_ok"]
+           "scene_batch_counts", "scene_batch_cameras", "scene_batch_frames_ok"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 KERNELS = {"auto": 0, "mega": 1, "persistent": 2, "wavefront": 3, "warpqueue": 4, "streamqueue": 5, "lanewalk": 6}
@@ -177,7 +177,10 @@ def load_library(variant=""):
         "ray_b200_render_gbuffer": (C.c_int, [vp, vp, i64, i64, i32, vp, vp, vp, vp, vp]),
         "ray_b200_entry_render_spp": (C.c_int, [vp, pp, i64, i64, i32, vp]),
         "ray_b200_scene_batch_new_device": (C.c_int, [vp, pp, i64, i64, vp, i32, i64, vp]),
+        "ray_b200_scene_batch_new_ragged": (C.c_int, [vp, pp, i64, i64, vp, i32, vp, vp]),
         "ray_b200_scene_batch_update": (C.c_int, [vp, vp, vp, vp]),
+        "ray_b200_scene_batch_update_ragged": (C.c_int, [vp, vp, vp, vp, vp]),
+        "ray_b200_scene_batch_counts": (C.c_int, [vp, vp, vp]),
         "ray_b200_scene_batch_free": (C.c_int, [vp, vp]),
         "ray_b200_scene_batch_shape": (C.c_int, [vp, vp, C.POINTER(i32), C.POINTER(i64)]),
         "ray_b200_scene_batch_member": (C.c_int, [vp, vp, i32, pp]),
@@ -344,6 +347,34 @@ def scene_batch_rows(device, spheres):
     if B * n > 1 << 26:
         raise ValueError(f"a scene batch holds at most 2^26 spheres, got {B} x {n}")
     return B, n
+
+
+def scene_batch_counts(device, spheres, counts, B=None):
+    """(B, counts) of a ragged scene batch: counts, B >= 1 host integers (a sequence, array or CPU tensor; B of them when
+    B is given, as for an update), each >= 2 and summing to N <= 2^26, as a contiguous int64 array, and spheres, a
+    contiguous float32 CUDA tensor [N, 7] on cuda:device (scene b's records from row counts[0] + .. + counts[b - 1]);
+    ValueError for anything else.  The counts are checked first, on the host."""
+    import torch
+    if isinstance(counts, torch.Tensor):
+        if counts.device.type != "cpu":
+            raise ValueError("counts must be on the host (reading a CUDA tensor would synchronise the device)")
+        counts = counts.numpy()
+    c = np.asarray(counts) if counts is not None else np.zeros((0,), np.float32)
+    if c.ndim != 1 or len(c) < 1 or c.dtype.kind not in "iu":
+        raise ValueError(f"counts must be a 1-d sequence of B >= 1 integers, got {c.dtype} {c.shape}")
+    if B is not None and len(c) != B:
+        raise ValueError(f"counts must hold the batch's {B} counts, got {len(c)}")
+    if int(c.min()) < 2:
+        raise ValueError(f"every scene of a batch needs at least 2 spheres, got a count of {int(c.min())}")
+    if int(c.max()) > 1 << 26 or int(c.astype(np.int64).sum()) > 1 << 26:
+        raise ValueError("a scene batch holds at most 2^26 spheres, the counts sum to more")
+    c = np.ascontiguousarray(c, np.int64)
+    N = int(c.sum())
+    if not isinstance(spheres, torch.Tensor) or spheres.dim() != 2 or int(spheres.shape[0]) != N:
+        raise ValueError(f"spheres must be a float32 CUDA tensor of shape [N, 7] with N = sum(counts) = {N}, got "
+                         f"{tuple(spheres.shape) if isinstance(spheres, torch.Tensor) else type(spheres).__name__}")
+    _check_tensor(device, "spheres", spheres, (torch.float32,), (N, 7))
+    return len(c), c
 
 
 def scene_batch_cameras(cams, B):
@@ -523,16 +554,24 @@ class PreparedScene(_Handle):
 
 
 class SceneBatch(_Handle):
-    """B scenes of n spheres each, built together from device memory, rendered in one launch and traced by ray queries
-    in one launch (include/ray_b200.h "scene batches"; Context.render_scene_batch, Context.trace_scene_batch_*)."""
+    """B scenes, of n spheres each or of counts[b] spheres (a ragged batch), built together from device memory, rendered
+    in one launch and traced by ray queries in one launch (include/ray_b200.h "scene batches"; Context.render_scene_batch,
+    Context.trace_scene_batch_*)."""
     _free_fn = "ray_b200_scene_batch_free"
 
     @property
     def shape(self):
-        """(B, n)"""
+        """(B, n), n = 0 when the members' counts differ"""
         b, n = C.c_int32(0), C.c_int64(0)
         self.ctx._check(self.ctx.lib.ray_b200_scene_batch_shape(self.ctx.handle, self.handle, C.byref(b), C.byref(n)))
         return int(b.value), int(n.value)
+
+    @property
+    def counts(self):
+        """The B members' sphere counts, an int64 host array"""
+        out = np.empty(self.shape[0], np.int64)
+        self.ctx._check(self.ctx.lib.ray_b200_scene_batch_counts(self.ctx.handle, self.handle, out.ctypes.data))
+        return out
 
     def update_from_ptr(self, spheres_dev, cams=None):
         """ray_b200_scene_batch_update: every member rebuilt from the records at device address spheres_dev (float[B][n][7],
@@ -540,11 +579,31 @@ class SceneBatch(_Handle):
         c = None if cams is None else scene_batch_cameras(cams, self.shape[0])
         self.ctx._check(self.ctx.lib.ray_b200_scene_batch_update(self.ctx.handle, self.handle, _ptr(spheres_dev), _ptr(c)))
 
-    def update(self, spheres, cams=None):
+    def update_ragged_from_ptr(self, spheres_dev, counts, cams=None):
+        """ray_b200_scene_batch_update_ragged: every member rebuilt from the records at device address spheres_dev
+        (float[N][7], N = sum(counts), read on the context's stream), B new counts (host int64 array-like) and the host
+        cameras cams ([B, 7], None keeps them)."""
+        B = self.shape[0]
+        c = np.ascontiguousarray(counts, np.int64)
+        if c.shape != (B,):
+            raise ValueError(f"counts must hold the batch's {B} counts, got shape {c.shape}")
+        cam = None if cams is None else scene_batch_cameras(cams, B)
+        self.ctx._check(self.ctx.lib.ray_b200_scene_batch_update_ragged(self.ctx.handle, self.handle, _ptr(spheres_dev),
+                                                                        c.ctypes.data, _ptr(cam)))
+
+    def update(self, spheres, cams=None, counts=None):
         """Rebuilds every member from spheres, a contiguous float32 CUDA tensor of the batch's shape [B, n, 7], and cams
-        ([B, 7], see scene_batch_cameras) or None to keep the cameras.  Frames enqueued before the call render the old
-        trees.  Waits for torch's current stream before the call."""
+        ([B, 7], see scene_batch_cameras) or None to keep the cameras.  With counts (B host integers, see
+        scene_batch_counts; they may differ from the current ones), spheres is [sum(counts), 7], scene b's records from
+        row counts[0] + .. + counts[b - 1].  Frames enqueued before the call render the old trees.  Waits for torch's
+        current stream before the call."""
         import torch
+        if counts is not None:
+            B, c = scene_batch_counts(self.ctx.device, spheres, counts, B=self.shape[0])
+            cam = None if cams is None else scene_batch_cameras(cams, B)
+            torch.cuda.current_stream(spheres.device).synchronize()   # spheres may still be in flight on torch's stream
+            self.update_ragged_from_ptr(spheres.data_ptr(), c, cam)
+            return
         B, n = scene_batch_rows(self.ctx.device, spheres)
         if (B, n) != self.shape:
             raise ValueError(f"spheres must have the batch's shape {list(self.shape) + [7]}, got {list(spheres.shape)}")
@@ -667,11 +726,32 @@ class Context:
         c = scene_batch_cameras(cams, int(B))
         return self._out(SceneBatch, "ray_b200_scene_batch_new_device", int(h), int(w), _ptr(spheres_dev), int(B), int(n), _ptr(c))
 
-    def prepare_scene_batch(self, h, w, spheres, cams):
+    def prepare_scene_batch_ragged_from_ptr(self, h, w, spheres_dev, counts, cams):
+        """ray_b200_scene_batch_new_ragged: B = len(counts) scenes of counts[b] spheres, back to back from device address
+        spheres_dev (float[N][7], N = sum(counts), read on the context's stream) with the host cameras cams ([B, 7]).
+        Returns after the build's one read-back."""
+        c = np.ascontiguousarray(counts, np.int64)
+        if c.ndim != 1:
+            raise ValueError(f"counts must be a 1-d sequence of B integers, got shape {c.shape}")
+        cam = scene_batch_cameras(cams, len(c))
+        return self._out(SceneBatch, "ray_b200_scene_batch_new_ragged", int(h), int(w), _ptr(spheres_dev), len(c), c.ctypes.data,
+                         _ptr(cam))
+
+    def prepare_scene_batch(self, h, w, spheres, cams, counts=None):
         """A SceneBatch from spheres, a contiguous float32 CUDA tensor [B, n, 7] on the context's device (each scene in the
         layout of scene_from_arrays), and cams, [B, 7] cameras on the host or in a tensor.  Member b equals
-        prepare_scene_device(h, w, spheres[b], cams[b]) bit for bit.  Waits for torch's current stream before the call."""
+        prepare_scene_device(h, w, spheres[b], cams[b]) bit for bit.  With counts (B host integers, see
+        scene_batch_counts), the scenes may differ in size: spheres is [sum(counts), 7], scene b's records from row
+        off_b = counts[0] + .. + counts[b - 1], and member b equals prepare_scene_device(h, w, spheres[off_b:off_b +
+        counts[b]], cams[b]).  Waits for torch's current stream before the call."""
         import torch
+        if counts is not None:
+            B, c = scene_batch_counts(self.device, spheres, counts)
+            if not scene_batch_frames_ok(B, int(h), int(w)):
+                raise ValueError(f"{B} frames of {h}x{w} exceed one launch (2^25 tiles of 8x4 pixels, sides <= 65536)")
+            cam = scene_batch_cameras(cams, B)
+            torch.cuda.current_stream(spheres.device).synchronize()
+            return self.prepare_scene_batch_ragged_from_ptr(h, w, spheres.data_ptr(), c, cam)
         B, n = scene_batch_rows(self.device, spheres)
         if not scene_batch_frames_ok(B, int(h), int(w)):
             raise ValueError(f"{B} frames of {h}x{w} exceed one launch (2^25 tiles of 8x4 pixels, sides <= 65536)")

@@ -5,6 +5,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -114,8 +115,9 @@ struct futhark_opaque_prepared_scene {
   float root_box[6];
   int32_t max_depth = 0, stale_nodes = 0, refit_sweeps = 0;
   int64_t n = 0;
-  // > 1: the trees of a scene batch (ray_b200_scene_batch), `scenes` of n spheres each side by side in `dev`; max_depth is
-  // the deepest member's, root_box and cam are unused (the kernel reads each member's from dev.results / dev.cams)
+  // > 1: the trees of a scene batch (ray_b200_scene_batch), `scenes` trees of n spheres in all, back to back in `dev`
+  // (dev.scene_off places them); max_depth is the deepest member's, root_box and cam are unused (the kernel reads each
+  // member's from dev.results / dev.cams)
   int32_t scenes = 1;
   std::vector<futhark_opaque_prepared_scene *> peer_prepared;  // single-process multi-GPU: the same scene on every helper device
   DeviceBvh dev;    // everything resident in HBM (one stream-ordered allocation): packed BVH2C + the Karras-order LBVH
@@ -143,15 +145,19 @@ struct futhark_opaque_prepared_scene {
 };
 
 // The inner nodes and leaves of all of p's trees: what a launch plans over and stages
-inline int64_t n_inner_of(const futhark_opaque_prepared_scene *p) { return (int64_t)p->scenes * (p->n - 1); }
-inline int64_t n_leaves_of(const futhark_opaque_prepared_scene *p) { return (int64_t)p->scenes * p->n; }
+inline int64_t n_inner_of(const futhark_opaque_prepared_scene *p) { return p->n - p->scenes; }
+inline int64_t n_leaves_of(const futhark_opaque_prepared_scene *p) { return p->n; }
+// The refit sweeps of the reference's build of n spheres, trunc(log2f(n)) + 2 (bvh.fut:47), with the host libm as in
+// the reference's C backend
+inline int32_t refit_sweeps_of(int64_t n) { return (int32_t)log2f((float)n) + 2; }
 
-// B scenes of n spheres each, built and rendered together (include/ray_b200.h "scene batches")
+// B scenes of n_0 .. n_{B-1} spheres, built and rendered together (include/ray_b200.h "scene batches")
 struct ray_b200_scene_batch {
   futhark_opaque_prepared_scene scene;  // every member's tree (scene.scenes = B): planned, launched and released as one scene
   int64_t h = 0, w = 0;                 // of the build: the cameras' aspect ratio
   std::vector<float> cams7;             // [B][7] the members' cameras as given
   std::vector<BvhBuildResult> results;  // [B] each member's root box, depth and stale count
+  std::vector<int64_t> off;             // [B + 1] where each member's spheres start, as dev.scene_off (off[B] = scene.n)
 };
 
 struct futhark_i32_2d {

@@ -71,8 +71,8 @@ int trace(futhark_context *ctx, const futhark_opaque_prepared_scene *p, int64_t 
 }
 
 // A query of scene batch b, m rays per scene (include/ray_b200.h "scene batches"): the single-scene query of kind `kind`
-// as one launch over the B m rays, each traced in its own scene's tree (root node b (n - 1) and root box b of the
-// batch's device table, as the batch render reads them), planned over all B trees as the batch render is
+// as one launch over the B m rays, each traced in its own scene's tree (root node scene_off[b] - b and root box b of
+// the batch's device tables, as the batch render reads them), planned over all B trees as the batch render is
 int trace_batch(futhark_context *ctx, const ray_b200_scene_batch *b, int64_t m, Query kind, bool ranged, RayQuery Q,
                 const void *out, const char *what) {
   if (bad_ctx(ctx)) return 1;
@@ -85,7 +85,7 @@ int trace_batch(futhark_context *ctx, const ray_b200_scene_batch *b, int64_t m, 
     return 1;
   }
   Q.root_boxes = reinterpret_cast<const float *>(b->scene.dev.results);
-  Q.scene_inner = (int32_t)(b->scene.n - 1);
+  Q.scene_off = b->scene.dev.scene_off;
   Q.rays_per_scene = (int32_t)m;
   return enqueue(ctx, &b->scene, (int64_t)B * m, kind, ranged, Q, out, what);
 }

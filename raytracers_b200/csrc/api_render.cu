@@ -1018,6 +1018,6 @@ extern "C" int ray_b200_render_scene_batch_into(struct futhark_context *ctx, con
   f.q.n_views = b->scene.scenes;
   f.q.cams = b->scene.dev.cams;
   f.q.root_boxes = reinterpret_cast<const float *>(b->scene.dev.results);
-  f.q.scene_inner = (int32_t)(b->scene.n - 1);
+  f.q.scene_off = b->scene.dev.scene_off;
   return render_frame(ctx, f);
 }

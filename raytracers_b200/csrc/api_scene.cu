@@ -87,9 +87,9 @@ void free_prepared_device(futhark_context *ctx, futhark_opaque_prepared_scene *p
 }
 
 int build_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p, const float *d_spheres, int64_t n, bool drop_order) {
-  const int32_t sweeps = (int32_t)log2f((float)n) + 2;  // bvh.fut:47, host libm as in the reference's C backend
+  const int32_t sweeps = refit_sweeps_of(n), off[2] = {0, (int32_t)n};
   DeviceBvh fresh;
-  cudaError_t e = build_bvh_device(d_spheres, n, 1, sweeps, fresh, ctx->d_build_result, ctx->stream, &ctx->launches);
+  cudaError_t e = build_bvh_device(d_spheres, 1, off, &sweeps, fresh, ctx->d_build_result, ctx->stream, &ctx->launches);
   // the host needs the tree depth (stack sizing) and the root box (kernel parameter) before the first render
   if (e == cudaSuccess)
     e = cudaMemcpyAsync(ctx->h_build_result, ctx->d_build_result, sizeof(BvhBuildResult), cudaMemcpyDeviceToHost, ctx->stream);
@@ -608,25 +608,47 @@ int check_batch_context(futhark_context *ctx, const char *what) {
   return 0;
 }
 
-// The trees of bt's B scenes of n spheres from the records at spheres_dev and the cameras cams7 (host [B][7]) made for
-// bt's (h, w): built into a new block, then the old one is released behind the renders still reading it.  One read-back
-// of the B build results ends the call.  A failed build leaves bt as it was.
-int build_batch(futhark_context *ctx, ray_b200_scene_batch *bt, const float *spheres_dev, int32_t B, int64_t n, const float *cams7) {
+// The counts of a ragged batch (host [B], each >= 2, their sum <= 2^26) and the records at spheres_dev over their sum:
+// the checks of new_ragged and update_ragged (an error here changes nothing)
+int check_batch_counts(futhark_context *ctx, const char *what, const float *spheres_dev, int32_t B, const int64_t *counts) {
+  if (!counts) { set_error(ctx, "%s: null argument", what); return 1; }
+  int64_t total = 0;
+  for (int32_t b = 0; b < B; b++) {
+    if (counts[b] < 2) { set_error(ctx, "%s: scene %d has %lld spheres, a scene needs at least 2", what, b, (long long)counts[b]); return 1; }
+    total += counts[b] < ((int64_t)1 << 27) ? counts[b] : ((int64_t)1 << 27);  // (no overflow: the sum is checked as it grows)
+    if (total > ((int64_t)1 << 26)) {
+      set_error(ctx, "%s: the counts of %d scenes exceed 2^26 spheres (this build packs leaf indices into 26 bits)", what, B);
+      return 1;
+    }
+  }
+  return check_device_records(ctx, what, spheres_dev, total);
+}
+
+// The trees of bt's B scenes of counts[b] spheres, back to back from the records at spheres_dev, and the cameras cams7
+// (host [B][7]) made for bt's (h, w): built into a new block, then the old one is released behind the renders still
+// reading it.  One read-back of the B build results ends the call.  A failed build leaves bt as it was.
+int build_batch(futhark_context *ctx, ray_b200_scene_batch *bt, const float *spheres_dev, int32_t B, const int64_t *counts,
+                const float *cams7) {
   futhark_opaque_prepared_scene *p = &bt->scene;
-  const int32_t sweeps = (int32_t)log2f((float)n) + 2;  // bvh.fut:47, as build_on_device
   const size_t cam_bytes = (size_t)B * sizeof(CameraRec), res_bytes = (size_t)B * sizeof(BvhBuildResult);
+  const size_t off_bytes = ((size_t)B + 1) * 4, sweep_bytes = (size_t)B * 4;
   static_assert(sizeof(CameraRec) == 48 && sizeof(BvhBuildResult) == 32, "the batch's device tables");
-  if (acquire_pinned(ctx, p, cam_bytes + res_bytes)) return 1;
+  if (acquire_pinned(ctx, p, cam_bytes + res_bytes + off_bytes + sweep_bytes)) return 1;
   CameraRec *cams = reinterpret_cast<CameraRec *>(p->pinned);
   BvhBuildResult *res = reinterpret_cast<BvhBuildResult *>(p->pinned + cam_bytes);
-  for (int32_t b = 0; b < B; b++) {  // what prepare_scene makes of the camera: make_camera for the build's (h, w)
-    HostScene s;
+  int32_t *off = reinterpret_cast<int32_t *>(p->pinned + cam_bytes + res_bytes);
+  int32_t *sweeps = off + (B + 1);
+  off[0] = 0;
+  for (int32_t b = 0; b < B; b++) {
+    off[b + 1] = off[b] + (int32_t)counts[b];
+    sweeps[b] = refit_sweeps_of(counts[b]);
+    HostScene s;  // what prepare_scene makes of the camera: make_camera for the build's (h, w)
     const float *c = cams7 + 7 * (size_t)b;
     memcpy(s.look_from, c, 12); memcpy(s.look_at, c + 3, 12); s.fov = c[6];
     cams[b] = make_camera(s, bt->h, bt->w);
   }
   DeviceBvh fresh;
-  cudaError_t e = build_bvh_device(spheres_dev, n, B, sweeps, fresh, nullptr, ctx->stream, &ctx->launches);
+  cudaError_t e = build_bvh_device(spheres_dev, B, off, sweeps, fresh, nullptr, ctx->stream, &ctx->launches);
   if (e == cudaSuccess) e = cudaMemcpyAsync(fresh.cams, cams, cam_bytes, cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(res, fresh.results, res_bytes, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaEventRecord(p->pinned_event, ctx->stream);
@@ -638,17 +660,53 @@ int build_batch(futhark_context *ctx, ray_b200_scene_batch *bt, const float *sph
   }
   if (release_scene_block(ctx, p, true)) { cudaFreeAsync(fresh.block, ctx->stream); return 1; }
   p->dev = fresh;
-  p->n = n;
+  p->n = off[B];
   p->scenes = B;
-  p->refit_sweeps = sweeps;
+  p->refit_sweeps = 0;  // (each member's is its own, refit_sweeps_of its count)
   memset(p->root_box, 0, sizeof p->root_box);  // (each member's is in p->dev.results)
   p->max_depth = 0;
   for (int32_t b = 0; b < B; b++) p->max_depth = std::max(p->max_depth, res[b].max_depth);
   p->host_current = false;
   p->host_built = false;
   bt->results.assign(res, res + B);
+  bt->off.assign(off, off + B + 1);
   if (cams7 != bt->cams7.data()) bt->cams7.assign(cams7, cams7 + 7 * (size_t)B);
   return 0;
+}
+
+// ray_b200_scene_batch_new_device and _new_ragged: a batch of B scenes of counts[b] spheres
+int new_batch(futhark_context *ctx, ray_b200_scene_batch **out, int64_t h, int64_t w, const float *spheres_dev, int32_t n_scenes,
+              const int64_t *counts, const float *cams7_host, const char *what) {
+  if (!out || !cams7_host) { set_error(ctx, "%s: null argument", what); return 1; }
+  if (h <= 0 || w <= 0) { set_error(ctx, "%s: bad image size", what); return 1; }
+  if (n_scenes < 1) { set_error(ctx, "%s: n_scenes must be >= 1, got %d", what, n_scenes); return 1; }
+  if (check_batch_context(ctx, what)) return 1;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (check_batch_counts(ctx, what, spheres_dev, n_scenes, counts)) return 1;
+  if ((int64_t)n_scenes * tiles_total(h, w) > ((int64_t)1 << 25)) {
+    set_error(ctx, "%s: %d frames of %lldx%lld exceed 2^30 padded pixels", what, n_scenes, (long long)h, (long long)w);
+    return 1;
+  }
+  ray_b200_scene_batch *bt = new ray_b200_scene_batch;
+  bt->h = bt->scene.h = h;
+  bt->w = bt->scene.w = w;
+  if (build_batch(ctx, bt, spheres_dev, n_scenes, counts, cams7_host)) { free_prepared_device(ctx, &bt->scene); delete bt; return 1; }
+  *out = bt;
+  return 0;
+}
+
+// The count of every member of b, or 0 when they differ
+int64_t common_count(const ray_b200_scene_batch *b) {
+  const int64_t n = b->off[1] - b->off[0];
+  for (size_t s = 1; s + 1 < b->off.size(); s++)
+    if (b->off[s + 1] - b->off[s] != n) return 0;
+  return n;
+}
+
+std::vector<int64_t> counts_of(const ray_b200_scene_batch *b) {
+  std::vector<int64_t> c(b->off.size() - 1);
+  for (size_t s = 0; s < c.size(); s++) c[s] = b->off[s + 1] - b->off[s];
+  return c;
 }
 
 }  // namespace
@@ -670,16 +728,15 @@ int ray_b200_scene_batch_new_device(struct futhark_context *ctx, struct ray_b200
     set_error(ctx, "%s: %d scenes of %lld spheres exceed 2^26 spheres (this build packs leaf indices into 26 bits)", what, n_scenes, (long long)n);
     return 1;
   }
-  if ((int64_t)n_scenes * tiles_total(h, w) > ((int64_t)1 << 25)) {
-    set_error(ctx, "%s: %d frames of %lldx%lld exceed 2^30 padded pixels", what, n_scenes, (long long)h, (long long)w);
-    return 1;
-  }
-  ray_b200_scene_batch *bt = new ray_b200_scene_batch;
-  bt->h = bt->scene.h = h;
-  bt->w = bt->scene.w = w;
-  if (build_batch(ctx, bt, spheres_dev, n_scenes, n, cams7_host)) { free_prepared_device(ctx, &bt->scene); delete bt; return 1; }
-  *out = bt;
-  return 0;
+  const std::vector<int64_t> counts((size_t)n_scenes, n);
+  return new_batch(ctx, out, h, w, spheres_dev, n_scenes, counts.data(), cams7_host, what);
+}
+
+int ray_b200_scene_batch_new_ragged(struct futhark_context *ctx, struct ray_b200_scene_batch **out, int64_t h, int64_t w,
+                                    const float *spheres_dev, int32_t n_scenes, const int64_t *counts_host, const float *cams7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  return new_batch(ctx, out, h, w, spheres_dev, n_scenes, counts_host, cams7_host, "scene_batch_new_ragged");
 }
 
 int ray_b200_scene_batch_update(struct futhark_context *ctx, struct ray_b200_scene_batch *b, const float *spheres_dev,
@@ -689,9 +746,36 @@ int ray_b200_scene_batch_update(struct futhark_context *ctx, struct ray_b200_sce
   const char *what = "scene_batch_update";
   if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
   if (check_batch_context(ctx, what)) return 1;
+  if (common_count(b) == 0) {
+    set_error(ctx, "%s: the batch's scenes have different counts (ray_b200_scene_batch_update_ragged updates it)", what);
+    return 1;
+  }
   CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
   if (check_device_records(ctx, what, spheres_dev, b->scene.n)) return 1;
-  return build_batch(ctx, b, spheres_dev, b->scene.scenes, b->scene.n, cams7_host ? cams7_host : b->cams7.data());
+  const std::vector<int64_t> counts = counts_of(b);
+  return build_batch(ctx, b, spheres_dev, b->scene.scenes, counts.data(), cams7_host ? cams7_host : b->cams7.data());
+}
+
+int ray_b200_scene_batch_update_ragged(struct futhark_context *ctx, struct ray_b200_scene_batch *b, const float *spheres_dev,
+                                       const int64_t *counts_host, const float *cams7_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  const char *what = "scene_batch_update_ragged";
+  if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
+  if (check_batch_context(ctx, what)) return 1;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+  if (check_batch_counts(ctx, what, spheres_dev, b->scene.scenes, counts_host)) return 1;
+  return build_batch(ctx, b, spheres_dev, b->scene.scenes, counts_host, cams7_host ? cams7_host : b->cams7.data());
+}
+
+int ray_b200_scene_batch_counts(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int64_t *counts_host) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);  // an update on another thread replaces b->off
+  if (!b) { set_error(ctx, "scene_batch_counts: invalid scene batch"); return 1; }
+  if (!counts_host) { set_error(ctx, "scene_batch_counts: null argument"); return 1; }
+  const std::vector<int64_t> counts = counts_of(b);
+  memcpy(counts_host, counts.data(), counts.size() * sizeof(int64_t));
+  return 0;
 }
 
 int ray_b200_scene_batch_free(struct futhark_context *ctx, struct ray_b200_scene_batch *b) {
@@ -707,9 +791,10 @@ int ray_b200_scene_batch_free(struct futhark_context *ctx, struct ray_b200_scene
 
 int ray_b200_scene_batch_shape(struct futhark_context *ctx, const struct ray_b200_scene_batch *b, int32_t *n_scenes, int64_t *n) {
   if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);  // (common_count reads b->off, which an update replaces)
   if (!b) { set_error(ctx, "scene_batch_shape: invalid scene batch"); return 1; }
   if (n_scenes) *n_scenes = b->scene.scenes;
-  if (n) *n = b->scene.n;
+  if (n) *n = common_count(b);
   return 0;
 }
 
@@ -725,7 +810,8 @@ int ray_b200_scene_batch_member(struct futhark_context *ctx, const struct ray_b2
   futhark_opaque_prepared_scene *p = new futhark_opaque_prepared_scene;
   p->h = b->h; p->w = b->w;
   set_camera(p, b->cams7.data() + 7 * (size_t)s);
-  const cudaError_t e = extract_scene_device(b->scene.dev, s, b->scene.n, p->dev, ctx->stream, &ctx->launches);
+  const int64_t off_s = b->off[(size_t)s], n = b->off[(size_t)s + 1] - off_s;
+  const cudaError_t e = extract_scene_device(b->scene.dev, s, off_s, n, p->dev, ctx->stream, &ctx->launches);
   if (e != cudaSuccess) {
     set_error(ctx, "%s: %s", what, cudaGetErrorString(e));
     free_prepared_device(ctx, p); delete p;
@@ -735,8 +821,8 @@ int ray_b200_scene_batch_member(struct futhark_context *ctx, const struct ray_b2
   if (record_scene_use(ctx, &b->scene, 0)) { free_prepared_device(ctx, p); delete p; return 1; }  // an update or free waits for the copy
   const BvhBuildResult &r = b->results[(size_t)s];
   memcpy(p->root_box, r.root_box, sizeof p->root_box);
-  p->max_depth = r.max_depth; p->stale_nodes = r.stale_nodes; p->refit_sweeps = b->scene.refit_sweeps;
-  p->n = b->scene.n;
+  p->max_depth = r.max_depth; p->stale_nodes = r.stale_nodes; p->refit_sweeps = refit_sweeps_of(n);
+  p->n = n;
   p->host_current = false;
   p->host_built = false;
   *out = p;

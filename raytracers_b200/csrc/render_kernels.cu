@@ -269,7 +269,7 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // work items, cameras and outputs of a views launch (frame b = scene b), over B trees that lie side by side in P's arrays
 // with global child and leaf indices, so a ray that starts at scene b's root only ever reaches scene b's nodes and
 // spheres.  What depends on the scene is where a segment starts: its set-up tests scene b's root box (Q.root_boxes, not
-// P.root_box) and pushes scene b's root node b * Q.scene_inner, for camera rays and bounces alike; b is the slot's work
+// P.root_box) and pushes scene b's root node Q.scene_off[b] - b (scene_root), for camera rays and bounces alike; b is the slot's work
 // item's tile over Q.view_tiles, so the slot carries nothing more.  The packet walk takes the new rays of one scene, the
 // first new ray's; the others of the round start in the item queue.  Nodes and spheres are staged as for one tree (a BFS prefix of the concatenated node array, or all of
 // it), the plan is made over the totals and the deepest member, and the claim order is the plain chunk permutation.
@@ -278,8 +278,9 @@ __global__ void __launch_bounds__(256) adaptive_select_kernel(const float *__res
 // ray_b200_scene_batch_trace_*): kClosest, kAnyHit and kMultiHit (kSingle, the kind each computes) over the trees of a
 // scene batch.  Ray c of the claims is scene b = c / Q.rays_per_scene's, so scene_of reads the slot's work item as it does
 // for kSceneBatch, and every segment's set-up (a path query's bounces too) tests scene b's root box and pushes scene b's
-// root node, the same code.  Leaves are scene b's own in their own order, shifted by b n, so the closest-hit tie-break
-// and the multi-hit key order are those of the scene alone; the finish takes b n off perm's global index (sphere_of).
+// root node, the same code.  Leaves are scene b's own in their own order, shifted by Q.scene_off[b], so the closest-hit
+// tie-break and the multi-hit key order are those of the scene alone; the finish takes Q.scene_off[b] off perm's global
+// index (sphere_of).
 
 // Query::kAnyHit: a leaf batch runs as soon as this many leaf items are queued (the other kinds wait for 32, a full
 // batch), so a ray's first accepted sphere, which ends its traversal, is found sooner.  16 was measured against 1, 8 and
@@ -386,11 +387,13 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
     if constexpr (is_batch_ray(kQuery)) return (int)((unsigned)p_item[slot] / (unsigned)Q.rays_per_scene);
     else return (int)((unsigned)(p_item[slot] >> 5) / (unsigned)Q.view_tiles);
   };
+  // a scene batch: the root node of scene b, the first of its inner nodes (scene_off[b] spheres and b trees before it)
+  [[maybe_unused]] auto scene_root = [&](const int b) { return __ldg(Q.scene_off + b) - b; };
   // ray mode: the caller's index of the sphere of Morton-sorted leaf `leaf`, reached by the ray in `slot`; a batch ray
-  // kind: the index into the ray's own scene's records, perm's global index less the b n spheres of the scenes before it
+  // kind: the index into the ray's own scene's records, perm's global index less the spheres of the scenes before it
   [[maybe_unused]] auto sphere_of = [&](const int slot, const auto leaf) {
     const int s = __ldg(Q.perm + leaf);
-    if constexpr (is_batch_ray(kQuery)) return s - scene_of(slot) * (Q.scene_inner + 1);
+    if constexpr (is_batch_ray(kQuery)) return s - __ldg(Q.scene_off + scene_of(slot));
     else return s;
   };
   // The first sample c of pixel (row pj, column pi) in this launch: 0 for a whole frame or views, the chunk's first sample
@@ -1047,7 +1050,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
           // straddle at most a few scene boundaries) start at their own scene's root in the item queue
           if (gm) {
             const bool go = (gm >> lane) & 1u;
-            const int root = go ? scene_of(lane + 32 * k) * Q.scene_inner : -1;
+            const int root = go ? scene_root(scene_of(lane + 32 * k)) : -1;
             const int r0 = __shfl_sync(kFullMask, root, __ffs(gm) - 1);
             const unsigned same = __ballot_sync(kFullMask, root == r0) & gm, other = gm & ~same;
             if (other) {
@@ -1063,7 +1066,7 @@ __global__ void __launch_bounds__(kWqMaxThreads, 1) render_warpqueue_kernel(cons
       } else {
         const bool go = (gm >> lane) & 1u;
         if constexpr (kBatch || is_batch_ray(kQuery)) {  // (slot, its scene's root node)
-          if (go) nstk[ntop + __popc(gm & lt_mask)] = ((uint32_t)(lane + 32 * k) << kSlotShift) | (uint32_t)(scene_of(lane + 32 * k) * Q.scene_inner);
+          if (go) nstk[ntop + __popc(gm & lt_mask)] = ((uint32_t)(lane + 32 * k) << kSlotShift) | (uint32_t)scene_root(scene_of(lane + 32 * k));
         } else {
           if (go) nstk[ntop + __popc(gm & lt_mask)] = (uint32_t)(lane + 32 * k) << kSlotShift;  // (slot, root node 0)
         }

@@ -69,8 +69,8 @@ struct RenderParams {
 // that also keeps each pixel's running sum of squared deviations (m2).  kGBuffer, a pixel kind: the first hit of every
 // camera ray of a frame (its sphere, t, normal and albedo), reduced per pixel into the guide buffers (gb_id, gb_depth,
 // gb_normal, gb_albedo, gb_coverage).  kSceneBatch, a pixel kind: one frame of each scene of a scene batch (cams, n_views,
-// view_tiles as kViews, root_boxes, scene_inner).  kBatchClosest, kBatchAnyHit and kBatchMultiHit, ray kinds: the
-// single-scene ray kind over the trees of a scene batch, rays_per_scene rays per scene (root_boxes, scene_inner as
+// view_tiles as kViews, root_boxes, scene_off).  kBatchClosest, kBatchAnyHit and kBatchMultiHit, ray kinds: the
+// single-scene ray kind over the trees of a scene batch, rays_per_scene rays per scene (root_boxes, scene_off as
 // kSceneBatch).  New kinds go at the end: kernel names carry the values, and tools/sass_compare.py reads older builds'
 // names by them.
 enum class Query { kPixels, kClosest, kAnyHit, kMultiHit, kAccumulate, kViews, kAdaptive, kAdaptiveVar, kGBuffer, kSceneBatch,
@@ -155,15 +155,15 @@ struct RayQuery {
   float *gb_albedo;
   int32_t *gb_coverage;
   // a scene batch (Query::kSceneBatch; include/ray_b200.h ray_b200_render_scene_batch_into): n_views = B frames as kViews
-  // lays them out, frame b of scene b with the camera cams[b].  The B trees lie side by side in P's arrays with global
-  // indices, scene_inner inner nodes each, so scene b's root is node b * scene_inner; its root box is the first 6 floats of
-  // root_boxes[8 b .. 8 b + 8) (struct BvhBuildResult records, 32-byte aligned), tested at every segment's set-up instead
-  // of P.root_box
+  // lays them out, frame b of scene b with the camera cams[b].  The B trees lie back to back in P's arrays with global
+  // indices: scene b's leaves start at scene_off[b] (device [B + 1]) and its inner nodes at scene_off[b] - b, so its root
+  // is node scene_off[b] - b; its root box is the first 6 floats of root_boxes[8 b .. 8 b + 8) (struct BvhBuildResult
+  // records, 32-byte aligned), tested at every segment's set-up instead of P.root_box
   const float *root_boxes;
-  int32_t scene_inner;
+  const int32_t *scene_off;
   // the ray kinds of a scene batch (Query::kBatchClosest / kBatchAnyHit / kBatchMultiHit; include/ray_b200.h
   // ray_b200_scene_batch_trace_*): rays [b * rays_per_scene, (b + 1) * rays_per_scene) are scene b's, traced from its root
-  // node b * scene_inner and root box as kSceneBatch; n = B * rays_per_scene, and the outputs follow the rays' order
+  // node and root box as kSceneBatch; n = B * rays_per_scene, and the outputs follow the rays' order
   int32_t rays_per_scene;
 };
 
