@@ -580,6 +580,60 @@ int ray_b200_trace_multi_hits_ranged(struct futhark_context *ctx, const struct f
 /* sizeof(struct ray_b200_ray) as the library was compiled (32). */
 int64_t ray_b200_ray_size(void);
 
+/* ---- proximity queries: the spheres within a radius of a point, nearest first ----------------------------------------
+ * What is near this point: collision candidates of a sphere (the query is the sphere itself), the neighbours of an agent
+ * within a radius, how many spheres are within a radius (density, "is this spot free"), the closest sphere surface to a
+ * probe point.  A query is a ball (centre c, radius r).  For a sphere with centre p and radius rho (the record layout of
+ * ray_b200_scene_from_arrays), the distance is, in f32, in exactly this order, without contraction (IEEE sqrt):
+ *     dx = p.x - c.x;  dy = p.y - c.y;  dz = p.z - c.z
+ *     d  = sqrtf((dx*dx + dy*dy) + dz*dz) - rho
+ * d is the signed distance from c to the sphere's surface (negative when c is inside it), and the sphere is within the
+ * ball when d <= r; for a ball that is another sphere's (centre, radius) that means the two touch or overlap.
+ *   Answer.  W(i), the set of the scene's spheres within ball i, exactly as a brute force over every sphere computes it.
+ *   Unlike the ray queries this does not follow the reference's culling by stale boxes: the walk reads boxes that contain
+ *   their subtrees (for a scene with stale boxes they are rebuilt first, see below) with a ball-box test that is
+ *   conservative by a proved margin (DESIGN.md §5d), and every sphere it reaches is tested by the rule above.  A sphere
+ *   whose radius is negative or NaN (-0.0 is a valid point sphere), or with a non-finite centre component or radius, is
+ *   never reported.  A ball whose centre is not finite, or whose r is not finite and >= 0, gets the empty answer; it is
+ *   not an error (the host does not read the balls), and the other balls are unaffected.
+ *   Outputs.  counts_dev[i] = |W(i)|, not capped at k (device int32[n], or NULL).  near_dev[i][j], j < min(k, |W(i)|):
+ *   the j-th member of W(i) as struct ray_b200_near, ordered by ascending d, then ascending caller index; d is never -0.0
+ *   (it is x - rho rounded to nearest); the remaining records are d = +inf, sphere = -1 (device struct ray_b200_near[n][k],
+ *   record offsets are 64-bit; NULL is allowed when k == 0, the count-only query).
+ *   Stale boxes.  A scene whose stored boxes are all the union of their children's (ray_b200_prepared_info's stale_nodes
+ *   == 0) is walked as it is stored.  Otherwise each call first builds complete boxes (the refit run to its fixpoint) into
+ *   scratch the context owns, grown on demand and freed with the context: a copy of the records, two memsets and two
+ *   more launches.  The prepared scene is not changed.
+ *   Calls.  Asynchronous on the context's stream; balls_dev is read after the work enqueued there before the call.  One
+ *   launch, plus two for a scene with stale boxes, all counted by ray_b200_context_launch_count; last_plan and
+ *   last_render_ms are unchanged (this is not a warp-queue launch).  A prepared scene or batch may be freed or updated
+ *   while a query that reads it is in flight.  On a RAY_GPUS > 1 context the query runs on device d, which holds the scene.
+ *   Errors (nonzero return, futhark_context_get_error; nothing is written and the context stays usable): n outside
+ *   [0, 2^30], k outside [0, 64], a NULL balls_dev, a NULL near_dev with k > 0, k == 0 with a NULL counts_dev (no output),
+ *   and an invalid prepared scene.  n == 0 does nothing.
+ *   Scene batches.  ray_b200_scene_batch_query_spheres takes m balls per scene: balls_dev struct ray_b200_ball[B][m],
+ *   near_dev struct ray_b200_near[B][m][k], counts_dev int32[B][m], uniform or ragged.  The answer for ball j of scene b is
+ *   bit for bit the single-scene answer on ray_b200_scene_batch_member(b): sphere indexes scene b's own records.  Complete
+ *   boxes are built for the whole batch when any member has stale boxes.  Further errors: a NULL or invalid batch, m < 0
+ *   and B m > 2^30. */
+struct ray_b200_ball {
+  float c[3];   /* centre */
+  float r;      /* radius of the query */
+};              /* 16 bytes, 4-byte aligned */
+struct ray_b200_near {
+  float d;          /* signed distance from the ball's centre to the sphere's surface; +inf for an unused record */
+  int32_t sphere;   /* index into the scene's sphere array as given; -1 for an unused record */
+};                  /* 8 bytes */
+int ray_b200_query_spheres(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                           const struct ray_b200_ball *balls_dev, int64_t n, int32_t k, struct ray_b200_near *near_dev,
+                           int32_t *counts_dev);
+int ray_b200_scene_batch_query_spheres(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                       const struct ray_b200_ball *balls_dev, int64_t m, int32_t k,
+                                       struct ray_b200_near *near_dev, int32_t *counts_dev);
+/* sizeof(struct ray_b200_near) (8) and sizeof(struct ray_b200_ball) (16) as the library was compiled. */
+int64_t ray_b200_near_size(void);
+int64_t ray_b200_ball_size(void);
+
 /* ---- multi-GPU tile sharding (one process per GPU; the gather itself is NCCL, done by the host) -- */
 /* Number of 8x4 tiles rank `rank` of `world` owns for an h x w image, and the padded per-rank count
  * (equal on all ranks, so a plain all_gather / gather works). */

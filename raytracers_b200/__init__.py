@@ -20,7 +20,7 @@ import os
 
 import numpy as np
 
-__all__ = ["Context", "RayError", "Hit", "Ray", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
+__all__ = ["Context", "RayError", "Hit", "Ray", "Ball", "Near", "proximity_k", "proximity_balls", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
            "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays", "SceneBatch", "scene_batch_rows",
            "scene_batch_counts", "scene_batch_cameras", "scene_batch_frames_ok"]
 
@@ -86,6 +86,17 @@ class Ray(C.Structure):
     """struct ray_b200_ray (include/ray_b200.h): a ray with its own interval, 32 bytes; the rows of an [n, 8] float32
     tensor of rays (origin, t_min, direction, t_max)."""
     _fields_ = [("o", C.c_float * 3), ("t_min", C.c_float), ("d", C.c_float * 3), ("t_max", C.c_float)]
+
+
+class Ball(C.Structure):
+    """struct ray_b200_ball (include/ray_b200.h): a proximity query, centre and radius, 16 bytes; the rows of an [n, 4]
+    float32 tensor of balls."""
+    _fields_ = [("c", C.c_float * 3), ("r", C.c_float)]
+
+
+class Near(C.Structure):
+    """struct ray_b200_near (include/ray_b200.h): one sphere within a ball, signed distance d and caller index, 8 bytes."""
+    _fields_ = [("d", C.c_float), ("sphere", C.c_int32)]
 
 
 _libs = {}
@@ -205,6 +216,10 @@ def load_library(variant=""):
         "ray_b200_trace_occluded_ranged": (C.c_int, [vp, vp, vp, i64, vp]),
         "ray_b200_trace_multi_hits_ranged": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
         "ray_b200_ray_size": (i64, []),
+        "ray_b200_query_spheres": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_scene_batch_query_spheres": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_near_size": (i64, []),
+        "ray_b200_ball_size": (i64, []),
         "ray_b200_count_work": (C.c_int, [vp, i64, i64, i32, vp, C.POINTER(WorkCounters)]),
         "ray_b200_ipc_alloc": (C.c_int, [vp, i64, pp, vp]),
         "ray_b200_ipc_free": (C.c_int, [vp, vp]),
@@ -391,6 +406,35 @@ def scene_batch_cameras(cams, B):
 def scene_batch_frames_ok(B, h, w):
     """Whether B frames of h x w fit one launch: h, w in [1, 65536] and B x ceil(h / 4) x ceil(w / 8) <= 2^25 tiles"""
     return 0 < h <= 65536 and 0 < w <= 65536 and B * ((h + 3) // 4) * ((w + 7) // 8) <= 1 << 25
+
+
+def proximity_k(k):
+    """k of a proximity query, an integer in [0, 64] (0: count only); ValueError otherwise"""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 0 <= int(k) <= 64:
+        raise ValueError(f"k must be an integer in [0, 64], got {k!r}")
+    return int(k)
+
+
+def proximity_balls(device, balls, B=None):
+    """The balls of a proximity query: a contiguous float32 CUDA tensor on cuda:device of shape [n, 4] (centre.xyz, r), or
+    with B (a scene batch's) [B, m, 4] with B m <= 2^30.  Returns n, or m for a batch; ValueError for anything else,
+    including spheres' own [n, 7] rows (make balls of them with torch.cat([s[:, :3], s[:, 6:7]], 1))."""
+    import torch
+    dims = 2 if B is None else 3
+    shape = "[n, 4]" if B is None else "[B, m, 4]"
+    if not isinstance(balls, torch.Tensor) or balls.dim() != dims or balls.shape[-1] != 4:
+        got = f"{balls.dtype} {tuple(balls.shape)}" if isinstance(balls, torch.Tensor) else type(balls).__name__
+        raise ValueError(f"balls must be a float32 CUDA tensor of shape {shape} (centre.xyz, r), got {got}")
+    _check_tensor(device, "balls", balls, (torch.float32,), tuple(balls.shape))
+    if B is None:
+        if balls.shape[0] > 1 << 30:
+            raise ValueError(f"a proximity query takes at most 2^30 balls, got {balls.shape[0]}")
+        return int(balls.shape[0])
+    if int(balls.shape[0]) != B:
+        raise ValueError(f"balls must have one row per scene of the batch ({B}), got {int(balls.shape[0])}")
+    if B * int(balls.shape[1]) > 1 << 30:
+        raise ValueError(f"a batch proximity query takes at most 2^30 balls, got {B} x {int(balls.shape[1])}")
+    return int(balls.shape[1])
 
 
 def _camera7(cam7):
@@ -1417,6 +1461,51 @@ class Context:
         self.sync()
         return {"t": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "p": buf[..., 2:5], "normal": buf[..., 5:8],
                 "count": count}
+
+    # -- proximity queries (include/ray_b200.h): the spheres within a radius of each ball, nearest first -----------------
+    def query_spheres_into(self, balls_dev, n, prepared, k, near_dev, counts_dev=None):
+        """The spheres within n balls: balls_dev = device Ball[n] (float[n][4]: centre, r), near_dev = device Near[n][k]
+        (d, sphere) in ascending d, then caller index, (+inf, -1) after the last, or None when k == 0; counts_dev =
+        device int32[n] (or None) = every sphere within, not capped at k.  Exact against a brute force over every sphere.
+        Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_query_spheres(self.handle, prepared.handle, _ptr(balls_dev), int(n), int(k),
+                                                    _ptr(near_dev), _ptr(counts_dev)))
+
+    def query_scene_batch_spheres_into(self, balls_dev, m, batch, k, near_dev, counts_dev=None):
+        """query_spheres_into for every scene of a SceneBatch: balls_dev = device Ball[B][m], near_dev = device
+        Near[B][m][k], counts_dev = device int32[B][m]; sphere indexes the ball's own scene's records.  One launch."""
+        self._check(self.lib.ray_b200_scene_batch_query_spheres(self.handle, batch.handle, _ptr(balls_dev), int(m), int(k),
+                                                                _ptr(near_dev), _ptr(counts_dev)))
+
+    def query_spheres(self, prepared, balls, k=8):
+        """The spheres of a prepared scene within each ball of a [n, 4] float32 CUDA tensor (centre.xyz, r), nearest first:
+        dict(d [n, k] float32, sphere [n, k] int32, count [n] int32), views of one [n, k, 2] buffer of Near records and a
+        count buffer.  Unused records are d = +inf, sphere = -1; count is not capped at k.  Waits for torch's current
+        stream before, and synchronises the context after the query."""
+        import torch
+        n = proximity_balls(self.device, balls)
+        k = proximity_k(k)
+        buf = torch.empty((n, k, 2), dtype=torch.float32, device=balls.device)
+        count = torch.empty((n,), dtype=torch.int32, device=balls.device)
+        torch.cuda.current_stream(balls.device).synchronize()   # the balls may still be in flight on torch's stream
+        self.query_spheres_into(balls.data_ptr(), n, prepared, k, buf.data_ptr() if k else None, count.data_ptr())
+        self.sync()
+        return {"d": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "count": count}
+
+    def query_scene_batch_spheres(self, batch, balls, k=8):
+        """query_spheres for every scene of a SceneBatch: balls is a [B, m, 4] float32 CUDA tensor, m balls per scene.
+        Returns dict(d [B, m, k], sphere [B, m, k] int32, count [B, m] int32), sphere indexing the ball's own scene's
+        records.  Waits for torch's current stream before, and synchronises the context after the query."""
+        import torch
+        B = batch.shape[0]
+        m = proximity_balls(self.device, balls, B)
+        k = proximity_k(k)
+        buf = torch.empty((B, m, k, 2), dtype=torch.float32, device=balls.device)
+        count = torch.empty((B, m), dtype=torch.int32, device=balls.device)
+        torch.cuda.current_stream(balls.device).synchronize()
+        self.query_scene_batch_spheres_into(balls.data_ptr(), m, batch, k, buf.data_ptr() if k else None, count.data_ptr())
+        self.sync()
+        return {"d": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "count": count}
 
     def count_work(self, h, w, prepared, spp=1):
         wc = WorkCounters()

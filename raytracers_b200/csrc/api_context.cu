@@ -211,6 +211,7 @@ void futhark_context_free(struct futhark_context *ctx) {
   }
   for (auto &b : ctx->pinned_cache) { cudaEventDestroy(b.last_use); cudaFreeHost(b.ptr); }
   if (ctx->ok) free_wavefront(ctx);
+  if (ctx->ok) free_proximity_scratch(ctx);
   for (auto &L : ctx->lanes) {
     if (L.sample_buf) cudaFree(L.sample_buf);
     if (L.tile_order_block) cudaFree(L.tile_order_block);
@@ -284,6 +285,7 @@ int futhark_context_clear_caches(struct futhark_context *ctx) {
     L.tile_order_block = nullptr; L.tile_order_bytes = 0;
   }
   free_wavefront(ctx);
+  free_proximity_scratch(ctx);
   for (auto &b : ctx->pinned_cache) { cudaEventDestroy(b.last_use); cudaFreeHost(b.ptr); }
   ctx->pinned_cache.clear();
   if (cudaDeviceGetDefaultMemPool(&pool, ctx->cfg.device) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);

@@ -95,6 +95,12 @@ struct futhark_context {
   bool pipeline = false;                // ray_b200_context_set_pipeline: batches do not join lane 1 back
   uint32_t lane_seq = 0;                // pipelined submission: frames alternate lanes across calls
   cudaStream_t reclaim = nullptr;       // scene memory is freed here, ordered after its last use on either lane
+  // Proximity queries of scenes with stale boxes (api_proximity.cu): complete-box records and the refit's scratch, one
+  // grow-only allocation used on lane 0 only; `prox_done` is recorded behind its last use, so that a call on another
+  // stream (ray_b200_context_set_stream) waits for it before overwriting it.
+  unsigned char *prox_block = nullptr;
+  size_t prox_bytes = 0;
+  cudaEvent_t prox_done = nullptr;
   bool profiling_paused = false;
   int64_t renders = 0;
   bool ok = false;
@@ -263,5 +269,7 @@ int prepare_any(futhark_context *ctx, futhark_opaque_prepared_scene *p);
 // the 32-byte read-back.  The tree is built into a new block before p's old one is released, so a failed build leaves
 // p as it was.  `drop_order`: the scene changes, so its learned claim order is dropped with the old block.
 int build_on_device(futhark_context *ctx, futhark_opaque_prepared_scene *p, const float *d_spheres, int64_t n, bool drop_order);
+// api_proximity.cu: drops the proximity queries' complete-box scratch (context free, futhark_context_clear_caches)
+void free_proximity_scratch(futhark_context *ctx);
 
 }  // namespace rayb200_api
