@@ -634,6 +634,45 @@ int ray_b200_scene_batch_query_spheres(struct futhark_context *ctx, const struct
 int64_t ray_b200_near_size(void);
 int64_t ray_b200_ball_size(void);
 
+/* ---- nearest-sphere queries: the k nearest spheres to a point, with no radius to guess -----------------------------------
+ * Which k spheres are nearest to this point, however far away: the signed distance of the scene at a probe point (sphere
+ * tracing, collision margins, training data for distance fields), the k-nearest-neighbour graph of the spheres
+ * themselves, the closest object to a cursor.  A query is a struct ray_b200_ball (c, r) whose r is an upper limit on d,
+ * r = +inf for no limit.  d is the proximity queries' distance above, in f32 in the same operation order, and the same
+ * spheres are reportable (finite centre and radius, rho >= 0, -0.0 included).
+ *   Balls.  A ball is valid when its centre is finite and r >= 0, r = +inf included; a ball with a non-finite centre, or
+ *   whose r is NaN or negative, gets the empty answer.  That is not an error, and the other balls are unaffected.  This
+ *   differs from ray_b200_query_spheres only in accepting r = +inf (query_spheres still gives such a ball the empty answer).
+ *   Answer.  W(i), the reportable spheres with d <= r_i.  near_dev[i][j] for j < min(k, |W(i)|) is the j-th member of
+ *   W(i) in ascending d, then ascending caller index (query_spheres' order); the remaining records are d = +inf,
+ *   sphere = -1 (device struct ray_b200_near[n][k], record offsets are 64-bit).  With r = +inf a reportable sphere's d may
+ *   overflow to +inf: it is still a record, with sphere >= 0, so `sphere` tells a record from padding.  There is no count:
+ *   ray_b200_query_spheres counts the spheres within a bounded r.
+ *   Identities.  For a finite r the records are bit for bit ray_b200_query_spheres(ball, k)'s.  At k = 1, record 0's d is
+ *   the signed distance at c of the union of the scene's reportable spheres (min over them of |p - c| - rho), or +inf
+ *   when there are none.
+ *   Neighbour graph.  The k nearest other spheres of sphere i: query its own centre with k + 1 (r = +inf, or a limit) and
+ *   drop the record with sphere == i, or the last record when i is absent; that is exactly the first k of W minus {i},
+ *   whatever coincident copies do to the order.  As k is at most 64, this gives at most 63 neighbours.
+ *   Stale boxes, calls.  As for ray_b200_query_spheres: a scene with stale boxes is walked over complete boxes built into
+ *   the context's scratch first (the prepared scene is not changed); asynchronous on the context's stream, balls_dev read
+ *   after the work enqueued there before the call; one launch, plus two for a scene with stale boxes, all counted by
+ *   ray_b200_context_launch_count; last_plan and last_render_ms are unchanged.  A prepared scene or batch may be freed or
+ *   updated while a query that reads it is in flight.  On a RAY_GPUS > 1 context the query runs on device d.
+ *   Errors (nonzero return, futhark_context_get_error; nothing is written and the context stays usable): n outside
+ *   [0, 2^30], k outside [1, 64], a NULL balls_dev or near_dev with n > 0, an invalid prepared scene.  n == 0 does
+ *   nothing.
+ *   Scene batches.  ray_b200_scene_batch_query_nearest takes m balls per scene: balls_dev struct ray_b200_ball[B][m],
+ *   near_dev struct ray_b200_near[B][m][k], uniform or ragged; ball j of scene b gets the single-scene answer on
+ *   ray_b200_scene_batch_member(b), sphere indexing scene b's own records.  Further errors: a NULL or invalid batch, m < 0
+ *   and B m > 2^30. */
+int ray_b200_query_nearest(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                           const struct ray_b200_ball *balls_dev, int64_t n, int32_t k,
+                           struct ray_b200_near *near_dev);
+int ray_b200_scene_batch_query_nearest(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                       const struct ray_b200_ball *balls_dev, int64_t m, int32_t k,
+                                       struct ray_b200_near *near_dev);
+
 /* ---- multi-GPU tile sharding (one process per GPU; the gather itself is NCCL, done by the host) -- */
 /* Number of 8x4 tiles rank `rank` of `world` owns for an h x w image, and the padded per-rank count
  * (equal on all ranks, so a plain all_gather / gather works). */

@@ -20,7 +20,7 @@ import os
 
 import numpy as np
 
-__all__ = ["Context", "RayError", "Hit", "Ray", "Ball", "Near", "proximity_k", "proximity_balls", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
+__all__ = ["Context", "RayError", "Hit", "Ray", "Ball", "Near", "proximity_k", "proximity_balls", "nearest_k", "nearest_points", "Plan", "QUERIES", "lib_path", "load_library", "KERNELS", "declared_symbols", "host_scene",
            "host_camera", "host_lbvh", "host_sample_offsets", "camera_table", "camera_rays", "SceneBatch", "scene_batch_rows",
            "scene_batch_counts", "scene_batch_cameras", "scene_batch_frames_ok"]
 
@@ -218,6 +218,8 @@ def load_library(variant=""):
         "ray_b200_ray_size": (i64, []),
         "ray_b200_query_spheres": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
         "ray_b200_scene_batch_query_spheres": (C.c_int, [vp, vp, vp, i64, i32, vp, vp]),
+        "ray_b200_query_nearest": (C.c_int, [vp, vp, vp, i64, i32, vp]),
+        "ray_b200_scene_batch_query_nearest": (C.c_int, [vp, vp, vp, i64, i32, vp]),
         "ray_b200_near_size": (i64, []),
         "ray_b200_ball_size": (i64, []),
         "ray_b200_count_work": (C.c_int, [vp, i64, i64, i32, vp, C.POINTER(WorkCounters)]),
@@ -435,6 +437,37 @@ def proximity_balls(device, balls, B=None):
     if B * int(balls.shape[1]) > 1 << 30:
         raise ValueError(f"a batch proximity query takes at most 2^30 balls, got {B} x {int(balls.shape[1])}")
     return int(balls.shape[1])
+
+
+def nearest_k(k):
+    """k of a nearest-sphere query, an integer in [1, 64]; ValueError otherwise"""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= int(k) <= 64:
+        raise ValueError(f"k must be an integer in [1, 64], got {k!r}")
+    return int(k)
+
+
+def nearest_points(device, points, B=None):
+    """The balls of a nearest-sphere query from points, a contiguous float32 CUDA tensor on cuda:device of shape [n, 3]
+    (centres, no limit on the distance) or [n, 4] (centre.xyz, r), or with B (a scene batch's) [B, m, 3 | 4], B m <= 2^30.
+    Returns (n or m, balls): balls is points itself when it has 4 columns, else a new [.., 4] tensor with r = +inf.
+    ValueError for anything else."""
+    import torch
+    dims = 2 if B is None else 3
+    shape = "[n, 3] or [n, 4]" if B is None else "[B, m, 3] or [B, m, 4]"
+    if not isinstance(points, torch.Tensor) or points.dim() != dims or points.shape[-1] not in (3, 4):
+        got = f"{points.dtype} {tuple(points.shape)}" if isinstance(points, torch.Tensor) else type(points).__name__
+        raise ValueError(f"points must be a float32 CUDA tensor of shape {shape} (centre.xyz[, r]), got {got}")
+    _check_tensor(device, "points", points, (torch.float32,), tuple(points.shape))
+    count = int(points.shape[0]) if B is None else int(points.shape[1])
+    if B is None and count > 1 << 30:
+        raise ValueError(f"a nearest-sphere query takes at most 2^30 points, got {count}")
+    if B is not None and int(points.shape[0]) != B:
+        raise ValueError(f"points must have one row per scene of the batch ({B}), got {int(points.shape[0])}")
+    if B is not None and B * count > 1 << 30:
+        raise ValueError(f"a batch nearest-sphere query takes at most 2^30 points, got {B} x {count}")
+    if points.shape[-1] == 4:
+        return count, points
+    return count, torch.cat([points, torch.full_like(points[..., :1], float("inf"))], -1)
 
 
 def _camera7(cam7):
@@ -1506,6 +1539,50 @@ class Context:
         self.query_scene_batch_spheres_into(balls.data_ptr(), m, batch, k, buf.data_ptr() if k else None, count.data_ptr())
         self.sync()
         return {"d": buf[..., 0], "sphere": buf[..., 1].view(torch.int32), "count": count}
+
+    # -- nearest-sphere queries (include/ray_b200.h): the k nearest spheres to each point, with or without a limit -------
+    def query_nearest_into(self, balls_dev, n, prepared, k, near_dev):
+        """The k nearest spheres of n balls: balls_dev = device Ball[n] (float[n][4]: centre, r; r = +inf for no limit),
+        near_dev = device Near[n][k] (d, sphere) in ascending d, then caller index, of the spheres with d <= r, (+inf, -1)
+        after the last.  Exact against a brute force over every sphere.  Asynchronous on the context's stream."""
+        self._check(self.lib.ray_b200_query_nearest(self.handle, prepared.handle, _ptr(balls_dev), int(n), int(k),
+                                                    _ptr(near_dev)))
+
+    def query_scene_batch_nearest_into(self, balls_dev, m, batch, k, near_dev):
+        """query_nearest_into for every scene of a SceneBatch: balls_dev = device Ball[B][m], near_dev = device
+        Near[B][m][k]; sphere indexes the ball's own scene's records.  One launch."""
+        self._check(self.lib.ray_b200_scene_batch_query_nearest(self.handle, batch.handle, _ptr(balls_dev), int(m), int(k),
+                                                                _ptr(near_dev)))
+
+    def query_nearest(self, prepared, points, k=1):
+        """The k nearest spheres of a prepared scene to each point of a [n, 3] float32 CUDA tensor (no limit on the
+        distance), or to each ball of a [n, 4] one (centre.xyz, r: only spheres with d <= r): dict(d [n, k] float32,
+        sphere [n, k] int32), nearest first, views of one [n, k, 2] buffer of Near records.  Unused records are d = +inf,
+        sphere = -1; with no limit a record can have d = +inf (an overflow) and a sphere >= 0.  query_nearest(p, pts)["d"][:, 0]
+        is the signed distance of the union of the scene's spheres at each point.  Waits for torch's current stream
+        before, and synchronises the context after the query."""
+        import torch
+        n, balls = nearest_points(self.device, points)
+        k = nearest_k(k)
+        buf = torch.empty((n, k, 2), dtype=torch.float32, device=balls.device)
+        torch.cuda.current_stream(balls.device).synchronize()   # the balls may still be in flight on torch's stream
+        self.query_nearest_into(balls.data_ptr(), n, prepared, k, buf.data_ptr())
+        self.sync()
+        return {"d": buf[..., 0], "sphere": buf[..., 1].view(torch.int32)}
+
+    def query_scene_batch_nearest(self, batch, points, k=1):
+        """query_nearest for every scene of a SceneBatch: points is a [B, m, 3] or [B, m, 4] float32 CUDA tensor, m per
+        scene.  Returns dict(d [B, m, k], sphere [B, m, k] int32), sphere indexing the point's own scene's records.  Waits
+        for torch's current stream before, and synchronises the context after the query."""
+        import torch
+        B = batch.shape[0]
+        m, balls = nearest_points(self.device, points, B)
+        k = nearest_k(k)
+        buf = torch.empty((B, m, k, 2), dtype=torch.float32, device=balls.device)
+        torch.cuda.current_stream(balls.device).synchronize()
+        self.query_scene_batch_nearest_into(balls.data_ptr(), m, batch, k, buf.data_ptr())
+        self.sync()
+        return {"d": buf[..., 0], "sphere": buf[..., 1].view(torch.int32)}
 
     def count_work(self, h, w, prepared, spp=1):
         wc = WorkCounters()

@@ -1,6 +1,7 @@
 // C ABI, part 6: proximity queries (include/ray_b200.h "proximity queries") - the spheres within a radius of each of the
-// caller's balls, nearest first, for a prepared scene or every scene of a scene batch.  Validation, the choice between
-// the stored records and complete boxes, and the launch; the kernels are in proximity_kernels.cu.
+// caller's balls, nearest first - and nearest-sphere queries ("nearest-sphere queries") - the k nearest spheres within a
+// radius that may be +inf - for a prepared scene or every scene of a scene batch.  Validation, the choice between the
+// stored records and complete boxes, and the launch, shared by both queries; the kernels are in proximity_kernels.cu.
 #include "api_internal.h"
 
 #include <cstddef>
@@ -28,10 +29,13 @@ namespace {
 
 // Validates and enqueues one query of p's records on the context's stream (lane 0); the caller holds ctx->mu.  `stale`:
 // some box of p is not the union of its children's, so the walk reads complete boxes built into the context's scratch
-// first.  Q's balls, k and outputs are the caller's; a scene batch's query also sets Q's scene fields.
-int enqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool stale, ProximityQuery Q, const char *what) {
+// first.  Q's balls, k and outputs are the caller's; a scene batch's query also sets Q's scene fields.  `nearest`: the
+// nearest-sphere kernel (k in [1, 64], no counts) instead of the proximity kernel.
+int enqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool stale, ProximityQuery Q, bool nearest,
+            const char *what) {
+  const int k_min = nearest ? 1 : 0;
   if (Q.n < 0 || Q.n > ((int64_t)1 << 30)) { set_error(ctx, "%s: n = %lld is outside [0, 2^30]", what, (long long)Q.n); return 1; }
-  if (Q.k < 0 || Q.k > 64) { set_error(ctx, "%s: k = %d is outside [0, 64]", what, Q.k); return 1; }
+  if (Q.k < k_min || Q.k > 64) { set_error(ctx, "%s: k = %d is outside [%d, 64]", what, Q.k, k_min); return 1; }
   if (Q.n == 0) return 0;
   if (!Q.balls) { set_error(ctx, "%s: NULL balls buffer", what); return 1; }
   if (Q.k > 0 && !Q.near) { set_error(ctx, "%s: NULL near buffer with k = %d", what, Q.k); return 1; }
@@ -60,9 +64,24 @@ int enqueue(futhark_context *ctx, const futhark_opaque_prepared_scene *p, bool s
                                        &ctx->launches));
     Q.nodes = recs;
   }
-  CUDA_TRY(ctx, launch_proximity(Q, L.stream, &ctx->launches));
+  CUDA_TRY(ctx, nearest ? launch_nearest(Q, L.stream, &ctx->launches) : launch_proximity(Q, L.stream, &ctx->launches));
   if (stale) CUDA_TRY(ctx, cudaEventRecord(ctx->prox_done, L.stream));
   return record_scene_use(ctx, p, 0);
+}
+
+// A query of every scene of batch b, m balls per scene, as enqueue's
+int enqueue_batch(futhark_context *ctx, const ray_b200_scene_batch *b, ProximityQuery Q, int64_t m, bool nearest,
+                  const char *what) {
+  if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
+  const int32_t B = b->scene.scenes;
+  if (m < 0) { set_error(ctx, "%s: m = %lld balls per scene is negative", what, (long long)m); return 1; }
+  if (m > ((int64_t)1 << 30) / B) { set_error(ctx, "%s: %d scenes of %lld balls exceed 2^30 balls", what, B, (long long)m); return 1; }
+  bool stale = false;
+  for (const BvhBuildResult &r : b->results) stale = stale || r.stale_nodes > 0;
+  Q.n = (int64_t)B * m;
+  Q.scene_off = b->scene.dev.scene_off;
+  Q.balls_per_scene = m;
+  return enqueue(ctx, &b->scene, stale, Q, nearest, what);
 }
 
 }  // namespace
@@ -80,30 +99,44 @@ int ray_b200_query_spheres(struct futhark_context *ctx, const struct futhark_opa
   Q.k = k;
   Q.near = reinterpret_cast<float *>(near_dev);
   Q.counts = counts_dev;
-  return enqueue(ctx, p, p && p->stale_nodes > 0, Q, "query_spheres");
+  return enqueue(ctx, p, p && p->stale_nodes > 0, Q, false, "query_spheres");
 }
 
 int ray_b200_scene_batch_query_spheres(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
                                        const struct ray_b200_ball *balls_dev, int64_t m, int32_t k,
                                        struct ray_b200_near *near_dev, int32_t *counts_dev) {
-  const char *what = "scene_batch_query_spheres";
   if (bad_ctx(ctx)) return 1;
   std::lock_guard<std::mutex> g(ctx->mu);
-  if (!b || !b->scene.dev.block) { set_error(ctx, "%s: invalid scene batch", what); return 1; }
-  const int32_t B = b->scene.scenes;
-  if (m < 0) { set_error(ctx, "%s: m = %lld balls per scene is negative", what, (long long)m); return 1; }
-  if (m > ((int64_t)1 << 30) / B) { set_error(ctx, "%s: %d scenes of %lld balls exceed 2^30 balls", what, B, (long long)m); return 1; }
-  bool stale = false;
-  for (const BvhBuildResult &r : b->results) stale = stale || r.stale_nodes > 0;
   ProximityQuery Q;
   Q.balls = reinterpret_cast<const float *>(balls_dev);
-  Q.n = (int64_t)B * m;
   Q.k = k;
   Q.near = reinterpret_cast<float *>(near_dev);
   Q.counts = counts_dev;
-  Q.scene_off = b->scene.dev.scene_off;
-  Q.balls_per_scene = m;
-  return enqueue(ctx, &b->scene, stale, Q, what);
+  return enqueue_batch(ctx, b, Q, m, false, "scene_batch_query_spheres");
+}
+
+int ray_b200_query_nearest(struct futhark_context *ctx, const struct futhark_opaque_prepared_scene *p,
+                           const struct ray_b200_ball *balls_dev, int64_t n, int32_t k, struct ray_b200_near *near_dev) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  ProximityQuery Q;
+  Q.balls = reinterpret_cast<const float *>(balls_dev);
+  Q.n = n;
+  Q.k = k;
+  Q.near = reinterpret_cast<float *>(near_dev);
+  return enqueue(ctx, p, p && p->stale_nodes > 0, Q, true, "query_nearest");
+}
+
+int ray_b200_scene_batch_query_nearest(struct futhark_context *ctx, const struct ray_b200_scene_batch *b,
+                                       const struct ray_b200_ball *balls_dev, int64_t m, int32_t k,
+                                       struct ray_b200_near *near_dev) {
+  if (bad_ctx(ctx)) return 1;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  ProximityQuery Q;
+  Q.balls = reinterpret_cast<const float *>(balls_dev);
+  Q.k = k;
+  Q.near = reinterpret_cast<float *>(near_dev);
+  return enqueue_batch(ctx, b, Q, m, true, "scene_batch_query_nearest");
 }
 
 int64_t ray_b200_near_size(void) { return (int64_t)sizeof(struct ray_b200_near); }

@@ -16,9 +16,9 @@ struct ProximityQuery {
   const int32_t *perm = nullptr;     // Morton-sorted leaf -> caller index (global in a scene batch)
   const float *balls = nullptr;      // [n][4]: centre.xyz, r (4-byte aligned)
   int64_t n = 0;
-  int32_t k = 0;                     // records per ball, [0, 64]
+  int32_t k = 0;                     // records per ball, [0, 64] ([1, 64] for the nearest-sphere kernel)
   float *near = nullptr;             // [n][k] struct ray_b200_near (d, sphere); NULL when k == 0
-  int32_t *counts = nullptr;         // [n] or NULL
+  int32_t *counts = nullptr;         // [n] or NULL (always NULL for the nearest-sphere kernel)
   // scene batch: ball i belongs to scene i / balls_per_scene, whose root record is scene_off[b] - b and whose spheres
   // are numbered from scene_off[b]; NULL for one scene (root record 0, spheres from 0)
   const int32_t *scene_off = nullptr;
@@ -36,5 +36,8 @@ cudaError_t refit_complete_boxes(const float4 *nodes, const float4 *geom, int64_
                                  void *scratch, cudaStream_t stream, int64_t *launches);
 // One launch of the query kernel on `stream`, with the register bucket that holds Q.k records
 cudaError_t launch_proximity(const ProximityQuery &Q, cudaStream_t stream, int64_t *launches);
+// One launch of the nearest-sphere kernel on `stream` (include/ray_b200.h "nearest-sphere queries"): the Q.k nearest
+// spheres within each ball, r = +inf allowed, Q.k in [1, 64]; Q.counts is not written
+cudaError_t launch_nearest(const ProximityQuery &Q, cudaStream_t stream, int64_t *launches);
 
 }  // namespace rayb200

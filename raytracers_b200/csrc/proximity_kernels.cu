@@ -69,27 +69,44 @@ __global__ void prox_refit_kernel(float4 *__restrict__ out, const float4 *__rest
 
 // ---------------------------------------------------------------------------------------------- the query
 
-// Whether a box may hold a sphere within the ball (c, r): a lower bound of the squared distance from c to the box,
-// rounded down, against an upper bound of (r + 2^-20 (r + M) + FLT_MIN)^2, rounded up, where M is the box's largest
-// coordinate magnitude.  DESIGN.md §5d proves that every sphere with d <= r passes every complete box above it.  NaN
-// coordinates pass (fmaxf drops them, and a NaN bound compares false); a box with an infinite coordinate gets an infinite
-// bound unless c is infinitely far from it.
-__device__ __forceinline__ bool ball_meets_box(float cx, float cy, float cz, float r, const float4 lo, const float4 hi) {
+// The ball-box test, in two parts that both query kernels use: the bound G, a lower bound of the squared distance from c
+// to the box rounded down, and the threshold, an upper bound of (r + 2^-20 (r + M) + FLT_MIN)^2 rounded up, where M is
+// the box's largest coordinate magnitude.  A box may hold a sphere within the ball (c, r) when !(G > threshold).
+// DESIGN.md §5d proves that every sphere with d <= r passes every complete box above it.  NaN coordinates pass (fmaxf
+// drops them, and a NaN bound compares false); a box with an infinite coordinate gets an infinite threshold unless c is
+// infinitely far from it, and r = +inf gives an infinite threshold.
+__device__ __forceinline__ float box_gap2(float cx, float cy, float cz, const float4 lo, const float4 hi) {
   const float gx = fmaxf(fmaxf(__fsub_rd(lo.x, cx), __fsub_rd(cx, hi.x)), 0.0f);
   const float gy = fmaxf(fmaxf(__fsub_rd(lo.y, cy), __fsub_rd(cy, hi.y)), 0.0f);
   const float gz = fmaxf(fmaxf(__fsub_rd(lo.z, cz), __fsub_rd(cz, hi.z)), 0.0f);
-  const float g2 = __fadd_rd(__fadd_rd(__fmul_rd(gx, gx), __fmul_rd(gy, gy)), __fmul_rd(gz, gz));
-  const float m = fmaxf(fmaxf(fmaxf(fabsf(lo.x), fabsf(lo.y)), fmaxf(fabsf(lo.z), fabsf(hi.x))), fmaxf(fabsf(hi.y), fabsf(hi.z)));
-  const float s = __fadd_ru(__fadd_ru(r, __fmul_ru(0x1p-20f, __fadd_ru(r, m))), FLT_MIN);
-  return !(g2 > __fmul_ru(s, s));
+  return __fadd_rd(__fadd_rd(__fmul_rd(gx, gx), __fmul_rd(gy, gy)), __fmul_rd(gz, gz));
 }
 
-// (d, s) before (d2, s2): ascending distance, then ascending caller index
-__device__ __forceinline__ bool before(float d, int s, float d2, int s2) { return d < d2 || (d == d2 && s < s2); }
+__device__ __forceinline__ float box_mag(const float4 lo, const float4 hi) {
+  return fmaxf(fmaxf(fmaxf(fabsf(lo.x), fabsf(lo.y)), fmaxf(fabsf(lo.z), fabsf(hi.x))), fmaxf(fabsf(hi.y), fabsf(hi.z)));
+}
+
+__device__ __forceinline__ float ball_reach2(float r, float m) {
+  const float s = __fadd_ru(__fadd_ru(r, __fmul_ru(0x1p-20f, __fadd_ru(r, m))), FLT_MIN);
+  return __fmul_ru(s, s);
+}
+
+__device__ __forceinline__ bool ball_meets_box(float cx, float cy, float cz, float r, const float4 lo, const float4 hi) {
+  const float g2 = box_gap2(cx, cy, cz, lo, hi);
+  return !(g2 > ball_reach2(r, box_mag(lo, hi)));
+}
+
+// (d, s) before (d2, s2): ascending distance, then ascending caller index.  kInfD: records may have d = +inf (a ball
+// with no limit reports spheres whose d overflows), so the index compares unsigned and the unused record (+inf, -1)
+// stays after every record.
+template <bool kInfD = false>
+__device__ __forceinline__ bool before(float d, int s, float d2, int s2) {
+  return d < d2 || (d == d2 && (kInfD ? (unsigned)s < (unsigned)s2 : s < s2));
+}
 
 // The k best records of one ball.  KB = 0: none (count only); 1 and 8: in registers (the first k of KB); 64: in the
-// ball's own output row, kept sorted there.
-template <int KB>
+// ball's own output row, kept sorted there.  kth(): the k-th record once k are held (the nearest-sphere query's d_k).
+template <int KB, bool kInfD = false>
 struct Best {
   float d[KB];
   int s[KB];
@@ -97,10 +114,17 @@ struct Best {
 #pragma unroll
     for (int j = 0; j < KB; j++) { d[j] = INFINITY; s[j] = -1; }
   }
+  __device__ __forceinline__ void kth(float2 *, int k, int, float &dk, int &sk) const {
+    // the last slot below k wins: predicated moves (an equality select becomes an indexed load from local memory)
+#pragma unroll
+    for (int j = 0; j < KB; j++) {
+      if (j < k) { dk = d[j]; sk = s[j]; }
+    }
+  }
   __device__ __forceinline__ void insert(float2 *, int, int, float cd, int cs) {
 #pragma unroll
     for (int j = 0; j < KB; j++) {
-      if (before(cd, cs, d[j], s[j])) {
+      if (before<kInfD>(cd, cs, d[j], s[j])) {
         const float td = d[j]; const int ts = s[j];
         d[j] = cd; s[j] = cs; cd = td; cs = ts;
       }
@@ -125,13 +149,18 @@ struct Best<0> {
   __device__ __forceinline__ void store(float2 *, int) {}
 };
 
-template <>
-struct Best<64> {
+// The row's records are compared with each other only, never with an unused one, so one order serves both queries
+template <bool kInfD>
+struct Best<64, kInfD> {
   // the row is 4-byte aligned (struct ray_b200_near): word loads and stores
   __device__ __forceinline__ static float &dist(float2 *row, int j) { return reinterpret_cast<float *>(row)[2 * j]; }
   __device__ __forceinline__ static float &idx(float2 *row, int j) { return reinterpret_cast<float *>(row)[2 * j + 1]; }
   __device__ __forceinline__ void init(float2 *row, int k) {
     for (int j = 0; j < k; j++) { dist(row, j) = INFINITY; idx(row, j) = __int_as_float(-1); }
+  }
+  // `have`: the records held, this one included
+  __device__ __forceinline__ void kth(float2 *row, int k, int have, float &dk, int &sk) const {
+    if (have >= k) { dk = dist(row, k - 1); sk = __float_as_int(idx(row, k - 1)); }
   }
   // `have`: the records so far (the count before this sphere), of which min(have, k) are in the row
   __device__ __forceinline__ void insert(float2 *row, int k, int have, float cd, int cs) {
@@ -208,6 +237,90 @@ __global__ void __launch_bounds__(kThreads) prox_query_kernel(const ProximityQue
   if (Q.counts) Q.counts[i] = count;
 }
 
+// The k nearest spheres within a ball whose r may be +inf (include/ray_b200.h "nearest-sphere queries", DESIGN.md §5e).
+// The walk prunes with R = max(0, min(r, d_k)), d_k the k-th best d so far (+inf while fewer than k are held): R only
+// shrinks, every final record has d <= R throughout, so by §5d it passes every complete box above it.  Each record's
+// two children are ordered by their bounds G, the nearer one is walked first and the other is pushed with G and its box's
+// magnitude M, so that a pop tests it again against the R of that moment and drops it without loading its record.
+template <int KB>
+__global__ void __launch_bounds__(kThreads) prox_nearest_kernel(const ProximityQuery Q) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= Q.n) return;
+  const float *ball = Q.balls + 4 * i;
+  const float cx = __ldg(ball), cy = __ldg(ball + 1), cz = __ldg(ball + 2), r = __ldg(ball + 3);
+  int root = 0, base = 0;
+  if (Q.scene_off) {
+    const int b = (int)(i / Q.balls_per_scene);
+    base = __ldg(Q.scene_off + b);
+    root = base - b;
+  }
+  const int k = Q.k;
+  float2 *row = reinterpret_cast<float2 *>(Q.near) + i * k;
+  Best<KB, true> best;
+  best.init(row, k);
+  // an invalid ball gets the empty answer: r = +inf is valid, r NaN or negative is not (include/ray_b200.h)
+  if (isfinite(cx) && isfinite(cy) && isfinite(cz) && r >= 0.0f) {
+    float dk = INFINITY, R = r;     // d_k and R; the k-th record's caller index is sk
+    int sk = -1, have = 0;
+    int stack[kStackSize];
+    float stack_g[kStackSize], stack_m[kStackSize];
+    int sp = 0, cur = root;
+    for (;;) {
+      const float4 *rec = Q.nodes + 4 * (size_t)cur;
+      const float4 q0 = __ldg(rec), q1 = __ldg(rec + 1), q2 = __ldg(rec + 2), q3 = __ldg(rec + 3);
+      const int lptr = __float_as_int(q0.w), rptr = __float_as_int(q1.w);
+#pragma unroll
+      for (int side = 0; side < 2; side++) {
+        const int ptr = side == 0 ? lptr : rptr;
+        if (ptr >= 0) continue;
+        const float4 g = __ldg(Q.geom + ~ptr);
+        if (!(isfinite(g.x) && isfinite(g.y) && isfinite(g.z) && isfinite(g.w) && g.w >= 0.0f)) continue;
+        const float dx = __fsub_rn(g.x, cx), dy = __fsub_rn(g.y, cy), dz = __fsub_rn(g.z, cz);
+        const float d = __fsub_rn(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz))), g.w);
+        // d <= R is needed to be within r and before the k-th record; the caller index breaks a tie at d_k
+        if (!(d <= R)) continue;
+        const int s = __ldg(Q.perm + ~ptr) - base;
+        if (!before<true>(d, s, dk, sk)) continue;
+        best.insert(row, k, have, d, s);
+        have++;
+        best.kth(row, k, have, dk, sk);
+        R = fmaxf(fminf(r, dk), 0.0f);
+      }
+      float gl = 0.0f, gr = 0.0f, ml = 0.0f, mr = 0.0f;
+      bool tl = false, tr = false;
+      if (lptr >= 0) {
+        gl = box_gap2(cx, cy, cz, q0, q1);
+        ml = box_mag(q0, q1);
+        tl = !(gl > ball_reach2(R, ml));
+      }
+      if (rptr >= 0) {
+        gr = box_gap2(cx, cy, cz, q2, q3);
+        mr = box_mag(q2, q3);
+        tr = !(gr > ball_reach2(R, mr));
+      }
+      if (tl && tr) {
+        const bool left_first = !(gr < gl);   // ties (and a NaN bound) go left first
+        stack[sp] = left_first ? rptr : lptr;
+        stack_g[sp] = left_first ? gr : gl;
+        stack_m[sp] = left_first ? mr : ml;
+        sp++;
+        cur = left_first ? lptr : rptr;
+      } else if (tl || tr) {
+        cur = tl ? lptr : rptr;
+      } else {
+        // pop the next entry that still passes against the current R
+        cur = -1;
+        while (sp > 0) {
+          sp--;
+          if (!(stack_g[sp] > ball_reach2(R, stack_m[sp]))) { cur = stack[sp]; break; }
+        }
+        if (cur < 0) break;
+      }
+    }
+  }
+  best.store(row, k);
+}
+
 inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -242,6 +355,15 @@ cudaError_t launch_proximity(const ProximityQuery &Q, cudaStream_t stream, int64
   else if (Q.k == 1) prox_query_kernel<1><<<g, kThreads, 0, stream>>>(Q);
   else if (Q.k <= 8) prox_query_kernel<8><<<g, kThreads, 0, stream>>>(Q);
   else prox_query_kernel<64><<<g, kThreads, 0, stream>>>(Q);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_nearest(const ProximityQuery &Q, cudaStream_t stream, int64_t *launches) {
+  const unsigned g = blocks_for(Q.n);
+  if (Q.k == 1) prox_nearest_kernel<1><<<g, kThreads, 0, stream>>>(Q);
+  else if (Q.k <= 8) prox_nearest_kernel<8><<<g, kThreads, 0, stream>>>(Q);
+  else prox_nearest_kernel<64><<<g, kThreads, 0, stream>>>(Q);
   if (launches) *launches += 1;
   return cudaGetLastError();
 }
